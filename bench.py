@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- update-iteration throughput of the DPVO hot path on B200.
+"""bench.py -- update-iteration throughput of the DPVO hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config default|fast]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config default|fast] [--dump-outputs DIR]
 
 One "step" = one DPVO.update() (dpvo/dpvo.py:328-360): reprojection, 2-level patch correlation,
 update operator, 2 Gauss-Newton BA iterations, on the steady-state synthetic patch graph of
@@ -13,14 +13,18 @@ Prints ONE JSON line (rank 0).  `value` is device-resident throughput, `e2e` the
 public API with the new frame coming from pinned host memory and poses/depths read back to the host.
 `roofline` is for the dominant kernel CLASS of the step, the update operator's dense layers
 (linear_f16_kernel, 15 launches): algorithmic FLOPs (SURVEY 8(d): 5.396 MFLOP/edge) / the summed CUDA-event
-time of those launches in the eager pass, vs the measured sustained dense tensor peak in MEASURED_PEAKS.json.
+time of those launches in the eager pass, vs the dense 16-bit tensor peak of the H100 SXM data sheet (or the
+measured sustained peak in MEASURED_PEAKS.json when present).
 `roofline_corr` keeps the correlation kernel's numbers: algorithmic bytes/time (served mostly by L2, so NOT an
-HBM fraction) next to the DRAM and L2 bytes of one launch from the committed ncu capture.
+HBM fraction).
 `reference_cuda` = the reference's OWN CUDA pipeline for the same update on the same state, timed in the same
 run (oracle/ref_pipeline.py:RefCudaStep: ref_cuda_corr x2 + stack, torch Update under autocast, ref_cuda_ba
 from oracle/_ref) -- the same-box denominator of north_star's ">= 5x the reference CUDA build".
 `--impl reference` times the reference's CPU path (oracle port of F.grid_sample correlation + PyTorch
 Update + dpvo/ba.py BA, BASELINE.json configs[0] style) on a bounded sample of the same workload.
+`--dump-outputs DIR` writes what the timed loop computed in its last step as DIR/<name>.npy (target, weight, the
+updated poses and patches, a fixed seeded sample of the recurrent state's rows and their indices); the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -44,13 +48,16 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        tf = d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1416.5))
-        return d.get("hbm_gbs", 6650.0), tf, "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1416.5, "fallback (B200_PROFILING.md)"
+        tf = d.get("bf16_tflops_sustained", d.get("bf16_tflops"))
+        hbm = d.get("hbm_gbs")
+        if tf is not None and hbm is not None:
+            return hbm, tf, "measured (MEASURED_PEAKS.json)"
+        return hbm or 3350.0, tf or 989.0, "MEASURED_PEAKS.json where present, else the H100 SXM data sheet (dense), not measured"
+    return 3350.0, 989.0, "H100 SXM data sheet (dense), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, gpu_index):
         self.rows, self.proc, self.gpu = [], None, gpu_index
@@ -206,35 +213,6 @@ def run_reference(args):
     print(json.dumps(out))
 
 
-def _bytes(txt):
-    scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    val, unit = txt.split()
-    return float(val) * scale[unit]
-
-
-def ncu_summaries():
-    """hardware counters of the committed `ncu --set full` captures (profiles/): newest round first"""
-    out = {}
-    prof = os.path.join(ROOT, "profiles")
-    for rnd in ("r02", "r01"):
-        path = os.path.join(prof, "%s_ncu_corr_fwd_tc.json" % rnd)
-        if "corr_dram_bytes" not in out and os.path.exists(path):
-            try:
-                k = json.load(open(path))["kernels"][0]
-                out["corr_dram_bytes"] = _bytes(k["dram_read"]) + _bytes(k["dram_write"])
-                out["corr_l2_bytes"] = _bytes(k["l2_to_sm_read"]) if "l2_to_sm_read" in k else None
-                out["corr_source"] = "profiles/" + os.path.basename(path)
-            except Exception:
-                pass
-        path = os.path.join(prof, "%s_ncu_gemm_step.json" % rnd)
-        if "gemm_dram_bytes" not in out and os.path.exists(path):
-            try:
-                out["gemm_dram_bytes"] = sum(_bytes(k["dram_read"]) + _bytes(k["dram_write"]) for k in json.load(open(path))["kernels"])
-            except Exception:
-                pass
-    return out
-
-
 def reference_cuda_leg(st, run, our_ms, iters=10, warmup=3):
     """The reference's own CUDA pipeline for the SAME update on the SAME state, timed here with CUDA events:
     ref_cuda_corr.forward x2 + stack (dpvo.py:200-207), the torch Update under autocast (dpvo.py:332) with the same
@@ -261,7 +239,7 @@ def reference_cuda_leg(st, run, our_ms, iters=10, warmup=3):
     torch.cuda.synchronize()
     ms = a.elapsed_time(b) / iters
     return {"ms_per_step": ms, "value": 1e3 / ms, "unit": "frames/s", "iters": iters, "speedup_ours": ms / our_ms,
-            "what": "reference CUDA kernels (oracle/_ref: correlation_kernel.cu, ba_cuda.cu compiled for sm_100a) + torch Update under "
+            "what": "reference CUDA kernels (oracle/_ref: correlation_kernel.cu, ba_cuda.cu compiled for sm_90a) + torch Update under "
                     "autocast, eager launches as in dpvo.py:328-360, same synthetic state and weights, same GPU, same process"}
 
 
@@ -270,11 +248,30 @@ def workload_config(config, E):
         w = "BASELINE configs[1]: synthetic 480x640 stream, default.yaml (96 patches, 10-pose window), E=%d edges, 2208 live patches" % E
     else:
         w = "BASELINE configs[2]: synthetic 480x752 stream, fast.yaml (48 patches, 7-pose window), E=%d edges" % E
-    return {"workload": w, "edges": E, "l2_policy": "inputs larger than L2 (fp16 feature ring 188 MB > 126 MB L2); no flush",
+    return {"workload": w, "edges": E, "l2_policy": "inputs larger than L2 (fp16 feature ring 188 MB > 50 MB L2); no flush",
             "parallelism": "one independent stream per GPU, no collectives"}
 
 
 # ------------------------------------------------------------------------------------ GPU path
+DUMP_NET_ROWS = 8192                 # rows of the recurrent state written by --dump-outputs (all of it is ~73 MB)
+
+
+def dump_outputs(out_dir, run, target, weight):
+    """what the timed loop computed in its last step, as float32 / float64 .npy files"""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    st = run.s
+    net = run.net.reshape(-1, run.net.shape[-1])
+    rows = torch.randperm(net.shape[0], generator=torch.Generator().manual_seed(0))[:DUMP_NET_ROWS].sort().values
+    arrays = {"target": target, "weight": weight, "poses": st.poses[:st.n], "patches": st.patches[:st.n * run.M],
+              "net_rows": net[rows.to(net.device)]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "net_row_index.npy"), rows.double().numpy())
+
+
 def run_ours(args):
     import torch
     import dpvo_b200
@@ -316,7 +313,7 @@ def run_ours(args):
     for i in range(args.steps):
         run.timers = {k: v[i] for k, v in ev.items()}
         run.reset()
-        run.step()
+        last = run.step()
     t_end.record()
     barrier()
     windows.append((w0, time.time()))
@@ -343,7 +340,7 @@ def run_ours(args):
             t_start.record()
             for i in range(args.steps):
                 run.reset()
-                run.step_graph()
+                last = run.step_graph()
             t_end.record()
             barrier()
             windows.append((w0, time.time()))
@@ -353,6 +350,9 @@ def run_ours(args):
         except Exception as exc:                           # noqa: BLE001 -- report and keep the eager number
             run.graph = None
             launch_mode = "eager launches (graph capture failed: %s)" % str(exc).splitlines()[0][:120]
+
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, run, *last)
 
     # ---- end to end: new frame from pinned host memory every step, poses + depths back to host
     hf = run.make_host_frame()
@@ -412,30 +412,26 @@ def run_ours(args):
     # dense layers: 17 layers x E rows (+ the two h layers on the group rows, < 1 % and not counted)
     gemm_flop = FLOP_PER_EDGE * E
     gemm_tf = gemm_flop / (gemm_ms * 1e-3) / 1e12
-    ncu = ncu_summaries()
     out = {"metric": METRIC, "value": world * 1e3 / ms, "unit": "frames/s", "n_gpus": world, "steps": args.steps,
            "warmup": max(args.warmup, 3), "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
            "dtype": "f16 operands, f32 accumulate/state (BA f32)", "data": "synthetic", "config": workload_config(args.config, E),
            "breakdown_ms": {"corr": corr_ms, "ba": ba_ms, "dense_layers": gemm_ms, "dense_layer_launches": gemm_launches,
                             "row_kernels_grouping_and_rest": ms_eager - corr_ms - ba_ms - gemm_ms,
-                            "gemm_backend": "tcgen05: fused layer chains (dpvo_update_corr_norm / neighbor_mlp x2 / gru_heads) + dpvo_linear_f16 for the SoftAgg layers", "eager_ms_per_step": ms_eager, "launch": launch_mode},
+                            "gemm_backend": "wgmma: fused layer chains (dpvo_update_corr_norm / neighbor_mlp x2 / gru_heads) + dpvo_linear_f16 for the SoftAgg layers", "eager_ms_per_step": ms_eager, "launch": launch_mode},
            "e2e": {"value": world * 1e3 / e2e_ms, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                    "pipeline": "frame t+1: pinned host -> staging on a copy stream while update t runs; staging -> ring slots, update (CUDA graph), "
                                "D2H of poses + depths into one of two pinned result buffers; the host waits for and reads frame t's results after it has issued frame t+1"},
            "gpu_launches": int(launches), "clocks": clocks,
-           "roofline": {"kernel": "chain_kernel x4 + linear_f16_kernel x4 (%d launches: the 17 dense layers of the update operator with their LayerNorm / gating / heads epilogues, tcgen05.mma + TMA + TMEM)" % gemm_launches,
+           "roofline": {"kernel": "chain_kernel x4 + linear_f16_kernel x4 (%d launches: the 17 dense layers of the update operator with their LayerNorm / gating / heads epilogues, wgmma + TMA)" % gemm_launches,
                         "bound": "tensor", "achieved": gemm_tf, "peak": tensor_tf, "unit": "TFLOP/s", "frac": gemm_tf / tensor_tf,
-                        "traffic": ncu.get("gemm_dram_bytes"), "peak_source": which + ", sustained dense 16-bit (kernels timed inside a step)",
+                        "peak_source": which + ", sustained dense 16-bit (kernels timed inside a step)",
                         "algorithmic_flop_per_step": gemm_flop, "kernel_ms": gemm_ms,
                         "timing": "sum of CUDA-event intervals around each of the launches, eager pass, same stream; since round 2 the intervals also contain the LayerNorm, gating, residual and heads work that is fused into the chain kernels' epilogues",
-                        "traffic_note": "sum of dram__bytes_read+write over the 8 dense-layer launches of one update, ncu --set full capture of this build: profiles/r02_ncu_gemm_step.json"},
-           "roofline_corr": {"kernel": "corr_fwd_tc (2-level patch correlation, tcgen05 + TMA)", "kernel_ms": corr_ms,
+                        "traffic_note": "DRAM traffic not measured"},
+           "roofline_corr": {"kernel": "corr_fwd_tc (2-level patch correlation, wgmma + TMA)", "kernel_ms": corr_ms,
                              "algorithmic_bytes_per_launch": BYTES_PER_EDGE_FP16 * E, "algorithmic_GBps": corr_alg,
                              "note": "SURVEY 8(d)'s per-edge window bytes are served by L2 (each frame is reused ~11x), so algorithmic/HBM-peak (%.2f) is "
-                                     "NOT a DRAM fraction; the hardware counters of one launch are below" % (corr_alg / hbm),
-                             "dram_bytes": ncu.get("corr_dram_bytes"), "l2_to_sm_bytes": ncu.get("corr_l2_bytes"),
-                             "dram_frac_of_hbm_peak": (ncu["corr_dram_bytes"] / (corr_ms * 1e-3) / 1e9 / hbm) if ncu.get("corr_dram_bytes") else None,
-                             "ncu_source": ncu.get("corr_source")}}
+                                     "NOT a DRAM fraction" % (corr_alg / hbm)}}
     if not args.no_reference_cuda and world == 1:
         out["reference_cuda"] = reference_cuda_leg(st, run, ms)
     if not args.no_cpu_baseline and world == 1:          # the CPU leg is timed at N = 1 only
@@ -467,7 +463,7 @@ def synthetic_clip(device, seed, n_frames=15, ht=480, wd=640):
 
 def run_train(args):
     """BASELINE configs[3]: global batch 8 clips per optimiser step, split over the ranks (strong scaling: 1 GPU runs
-    8 clips with gradient accumulation, 8 GPUs one clip each), gradients averaged over NVLink by
+    8 clips with gradient accumulation, 8 GPUs one clip each), gradients averaged over NVLink / NVSwitch by
     dpvo_b200.multigpu.GradReducer (bucketed NCCL all-reduce launched from autograd hooks)."""
     import numpy as np
     import torch
@@ -541,7 +537,13 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-reference-cuda", action="store_true", help="skip the reference-CUDA-pipeline leg")
     ap.add_argument("--no-graph", action="store_true", help="time eager launches only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (--mode infer --impl ours only)")
     args = ap.parse_args()
+    if args.steps is not None and args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.mode != "infer" or args.impl != "ours"):
+        ap.error("--dump-outputs writes the outputs of the GPU inference path: it needs --mode infer --impl ours")
     if args.mode == "train":
         args.steps = 3 if args.steps is None else args.steps
         args.warmup = 1 if args.warmup is None else args.warmup

@@ -1,4 +1,4 @@
-"""dpvo_b200 -- B200-native (sm_100a) implementation of DPVO's per-frame update hot path.
+"""dpvo_b200 -- H100-native (sm_90a) implementation of DPVO's per-frame update hot path.
 
 Importing the package locates the in-tree build products and makes the three reference-named
 torch extensions importable by their top-level names, exactly as the reference's Python files

@@ -1,13 +1,13 @@
-"""In-tree build of the sm_100a library and its torch-extension shims.
+"""In-tree build of the sm_90a library and its torch-extension shims.
 
     python -m dpvo_b200.build            # build what is out of date
     python -m dpvo_b200.build --force    # rebuild everything
 
-Products (git-ignored, shipped to the GPU box by gpurun):
+Products (git-ignored):
     dpvo_b200/lib/libdpvo_b200.so                  C-ABI library (nvcc, no torch dependency)
     dpvo_b200/_ext/{cuda_corr,cuda_ba,lietorch_backends,dpvo_b200_ext}<EXT_SUFFIX>
                                                    pybind shims, one object copied four times
-nvcc cross-compiles for sm_100a without a GPU, so this also is the CPU-side "does it build" check.
+nvcc cross-compiles for sm_90a without a GPU, so this also is the CPU-side "does it build" check.
 """
 import os
 import shutil
@@ -26,11 +26,11 @@ INCLUDE = os.path.join(os.path.dirname(ROOT), "include")
 CU_SOURCES = ["common.cu", "chain.cu", "corr.cu", "corr_tc.cu", "patchify.cu", "lie.cu", "graph.cu", "pgraph.cu", "ba.cu", "ba_wide.cu", "update_ops.cu", "gemm.cu"]
 SHIM_MODULES = ["cuda_corr", "cuda_ba", "lietorch_backends", "dpvo_b200_ext"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
 ]
-# perf-attribution switches (timestamps, dropped loads/stores, alternative code paths selected by environment
-# variables) exist only in builds made with DPVO_B200_PERF_EXPERIMENTS=1 (tools/); the release library has none
+# the bundle adjustment's phase timestamps (DPVO_B200_BA_TIMING, ba.cu) exist only in builds made with
+# DPVO_B200_PERF_EXPERIMENTS=1; the release library has none
 if os.environ.get("DPVO_B200_PERF_EXPERIMENTS"):
     NVCC_FLAGS.append("-DDPVO_B200_PERF_EXPERIMENTS")
 
@@ -73,10 +73,18 @@ def build_library(force=False, verbose=False):
         if force or _newer(obj, [src] + hdrs):
             jobs.append([_nvcc()] + NVCC_FLAGS + ["-I", INCLUDE, "-c", src, "-o", obj])
     if jobs:
+        # the CPUs this process may run on (a container or batch slot can have far fewer than the host reports)
+        workers = min(len(jobs), len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 4))
         if verbose:
-            print("[dpvo_b200.build] nvcc: %d translation units" % len(jobs), flush=True)
-        with ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 4)) as ex:
-            list(ex.map(_run, jobs))
+            print("[dpvo_b200.build] nvcc: %d translation units, %d at a time" % (len(jobs), workers), flush=True)
+
+        def compile_one(cmd):
+            _run(cmd)
+            if verbose:
+                print("[dpvo_b200.build]   %s" % os.path.basename(cmd[cmd.index("-c") + 1]), flush=True)
+
+        with ThreadPoolExecutor(max_workers=workers) as ex:
+            list(ex.map(compile_one, jobs))
     lib = os.path.join(LIBDIR, "libdpvo_b200.so")
     if force or jobs or _newer(lib, objs):
         _run([_nvcc(), "-shared", "-o", lib] + objs + ["-lcudart", "-Xlinker", "--no-undefined"])

@@ -1,4 +1,4 @@
-// fastba: in-place Gauss-Newton bundle adjustment over the patch graph, sm_100a.
+// fastba: in-place Gauss-Newton bundle adjustment over the patch graph, sm_90a.
 //
 // Replaces dpvo/fastba/ba_cuda.cu:232-376 (per-edge kernel with ~340 global float atomics per
 // edge), the ~30 ATen launches per iteration around it (:484-563, dense E, matmuls, cuSOLVER

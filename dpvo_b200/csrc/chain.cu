@@ -1,5 +1,5 @@
-// The row-local layer chains of the update operator (dpvo/net.py:74-92, dpvo/blocks.py:15-29) as ONE tcgen05 kernel
-// each: a 128-edge tile goes through all dense layers of a chain without leaving the SM.
+// The row-local layer chains of the update operator (dpvo/net.py:74-92, dpvo/blocks.py:15-29) as ONE wgmma kernel
+// each: a 64-edge tile goes through all dense layers of a chain without leaving the SM.
 //
 //   chain A  (net.py:76-77)   net = LN( net + inp[kk] + corr-MLP(corr) )          882->384 ReLU 384 LN ReLU 384
 //   chain C  (net.py:83-85)   net = net + c( mask * net[ix] )                      384 ReLU 384   (c1 and c2)
@@ -10,72 +10,58 @@
 // (with its tail wave) per layer.
 //
 // One persistent CTA per SM, warp-specialised:
-//   warps 0-7  epilogue    TMEM lane quarter = warp % 4 (32 rows), column half = warp / 4 (192 columns).  Bias,
-//                          activation, LayerNorm (row statistics exchanged between the two warps that share a row),
-//                          gating, heads; the fp16 result is written straight into the shared-memory operand tile of
-//                          the NEXT layer in the SWIZZLE_128B K-major layout the UMMA descriptors expect.  TMEM loads
-//                          run one 32-column chunk ahead of the arithmetic; all parameters sit in shared memory.
-//   warp  8    MMA issuer  tcgen05.mma.cta_group::1.kind::f16, M=128 N=192 K=16; a layer is 2 column halves x 6
-//                          k-blocks x 4 instructions into a 384-column fp32 accumulator in TMEM
-//   warp  9    W producer  streams the weight k-blocks (192 x 64 fp16 = 24 KB) of every layer of every tile through
-//                          a TMA ring (4 deep, 3 in chains A and C); it depends on no data, so it runs ahead across
+//   warps 0-7  consumers   two warpgroups, warpgroup h owns column half h (192 columns) of the 64-row tile: it issues
+//                          wgmma.m64n192k16 on shared-memory descriptors (a layer is 6 k-blocks x 4 instructions), keeps the
+//                          64 x 192 fp32 accumulator in registers and runs the epilogue from them: bias, activation,
+//                          LayerNorm (row statistics exchanged between the two warps that share a row), gating, heads; the
+//                          fp16 result is written straight into the shared-memory operand tile of the NEXT layer in the
+//                          SWIZZLE_128B K-major layout the descriptors expect.  All parameters sit in shared memory.
+//   warp  8    W producer  streams the weight k-blocks (192 x 64 fp16 = 24 KB) of every layer of every tile through a
+//                          4-deep TMA ring, alternating the column halves; it depends on no data, so it runs ahead across
 //                          layers and tiles
-//   warp 10    (chain A)   streams the 14 k-blocks of the 896-column correlation rows through the operand slots
-//   warps 10-13 (chain C)  gather the neighbour rows net[ix] (masked) into the operand slots with cp.async
-// Shared memory: 6 operand slots of 128 rows x 64 halves (96 KB, one K=384 activation tile, overwritten in place by
-// the layer's own output once its MMAs have retired), the weight ring, the parameter vectors, 2-4 KB of exchange.
-// The fp32 recurrent state enters and leaves through TMA boxes of 32 rows x 32 columns (128-byte rows; 64-byte rows
-// halve the achieved rate): loads land in the warp's own 12 KB of the operand slots -- dead once the chain's last MMAs
-// have retired -- so staging needs no synchronisation between warps; chains A and C hand the slots back to their
-// producers as soon as the loads are consumed (the next tile's rows then travel under the rest of the epilogue) and
-// stage their stores in 6 KB of dedicated memory per warp.  The un-normalised values of a LayerNorm wait in TMEM
-// (tcgen05.st) between the statistics pass and the normalisation pass.
-// Row-private intermediates of chain G (the sigmoid gate, the fp32 LayerNorm output that the gated residual adds
-// to) live in a per-CTA global scratch laid out chunk-major ([16-byte chunk][row]), so that the row-per-thread
-// ownership TMEM imposes gives perfectly coalesced 512-byte accesses; it is rewritten every tile and stays in L2
-// (TMEM is full: 384 accumulator columns of 512).  Measured timelines and what bounds each phase: DESIGN.md 3.1, 5.2.
+//   warp  9    (chain A)   streams the 14 k-blocks of the 896-column correlation rows through the operand slots
+//   warps 9-10 (chain C)   gather the neighbour rows net[ix] (masked) into the operand slots with cp.async
+//   (warps 8-11 form the producer warpgroup; they hand most of their registers to the consumers)
+// Shared memory: 6 operand slots of 64 rows x 64 halves (48 KB, one K=384 activation tile, overwritten in place by the
+// layer's own output once both warpgroups' MMAs have retired), the weight ring (96 KB), the parameter vectors, 2 KB of
+// exchange.  The fp32 recurrent state is read and written by the consumers directly: a warp's accesses cover 8 rows x
+// 32 contiguous bytes, whole sectors.
+// Row-private intermediates of chain G (the sigmoid gate, the fp32 LayerNorm output that the gated residual adds to)
+// do not fit next to the accumulator in registers; they live in a per-CTA global scratch laid out fragment-major
+// ([element pair][thread]) so that every access is a coalesced 256-byte warp transaction; it is rewritten every tile
+// and stays in L2.
 #include "common.cuh"
 #include "tc.cuh"
 #include <cuda.h>
 
 namespace dpvo {
 
-constexpr int CH_M = 128, CH_DIM = 384, CH_KB = 6, CH_NH = 192;
-constexpr int CH_SLOT = CH_M * 128;            // one k-block of the operand tile: 128 rows x 128 bytes
+constexpr int CH_M = 64, CH_DIM = 384, CH_KB = 6, CH_NH = 192;
+constexpr int CH_SLOT = CH_M * 128;            // one k-block of the operand tile: 64 rows x 128 bytes
 constexpr int CH_WSTAGE = CH_NH * 128;         // one weight k-block of a column half: 192 rows x 128 bytes
+constexpr int CH_WST = 4;                      // weight ring depth (even: each column half keeps to its own stages)
 constexpr int CH_K0 = 896, CH_KB0 = CH_K0 / 64;
-constexpr int CH_EPI_WARPS = 8, CH_MMA_WARP = 8, CH_W_WARP = 9, CH_A_WARP = 10;
-constexpr int CH_GATHER_THREADS = 128;
-constexpr uint32_t CH_IDESC = (1u << 4) | ((uint32_t)(CH_NH >> 3) << 17) | ((uint32_t)(CH_M >> 4) << 24);
+constexpr int CH_CONS_WARPS = 8, CH_CONS = CH_CONS_WARPS * 32, CH_W_WARP = 8, CH_A_WARP = 9;
+constexpr int CH_GATHER_THREADS = 64;
 constexpr float CH_EPS = 1e-3f;
 
 enum { CHAIN_A = 0, CHAIN_C = 1, CHAIN_G = 2 };
-constexpr int chain_threads(int chain) { return chain == CHAIN_C ? 320 + CH_GATHER_THREADS : (chain == CHAIN_A ? 352 : 320); }
+// two consumer warpgroups and one producer warpgroup (whole warpgroups, so that registers can move between them)
+constexpr int CH_THREADS = CH_CONS + 128;
 
 struct ChainBars {
-  uint64_t w_full[4], w_empty[4];
+  uint64_t w_full[CH_WST], w_empty[CH_WST];
   uint64_t a_full[CH_KB], a_empty[CH_KB];
-  uint64_t acc_full[2], epi_done, slots_free;     // acc_full[h]: the MMAs of column half h of a layer have retired
-  uint64_t stg[CH_EPI_WARPS][6];
-  uint32_t tmem_base;
+  uint64_t slots_free;                           // the tile's last MMAs on the operand slots have retired
 };
-constexpr int CH_BAR_BYTES = 640;
-static_assert(sizeof(ChainBars) <= CH_BAR_BYTES, "barrier block");
-// Shared-memory plan per chain.  Chains A and C end in an epilogue that streams the fp32 state through TMA staging; they
-// get 6 KB of dedicated staging per epilogue warp (and a 3-deep weight ring) so that the operand slots are free for the
-// next tile's producers as soon as the last MMAs have retired.  Chain G stages in the (then dead) operand slots.
 template <int CHAIN> struct ChainCfg {
-  static constexpr int WST = CHAIN == 2 ? 4 : 3;                                    // weight ring depth
-  static constexpr int NPARAM = CHAIN == 0 ? 5 * CH_DIM : (CHAIN == 1 ? 2 * CH_DIM : 14 * CH_DIM + 8);   // fp32 parameters kept in shared memory
-  static constexpr int PARAM_SKIP = CHAIN == 0 ? 2 * CH_DIM : 0;                    // chain A: corr.0 / corr.2 biases are read from global
-  static constexpr int STG_PER_WARP = CHAIN == 2 ? 0 : 6144;
-  static constexpr int XCH_BYTES = CHAIN == 2 ? 2 * CH_M * 16 : 2 * CH_M * 8;
+  static constexpr int NPARAM = CHAIN == 0 ? 7 * CH_DIM : (CHAIN == 1 ? 2 * CH_DIM : 14 * CH_DIM + 8);   // fp32 parameters kept in shared memory
+  static constexpr int XCH_BYTES = 2 * CH_M * 16;
   static constexpr int OFF_WRING = CH_KB * CH_SLOT;
-  static constexpr int OFF_STG = OFF_WRING + WST * CH_WSTAGE;
-  static constexpr int OFF_XCH = OFF_STG + CH_EPI_WARPS * STG_PER_WARP;
+  static constexpr int OFF_XCH = OFF_WRING + CH_WST * CH_WSTAGE;
   static constexpr int OFF_PARAM = OFF_XCH + XCH_BYTES;
   static constexpr int OFF_BARS = OFF_PARAM + NPARAM * 4;
-  static constexpr int SMEM = OFF_BARS + CH_BAR_BYTES;
+  static constexpr int SMEM = OFF_BARS + (int)sizeof(ChainBars);
 };
 static_assert(ChainCfg<0>::SMEM <= 232448 && ChainCfg<1>::SMEM <= 232448 && ChainCfg<2>::SMEM <= 232448, "shared memory budget");
 static_assert(ChainCfg<0>::OFF_BARS % 8 == 0 && ChainCfg<1>::OFF_BARS % 8 == 0 && ChainCfg<2>::OFF_BARS % 8 == 0, "barrier alignment");
@@ -84,7 +70,8 @@ constexpr int64_t CH_SCRATCH_PER_CTA = CH_SCRATCH_GATE + CH_SCRATCH_X;
 
 struct ChainArgs {
   int64_t rows;
-  const float* state;          // the fp32 recurrent state [rows, 384] (for L2 prefetches; the data path goes through tensor maps)
+  float* state;                // the fp32 recurrent state [rows, 384]
+  __half* state16;             // A, C: fp16 copy of the new state [rows, 384]
   const float* p;              // fp32 parameter block, layout per chain (see the launchers)
   const __half* inp16;         // A: context table, row e uses inp16[inp_index ? inp_index[e] : e]
   const int64_t* inp_index;
@@ -98,23 +85,12 @@ struct ChainArgs {
   float* delta; float* weight;
   unsigned char* scratch;
   int n_params;                // floats in p
-  long long* dbg;              // perf-experiment builds: SM-clock stamps of CTA 0 (NULL = off)
 };
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-// dbg[((tile_iter * 8 + step) * 4 + k]: k = 0 MMA warp starts the step, 1 all its MMAs issued, 2 epilogue sees the accumulator, 3 epilogue done
-#define CH_STAMP(ti, step, k) do { if (a.dbg && blockIdx.x == 0 && lane == 0 && (ti) < 3 && (step) < 8) a.dbg[(((ti) * 8 + (step)) << 2) + (k)] = clock64(); } while (0)
-// fine ticks of epilogue warp 0 in the second tile: dbg[96 + step * 16 + tick]
-#define CH_TICK() do { if (a.dbg && blockIdx.x == 0 && warp == 0 && lane == 0 && e_ti == 1 && e_l < 8 && e_tick < 16) a.dbg[96 + e_l * 16 + e_tick] = clock64(); ++e_tick; } while (0)
-#else
-#define CH_STAMP(ti, step, k) do { } while (0)
-#define CH_TICK() do { } while (0)
-#endif
 
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
-// one MUFU op instead of two (the gate layers evaluate 49k sigmoids per tile and the SFU does 16 per clock):
-// sigmoid(x) = 0.5 + 0.5 tanh(x / 2), tanh.approx has a relative error of 2^-11; the result is rounded to fp16 anyway
 // two gates per SFU op: the pre-activations are rounded to fp16 first (which is where the reference's autocast computes
-// its sigmoid, blocks.py:19 under dpvo.py:332), tanh.approx.f16x2 has an absolute error of 2^-11, the gate is stored as fp16
+// its sigmoid, blocks.py:19 under dpvo.py:332), sigmoid(x) = 0.5 + 0.5 tanh(x / 2), tanh.approx.f16x2 has an absolute
+// error of 2^-11, the gate is stored as fp16
 __device__ __forceinline__ __half2 sigmoid_tanh_h2(float a, float b) {
   const __half2 x = __floats2half2_rn(0.5f * a, 0.5f * b);
   uint32_t t;
@@ -122,19 +98,12 @@ __device__ __forceinline__ __half2 sigmoid_tanh_h2(float a, float b) {
   const __half2 half = __float2half2_rn(0.5f);
   return __hfma2(*reinterpret_cast<const __half2*>(&t), half, half);
 }
-__device__ __forceinline__ float sigmoid_tanh(float x) {
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
-  return fmaf(0.5f, t, 0.5f);
-}
 
 template <int CHAIN>
-__global__ void __launch_bounds__(chain_threads(CHAIN), 1)
+__global__ void __launch_bounds__(CH_THREADS, 1)
 chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW0, const __grid_constant__ CUtensorMap tmW,
-             const __grid_constant__ CUtensorMap tmNet, const __grid_constant__ CUtensorMap tmN16, const __grid_constant__ CUtensorMap tmPf,
              const ChainArgs a) {
   using Cfg = ChainCfg<CHAIN>;
-  constexpr int CH_WST = Cfg::WST;
   extern __shared__ __align__(1024) unsigned char ch_smem[];
   unsigned char* slots = ch_smem;
   unsigned char* wring = ch_smem + Cfg::OFF_WRING;
@@ -148,24 +117,17 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
 
   if (threadIdx.x == 0) {
     if ((smem_u32(ch_smem) & 1023u) != 0) { printf("chain_kernel: shared memory base is not 1024-byte aligned\n"); __trap(); }
-    for (int s = 0; s < CH_WST; ++s) { mbar_init(&bars->w_full[s], 1); mbar_init(&bars->w_empty[s], 1); }
-    for (int s = 0; s < CH_KB; ++s) { mbar_init(&bars->a_full[s], CHAIN == CHAIN_C ? CH_GATHER_THREADS : 1); mbar_init(&bars->a_empty[s], 1); }
-    mbar_init(&bars->acc_full[0], 1);
-    mbar_init(&bars->acc_full[1], 1);
-    mbar_init(&bars->epi_done, CH_EPI_WARPS);
-    mbar_init(&bars->slots_free, CH_EPI_WARPS);
-    for (int w = 0; w < CH_EPI_WARPS; ++w) for (int j = 0; j < 6; ++j) mbar_init(&bars->stg[w][j], 1);
+    // consumer-side arrivals come from lane 0 of every warp that read the stage: 4 per column half, 8 for both
+    for (int s = 0; s < CH_WST; ++s) { mbar_init(&bars->w_full[s], 1); mbar_init(&bars->w_empty[s], 4); }
+    for (int s = 0; s < CH_KB; ++s) { mbar_init(&bars->a_full[s], CHAIN == CHAIN_C ? CH_GATHER_THREADS : 1); mbar_init(&bars->a_empty[s], CH_CONS_WARPS); }
+    mbar_init(&bars->slots_free, CH_CONS_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (warp == CH_MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&bars->tmem_base)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  for (int i = threadIdx.x; i < Cfg::NPARAM; i += blockDim.x) sparam[i] = (Cfg::PARAM_SKIP + i < a.n_params) ? a.p[Cfg::PARAM_SKIP + i] : 0.f;
-  tc_fence_before();
+  for (int i = threadIdx.x; i < Cfg::NPARAM; i += blockDim.x) sparam[i] = i < a.n_params ? a.p[i] : 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
+  // 168 registers per thread at launch (3 warpgroups); the consumers hold a 96-register accumulator next to their epilogue
+  if (warp >= CH_CONS_WARPS) {
+  warpgroup_reg_dealloc<56>();
   if (warp == CH_W_WARP) {
     // ===================================================================== weight producer
     if (lane == 0) {
@@ -184,8 +146,8 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
         }
         for (int l = (CHAIN == CHAIN_A ? 1 : 0); l < NLAYERS; ++l) {
           const int wrow = (CHAIN == CHAIN_A ? l - 1 : l) * CH_DIM;      // row block of the stacked K=384 weights
-          for (int h = 0; h < 2; ++h)
-            for (int kb = 0; kb < CH_KB; ++kb) wload(&tmW, kb * 64, wrow + h * CH_NH);
+          for (int kb = 0; kb < CH_KB; ++kb)
+            for (int h = 0; h < 2; ++h) wload(&tmW, kb * 64, wrow + h * CH_NH);
         }
       }
     }
@@ -194,7 +156,7 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     if (lane == 0) {
       uint32_t ait = 0, ti = 0;
       for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-        if (ti > 0) mbar_wait_bounded(&bars->slots_free, (ti - 1) & 1);   // the previous tile's last epilogue has consumed its staged loads
+        if (ti > 0) mbar_wait_bounded(&bars->slots_free, (ti - 1) & 1);   // the previous tile is done with the slots
         const int m0 = (int)(tile * CH_M);
         for (int kb = 0; kb < CH_KB0; ++kb, ++ait) {
           const uint32_t s = ait % CH_KB, ph = (ait / CH_KB) & 1;
@@ -204,13 +166,13 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
         }
       }
     }
-  } else if (CHAIN == CHAIN_C && warp >= CH_A_WARP) {
+  } else if (CHAIN == CHAIN_C && warp < CH_A_WARP + CH_GATHER_THREADS / 32) {
     // ===================================================================== chain C: masked row gather
     const int pt = threadIdx.x - CH_A_WARP * 32;
     const int ch = pt & 7;
     uint32_t ti = 0;
     auto src_of = [&](int64_t tile, int i) -> int64_t {
-      const int64_t gr = tile * CH_M + (pt >> 3) + 16 * i;
+      const int64_t gr = tile * CH_M + (pt >> 3) + 8 * i;
       return (tile < n_tiles && gr < a.rows) ? a.gidx[gr] : -1;
     };
     int64_t src[8];
@@ -223,7 +185,7 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
         const uint32_t dst = smem_u32(slots + kb * CH_SLOT);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const int row = (pt >> 3) + 16 * i;
+          const int row = (pt >> 3) + 8 * i;
           const bool ok = src[i] >= 0;
           cp_async16(dst + row * 128 + ((ch ^ (row & 7)) << 4), a.x16 + (ok ? src[i] : 0) * CH_DIM + kb * 64 + ch * 8, ok ? 16u : 0u);
         }
@@ -238,529 +200,312 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
       cp_async_wait<1>(); fence_proxy_async(); mbar_arrive(&bars->a_full[4]);
       cp_async_wait<0>(); fence_proxy_async(); mbar_arrive(&bars->a_full[5]);
     }
-  } else if (warp == CH_MMA_WARP) {
-    // ===================================================================== MMA issuer
-    uint32_t wit = 0, ait = 0, n_epi = 0, ti = 0, m_l = 0;
-    auto wait_epi = [&]() { mbar_wait_bounded(&bars->epi_done, n_epi & 1); ++n_epi; tc_fence_after(); };
-    auto issue = [&](uint32_t a_smem, int h, bool first) {          // one k-block of one column half; consumes one weight stage
+  }
+  } else {
+    // ===================================================================== consumers: MMA + epilogue
+    warpgroup_reg_alloc<224>();
+    // thread -> rows rl + 8 rr (rr = 0, 1) of the tile, columns colbase + 8 j + cl + {0, 1} (j = 0..23): acc[4 j + 2 rr + {0, 1}]
+    const int h = warp >> 2, wq = warp & 3;
+    const int rl = wq * 16 + (lane >> 2);
+    const int cl = 2 * (lane & 3);
+    const int colbase = h * CH_NH;
+    float2* xch2 = reinterpret_cast<float2*>(xch);
+    auto SP = [&](int vec) { return sparam + vec * CH_DIM; };
+    float acc[96];
+    uint32_t wit = h, ait = 0;                                       // weight stages alternate between the column halves
+    auto cons_sync = [&]() { named_bar_sync(1, CH_CONS); };          // both warpgroups
+    auto pair_sync = [&]() { named_bar_sync(2 + wq, 64); };          // the two warps that share this thread's rows
+    auto warp_arrive = [&](uint64_t* bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+    // one k-block of this column half: 4 MMAs on the operand at a_smem, one weight stage; the previous k-block's
+    // stages are handed back once its MMAs have retired
+    uint32_t prev_w = 0, prev_a = 0;
+    auto mma_kblock = [&](uint32_t a_smem, bool first) {
       const uint32_t ws = wit % CH_WST;
       mbar_wait_bounded(&bars->w_full[ws], (wit / CH_WST) & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint64_t ad = umma_desc_sw128(a_smem), bd = umma_desc_sw128(smem_u32(wring + ws * CH_WSTAGE));
+      wit += 2;
+      const uint64_t ad = wgmma_desc_sw128(a_smem), bd = wgmma_desc_sw128(smem_u32(wring + ws * CH_WSTAGE));
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) tc_mma_f16(tmem_base + h * CH_NH, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), CH_IDESC, (!first || k) ? 1u : 0u);
-        tc_commit(&bars->w_empty[ws]);
-      }
-      __syncwarp();
-      ++wit;
+      for (int k = 0; k < 4; ++k) wgmma_m64n192k16(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (!first || k) ? 1u : 0u);
+      wgmma_commit();
+      return ws;
     };
-    auto chained_layer = [&]() {                                     // operand = the six slots, in place
-      CH_STAMP(ti, m_l, 0);
-      for (int h = 0; h < 2; ++h) {
-        for (int kb = 0; kb < CH_KB; ++kb) issue(smem_u32(slots + kb * CH_SLOT), h, kb == 0);
-        if (lane == 0) tc_commit(&bars->acc_full[h]);                // half h complete: an epilogue that does not touch the
-        __syncwarp();                                                // operand slots may start on it while the other half runs
+    auto mma_slots = [&]() {                                         // operand = the six slots
+      for (int kb = 0; kb < CH_KB; ++kb) {
+        const uint32_t ws = mma_kblock(smem_u32(slots + kb * CH_SLOT), kb == 0);
+        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&bars->w_empty[prev_w]); }
+        prev_w = ws;
       }
-      CH_STAMP(ti, m_l, 1);
-      ++m_l;
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      warp_arrive(&bars->w_empty[prev_w]);
     };
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-      m_l = 0;
-      if constexpr (CHAIN == CHAIN_A) {
-        if (ti > 0) wait_epi();                                     // accumulator drained by the previous tile's last epilogue
-        CH_STAMP(ti, m_l, 0);
-        for (int kb = 0; kb < CH_KB0; ++kb, ++ait) {
-          const uint32_t s = ait % CH_KB;
-          mbar_wait_bounded(&bars->a_full[s], (ait / CH_KB) & 1);
-          for (int h = 0; h < 2; ++h) issue(smem_u32(slots + s * CH_SLOT), h, kb == 0);
-          if (lane == 0) tc_commit(&bars->a_empty[s]);
-          __syncwarp();
+    auto mma_gathered = [&](uint32_t ti) {                           // chain C: wait for each gathered k-block
+      for (int kb = 0; kb < CH_KB; ++kb) {
+        mbar_wait_bounded(&bars->a_full[kb], ti & 1);
+        const uint32_t ws = mma_kblock(smem_u32(slots + kb * CH_SLOT), kb == 0);
+        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&bars->w_empty[prev_w]); }
+        prev_w = ws;
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      warp_arrive(&bars->w_empty[prev_w]);
+    };
+    auto mma_corr = [&]() {                                          // chain A: 14 k-blocks through the slot ring
+      for (int kb = 0; kb < CH_KB0; ++kb, ++ait) {
+        const uint32_t s = ait % CH_KB;
+        mbar_wait_bounded(&bars->a_full[s], (ait / CH_KB) & 1);
+        const uint32_t ws = mma_kblock(smem_u32(slots + s * CH_SLOT), kb == 0);
+        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&bars->w_empty[prev_w]); warp_arrive(&bars->a_empty[prev_a]); }
+        prev_w = ws; prev_a = s;
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      warp_arrive(&bars->w_empty[prev_w]);
+      warp_arrive(&bars->a_empty[prev_a]);
+    };
+    // fp16 activation -> operand slots of the next layer (SWIZZLE_128B K-major).  Both warpgroups' MMAs must have
+    // retired before the slots are overwritten, and the writes must be visible to the async proxy before the next MMAs.
+    auto store_act = [&]() {
+      cons_sync();
+#pragma unroll
+      for (int j = 0; j < 24; ++j) {
+        const int col = colbase + 8 * j;
+        unsigned char* slot = slots + (col >> 6) * CH_SLOT;
+        const int chunk = (col & 63) >> 3;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int row = rl + 8 * rr;
+          *reinterpret_cast<__half2*>(slot + row * 128 + ((chunk ^ (row & 7)) << 4) + cl * 2) = __floats2half2_rn(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
         }
-        if (lane == 0) { tc_commit(&bars->acc_full[0]); tc_commit(&bars->acc_full[1]); }
-        __syncwarp();
-        CH_STAMP(ti, m_l, 1);
-        ++m_l;
-        for (int l = 1; l < NLAYERS; ++l) { wait_epi(); chained_layer(); }
-      } else if constexpr (CHAIN == CHAIN_C) {
-        if (ti > 0) wait_epi();
-        CH_STAMP(ti, m_l, 0);
-        for (int h = 0; h < 2; ++h)
-          for (int kb = 0; kb < CH_KB; ++kb) {
-            if (h == 0) mbar_wait_bounded(&bars->a_full[kb], ti & 1);
-            issue(smem_u32(slots + kb * CH_SLOT), h, kb == 0);
-          }
-        if (lane == 0) { tc_commit(&bars->acc_full[0]); tc_commit(&bars->acc_full[1]); }
-        __syncwarp();
-        CH_STAMP(ti, m_l, 1);
-        ++m_l;
-        wait_epi();
-        chained_layer();
-      } else {
-        if (ti > 0) wait_epi();                                     // last epilogue of the previous tile
-        for (int l = 0; l < NLAYERS; ++l) { wait_epi(); chained_layer(); }   // l = 0 waits for the prologue
       }
-    }
-  } else if (warp < CH_EPI_WARPS) {
-    // ===================================================================== epilogue
-    const int q = warp & 3, h = warp >> 2;
-    const int row = q * 32 + lane;                                   // row of the tile this thread owns
-    const int colbase = h * CH_NH;                                   // first of its 192 columns
-    const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + colbase;
-    unsigned char* const piece0 = slots + 3 * h * CH_SLOT + q * 4096;   // this warp's 3 x 4 KB of the slots: rows 32q.., k-blocks 3h..3h+2
-    auto piece = [&](int j) { return piece0 + j * CH_SLOT; };
-    unsigned char* const stg0 = ch_smem + Cfg::OFF_STG + warp * Cfg::STG_PER_WARP;   // dedicated store staging (chains A, C): 6 KB
-    uint32_t acc_n = 0, stg_par = 0, e_l = 0, e_ti = 0, e_tick = 0;  // accumulator events seen; phase parity of each staging barrier
-    float2* xch2 = reinterpret_cast<float2*>(xch);
-    // parameter vectors: shared-memory copy (index in units of 384 floats, see the launchers for the order)
-    auto SP = [&](int vec) { return sparam + (vec * CH_DIM - Cfg::PARAM_SKIP); };
-
-    auto wait_acc = [&]() {                                          // both halves of the layer have retired
-      mbar_wait_bounded(&bars->acc_full[0], acc_n & 1);
-      mbar_wait_bounded(&bars->acc_full[1], acc_n & 1);
-      ++acc_n; tc_fence_after();
-      if (warp == 0) CH_STAMP(e_ti, e_l, 2);
-    };
-    // for an epilogue that only reads its own accumulator half and writes nothing the MMAs read: the warps of half 0 start
-    // as soon as their half has retired (the second half is still being multiplied) and catch up with the second barrier
-    // before they report the epilogue done -- every warp passes every phase of both barriers, in order
-    auto wait_acc_own_half = [&]() {
-      mbar_wait_bounded(&bars->acc_full[0], acc_n & 1);
-      if (h == 1) mbar_wait_bounded(&bars->acc_full[1], acc_n & 1);
-      tc_fence_after();
-      if (warp == 0) CH_STAMP(e_ti, e_l, 2);
-    };
-    auto wait_acc_other_half = [&]() {
-      if (h == 0) mbar_wait_bounded(&bars->acc_full[1], acc_n & 1);
-      ++acc_n;
-    };
-    auto epi_arrive = [&]() {                                        // TMEM reads done, operand tile written
       fence_proxy_async();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->epi_done);
-      if (warp == 0) CH_STAMP(e_ti, e_l, 3);
-      ++e_l; e_tick = 0;
+      cons_sync();
     };
-    // ---- accumulator chunk iterators: the TMEM load of chunk c+1 is in flight while chunk c is processed --------------
-    auto for_chunks32 = [&](auto&& f) {                              // 6 chunks of 32 columns
-      uint32_t ra[32], rb[32];
-      tc_ld32(tacc, ra);
-#pragma unroll 1
-      for (int c = 0; c < 6; c += 2) {
-        tc_ld_wait();
-        tc_ld32(tacc + (c + 1) * 32, rb);
-        CH_TICK();
-        f(c, ra);
-        tc_ld_wait();
-        if (c + 2 < 6) tc_ld32(tacc + (c + 2) * 32, ra);
-        CH_TICK();
-        f(c + 1, rb);
+    auto add_bias = [&](const float* b) {
+#pragma unroll
+      for (int j = 0; j < 24; ++j) {
+        const float2 bv = *reinterpret_cast<const float2*>(b + colbase + 8 * j + cl);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) { acc[4 * j + 2 * rr] += bv.x; acc[4 * j + 2 * rr + 1] += bv.y; }
       }
     };
-    auto for_chunks16 = [&](auto&& f) {                              // 12 chunks of 16 columns
-      uint32_t ra[16], rb[16];
-      tc_ld16(tacc, ra);
-#pragma unroll 1
-      for (int c = 0; c < 12; c += 2) {
-        tc_ld_wait();
-        tc_ld16(tacc + (c + 1) * 16, rb);
-        CH_TICK();
-        f(c, ra);
-        tc_ld_wait();
-        if (c + 2 < 12) tc_ld16(tacc + (c + 2) * 16, ra);
-        CH_TICK();
-        f(c + 1, rb);
+    auto relu_all = [&]() {
+#pragma unroll
+      for (int i = 0; i < 96; ++i) acc[i] = fmaxf(acc[i], 0.f);
+    };
+    // LayerNorm over the 384 columns of each of this thread's two rows: 48 columns here, the rest in the 3 other lanes of
+    // the quad and in the paired warp of the other column half
+    auto layer_norm = [&](const float* g, const float* b) {
+      float s[2] = {0.f, 0.f}, q[2] = {0.f, 0.f};
+#pragma unroll
+      for (int j = 0; j < 24; ++j)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const float t0 = acc[4 * j + 2 * rr], t1 = acc[4 * j + 2 * rr + 1];
+          s[rr] += t0 + t1;
+          q[rr] += t0 * t0 + t1 * t1;
+        }
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) { s[rr] += __shfl_xor_sync(0xffffffffu, s[rr], o); q[rr] += __shfl_xor_sync(0xffffffffu, q[rr], o); }
+      if ((lane & 3) == 0) { xch2[h * CH_M + rl] = make_float2(s[0], q[0]); xch2[h * CH_M + rl + 8] = make_float2(s[1], q[1]); }
+      pair_sync();
+      float mean[2], rstd[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const float2 o = xch2[(h ^ 1) * CH_M + rl + 8 * rr];
+        const float S = h ? o.x + s[rr] : s[rr] + o.x, S2 = h ? o.y + q[rr] : q[rr] + o.y;     // same order in both halves
+        mean[rr] = S * (1.0f / CH_DIM);
+        rstd[rr] = rsqrtf(fmaxf(S2 * (1.0f / CH_DIM) - mean[rr] * mean[rr], 0.f) + CH_EPS);
       }
-    };
-    // v[j] (op)= p[j]: p holds the same N floats for every lane (bias / LayerNorm parameters)
-    auto add_vec32 = [&](uint32_t (&r)[32], const float* p) {
+      pair_sync();                                                   // exchange slots free for the next use
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float4 b = *reinterpret_cast<const float4*>(p + 4 * j);
-        r[4 * j] = __float_as_uint(__uint_as_float(r[4 * j]) + b.x); r[4 * j + 1] = __float_as_uint(__uint_as_float(r[4 * j + 1]) + b.y);
-        r[4 * j + 2] = __float_as_uint(__uint_as_float(r[4 * j + 2]) + b.z); r[4 * j + 3] = __float_as_uint(__uint_as_float(r[4 * j + 3]) + b.w);
-      }
-    };
-    // fp16 activation -> operand slot of the next layer (SWIZZLE_128B K-major); c16 = 16-byte chunk index 0..23 of this thread's 192 columns
-    auto store_act8 = [&](int c16, float v0, float v1, float v2, float v3, float v4, float v5, float v6, float v7) {
-      uint4 o;
-      *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(v0, v1);
-      *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(v2, v3);
-      *reinterpret_cast<__half2*>(&o.z) = __floats2half2_rn(v4, v5);
-      *reinterpret_cast<__half2*>(&o.w) = __floats2half2_rn(v6, v7);
-      *reinterpret_cast<uint4*>(piece(c16 >> 3) + lane * 128 + (((c16 & 7) ^ (lane & 7)) << 4)) = o;
-    };
-    // row statistics over the 384 columns two threads share
-    auto ln_stats = [&](float sum, float sq, float& mean, float& rstd) {
-      xch2[h * CH_M + row] = make_float2(sum, sq);
-      named_bar_sync(1 + q, 64);
-      const float2 o = xch2[(h ^ 1) * CH_M + row];
-      named_bar_sync(1 + q, 64);
-      const float s = h ? o.x + sum : sum + o.x, s2 = h ? o.y + sq : sq + o.y;     // same order in both threads
-      mean = s * (1.0f / CH_DIM);
-      rstd = rsqrtf(fmaxf(s2 * (1.0f / CH_DIM) - mean * mean, 0.f) + CH_EPS);
-    };
-    // ---- staging of fp32 state tiles: 32 rows x 32 columns (4 KB, SWIZZLE_128B, 128-byte rows: a TMA box costs per row
-    // request, 64-byte rows halve the achieved bandwidth).  Loads land in this warp's three pieces of the operand slots,
-    // which are dead once the chain's last MMAs have retired; stores leave from dedicated staging (chains A, C) so that the
-    // slots go back to the producers as soon as the loads have been consumed.
-    auto stage_load = [&](int j, int c, int m0) {                    // lane 0: chunk c of the state -> piece j
-      mbar_arrive_expect_tx(&bars->stg[warp][j], 4096);
-      tma_load_2d(smem_u32(piece(j)), &tmNet, colbase + 32 * c, m0 + q * 32, &bars->stg[warp][j]);
-    };
-    auto stage_wait = [&](int j) { mbar_wait_bounded(&bars->stg[warp][j], (stg_par >> j) & 1); stg_par ^= 1u << j; };
-    auto stage_write32 = [&](unsigned char* buf, const uint32_t (&v)[32]) {
-      unsigned char* dst = buf + lane * 128;
+      for (int j = 0; j < 24; ++j) {
+        const float2 gv = *reinterpret_cast<const float2*>(g + colbase + 8 * j + cl), bv = *reinterpret_cast<const float2*>(b + colbase + 8 * j + cl);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) *reinterpret_cast<uint4*>(dst + ((i ^ (lane & 7)) << 4)) = make_uint4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-    };
-    auto stage_write16 = [&](unsigned char* buf, const uint32_t (&v)[32]) {   // 32 rows x 64 bytes, SWIZZLE_64B
-      unsigned char* dst = buf + lane * 64;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 o;
-        *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(__uint_as_float(v[8 * i]), __uint_as_float(v[8 * i + 1]));
-        *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(__uint_as_float(v[8 * i + 2]), __uint_as_float(v[8 * i + 3]));
-        *reinterpret_cast<__half2*>(&o.z) = __floats2half2_rn(__uint_as_float(v[8 * i + 4]), __uint_as_float(v[8 * i + 5]));
-        *reinterpret_cast<__half2*>(&o.w) = __floats2half2_rn(__uint_as_float(v[8 * i + 6]), __uint_as_float(v[8 * i + 7]));
-        *reinterpret_cast<uint4*>(dst + ((i ^ ((lane >> 1) & 3)) << 4)) = o;
-      }
-    };
-    auto add_half32 = [&](uint32_t (&v)[32], const __half* p) {      // v += 32 halves of a (gathered) global row
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const uint4 o = __ldg(reinterpret_cast<const uint4*>(p) + i);
-        const uint32_t w[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[k]));
-          v[8 * i + 2 * k] = __float_as_uint(__uint_as_float(v[8 * i + 2 * k]) + f.x);
-          v[8 * i + 2 * k + 1] = __float_as_uint(__uint_as_float(v[8 * i + 2 * k + 1]) + f.y);
+        for (int rr = 0; rr < 2; ++rr) {
+          acc[4 * j + 2 * rr] = (acc[4 * j + 2 * rr] - mean[rr]) * rstd[rr] * gv.x + bv.x;
+          acc[4 * j + 2 * rr + 1] = (acc[4 * j + 2 * rr + 1] - mean[rr]) * rstd[rr] * gv.y + bv.y;
         }
       }
     };
-    // this thread's 768 bytes of the state rows of a tile, pulled into L2 well before the epilogue that stages them
-    auto prefetch_rows = [&](int64_t tile) {
-      const int64_t gr = tile * CH_M + row;
-      if (tile < n_tiles && gr < a.rows) {
-        const char* p = reinterpret_cast<const char*>(a.state + gr * CH_DIM + colbase);
+    // acc += 384-wide fp16 table row (per row of this thread; src < 0: nothing)
+    auto add_row16 = [&](const __half* tab, const int64_t (&src)[2]) {
 #pragma unroll
-        for (int i = 0; i < 6; ++i) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + 128 * i));
+      for (int rr = 0; rr < 2; ++rr) {
+        if (src[rr] < 0) continue;
+        const __half* p = tab + src[rr] * CH_DIM + colbase + cl;
+#pragma unroll
+        for (int j = 0; j < 24; ++j) {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p + 8 * j));
+          acc[4 * j + 2 * rr] += f.x; acc[4 * j + 2 * rr + 1] += f.y;
+        }
       }
     };
-    // pass 1 of the epilogues that add the fp32 state: v = acc (+ bias) + state + extra -> back into TMEM; row statistics.
-    // use_acc = false: no accumulator yet (chain G prologue), v = state + extra.
-    auto ingest_state = [&](int m0, const float* bias, bool use_acc, auto&& extra, float& sum_out, float& sq_out) {
-      if (lane == 0) for (int j = 0; j < 3; ++j) stage_load(j, j, m0);
-      float sum = 0.f, sq = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 6; ++c) {
-        CH_TICK();
-        const int j = c % 3;
-        uint32_t v[32];
-        if (use_acc) { tc_ld32(tacc + 32 * c, v); tc_ld_wait(); add_vec32(v, bias + colbase + 32 * c); }
-        else {
+    auto add_state = [&](const bool (&live)[2], const int64_t (&grow)[2]) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = 0u;
-        }
-        extra(c, v);
-        stage_wait(j);
-        const unsigned char* src = piece(j) + lane * 128;
+      for (int rr = 0; rr < 2; ++rr) {
+        if (!live[rr]) continue;
+        const float* p = a.state + grow[rr] * CH_DIM + colbase + cl;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 x = *reinterpret_cast<const float4*>(src + ((i ^ (lane & 7)) << 4));
-          const float t0 = __uint_as_float(v[4 * i]) + x.x, t1 = __uint_as_float(v[4 * i + 1]) + x.y, t2 = __uint_as_float(v[4 * i + 2]) + x.z, t3 = __uint_as_float(v[4 * i + 3]) + x.w;
-          sum += (t0 + t1) + (t2 + t3);
-          sq += (t0 * t0 + t1 * t1) + (t2 * t2 + t3 * t3);
-          v[4 * i] = __float_as_uint(t0); v[4 * i + 1] = __float_as_uint(t1); v[4 * i + 2] = __float_as_uint(t2); v[4 * i + 3] = __float_as_uint(t3);
+        for (int j = 0; j < 24; ++j) {
+          const float2 x = *reinterpret_cast<const float2*>(p + 8 * j);
+          acc[4 * j + 2 * rr] += x.x; acc[4 * j + 2 * rr + 1] += x.y;
         }
-        if (c + 3 < 6) {                                             // refill the piece with the chunk three ahead
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) stage_load(j, c + 3, m0);
-        }
-        tc_st32(tacc + 32 * c, v);
       }
-      tc_st_wait();
-      sum_out = sum; sq_out = sq;
     };
-    auto release_slots = [&]() {                                     // this warp is done with its pieces of the slots
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->slots_free);
-    };
-    // pass 2: TMEM -> (LayerNorm) -> fp32 state rows + fp16 copy through the dedicated staging (4 KB + 2 KB) and TMA stores
-    auto emit_state = [&](int m0, bool ln, float mean, float rstd, const float* g, const float* b) {
-      unsigned char* o32 = stg0;
-      unsigned char* o16 = stg0 + 4096;
-      for_chunks32([&](int c, uint32_t (&r)[32]) {
-        if (ln) {
+    auto emit_state = [&](const bool (&live)[2], const int64_t (&grow)[2], bool with16) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 gv = *reinterpret_cast<const float4*>(g + colbase + 32 * c + 4 * j), bv = *reinterpret_cast<const float4*>(b + colbase + 32 * c + 4 * j);
-            r[4 * j] = __float_as_uint((__uint_as_float(r[4 * j]) - mean) * rstd * gv.x + bv.x); r[4 * j + 1] = __float_as_uint((__uint_as_float(r[4 * j + 1]) - mean) * rstd * gv.y + bv.y);
-            r[4 * j + 2] = __float_as_uint((__uint_as_float(r[4 * j + 2]) - mean) * rstd * gv.z + bv.z); r[4 * j + 3] = __float_as_uint((__uint_as_float(r[4 * j + 3]) - mean) * rstd * gv.w + bv.w);
-          }
-        }
-        if (c >= 1) { if (lane == 0) bulk_wait_read<0>(); __syncwarp(); }      // the stores of the previous chunk have read the buffer
-        stage_write32(o32, r);
-        stage_write16(o16, r);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmNet, colbase + 32 * c, m0 + q * 32, smem_u32(o32));
-          tma_store_2d(&tmN16, colbase + 32 * c, m0 + q * 32, smem_u32(o16));
-          bulk_commit();
-        }
-      });
-      if (lane == 0) bulk_wait_read<0>();
-      __syncwarp();
-    };
-    // plain hidden layer: relu(acc + bias) -> operand tile
-    auto epi_relu_act = [&](const float* bias) {
-      wait_acc();
-      for_chunks32([&](int c, uint32_t (&r)[32]) {
-        add_vec32(r, bias + colbase + 32 * c);
+      for (int rr = 0; rr < 2; ++rr) {
+        if (!live[rr]) continue;
+        float* p = a.state + grow[rr] * CH_DIM + colbase + cl;
+        __half* p16 = with16 ? a.state16 + grow[rr] * CH_DIM + colbase + cl : nullptr;
 #pragma unroll
-        for (int i = 0; i < 4; ++i)
-          store_act8(4 * c + i, fmaxf(__uint_as_float(r[8 * i]), 0.f), fmaxf(__uint_as_float(r[8 * i + 1]), 0.f), fmaxf(__uint_as_float(r[8 * i + 2]), 0.f),
-                     fmaxf(__uint_as_float(r[8 * i + 3]), 0.f), fmaxf(__uint_as_float(r[8 * i + 4]), 0.f), fmaxf(__uint_as_float(r[8 * i + 5]), 0.f),
-                     fmaxf(__uint_as_float(r[8 * i + 6]), 0.f), fmaxf(__uint_as_float(r[8 * i + 7]), 0.f));
-      });
-      epi_arrive();
+        for (int j = 0; j < 24; ++j) {
+          *reinterpret_cast<float2*>(p + 8 * j) = make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+          if (with16) *reinterpret_cast<__half2*>(p16 + 8 * j) = __floats2half2_rn(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+        }
+      }
     };
 
-    // chain G scratch (row-private, chunk-major): 16-byte chunk `id` of this thread's row
-    unsigned char* sc_gate = a.scratch ? a.scratch + (int64_t)blockIdx.x * CH_SCRATCH_PER_CTA : nullptr;
-    unsigned char* sc_x = sc_gate + CH_SCRATCH_GATE;
-    auto gate_ptr = [&](int id) { return reinterpret_cast<uint4*>(sc_gate + ((int64_t)((h * 24 + id) * CH_M + row) << 4)); };   // id 0..23
-    auto x_ptr = [&](int id) { return reinterpret_cast<float4*>(sc_x + ((int64_t)((h * 48 + id) * CH_M + row) << 4)); };        // id 0..47
+    // chain G scratch (row-private, fragment-major): element pair (j, rr) of this thread
+    float2* sc_x = a.scratch ? reinterpret_cast<float2*>(a.scratch + (int64_t)blockIdx.x * CH_SCRATCH_PER_CTA + CH_SCRATCH_GATE) : nullptr;
+    __half2* sc_gate = a.scratch ? reinterpret_cast<__half2*>(a.scratch + (int64_t)blockIdx.x * CH_SCRATCH_PER_CTA) : nullptr;
+    // this thread's element pair (j, rr) at a constant offset from one per-thread base: addresses formed per pair
+    // would be loop-invariant across the two GRU blocks, hoisted and kept live next to the accumulator (register spills)
+    if (sc_x) { sc_x += threadIdx.x; sc_gate += threadIdx.x; }
+    auto sidx = [&](int j, int rr) { return (j * 2 + rr) * CH_CONS; };
+    auto save_x = [&]() {
+#pragma unroll
+      for (int j = 0; j < 24; ++j)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) __stcg(sc_x + sidx(j, rr), make_float2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]));
+    };
 
     uint32_t ti = 0;
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-      const int m0 = (int)(tile * CH_M);
-      e_l = 0; e_ti = ti;
-      const int64_t grow = (int64_t)m0 + row;
-      const bool live = grow < a.rows;
+      const int64_t m0 = tile * CH_M;
+      int64_t grow[2]; bool live[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) { grow[rr] = m0 + rl + 8 * rr; live[rr] = grow[rr] < a.rows; }
       if constexpr (CHAIN == CHAIN_A) {
-        // parameters: b0 | b2 (global) | g3 | be3 | b5 | gN | beN (shared)
-        prefetch_rows(tile);
-        const int64_t irow = live ? (a.inp_index ? a.inp_index[grow] : grow) : -1;
-        const __half* ip = a.inp16 + (irow >= 0 ? irow : 0) * CH_DIM + colbase;
-        epi_relu_act(a.p);                                           // corr.0 + ReLU
-        {                                                            // corr.2 -> LayerNorm -> ReLU
-          wait_acc();
-          const float* b2 = a.p + CH_DIM;
-          float sum = 0.f, sq = 0.f, mean, rstd;
-          for_chunks32([&](int c, uint32_t (&r)[32]) {
-            add_vec32(r, b2 + colbase + 32 * c);
+        // parameters: b0 | b2 | g3 | be3 | b5 | gN | beN
+        mma_corr();                                                  // corr.0 + ReLU
+        add_bias(SP(0)); relu_all(); store_act();
+        mma_slots();                                                 // corr.2 -> LayerNorm -> ReLU
+        add_bias(SP(1)); layer_norm(SP(2), SP(3)); relu_all(); store_act();
+        mma_slots();                                                 // corr.5 ; net + inp + . ; norm
+        warp_arrive(&bars->slots_free);
+        int64_t irow[2];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) { const float t = __uint_as_float(r[i]); sum += t; sq += t * t; }
-          });
-          ln_stats(sum, sq, mean, rstd);
-          for_chunks32([&](int c, uint32_t (&r)[32]) {
-            add_vec32(r, b2 + colbase + 32 * c);
-            const float* g = SP(2) + colbase + 32 * c;
-            const float* be = SP(3) + colbase + 32 * c;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 g0 = *reinterpret_cast<const float4*>(g + 8 * i), g1 = *reinterpret_cast<const float4*>(g + 8 * i + 4);
-              const float4 e0 = *reinterpret_cast<const float4*>(be + 8 * i), e1 = *reinterpret_cast<const float4*>(be + 8 * i + 4);
-              auto nrm = [&](uint32_t u, float gg, float bb) { return fmaxf((__uint_as_float(u) - mean) * rstd * gg + bb, 0.f); };
-              store_act8(4 * c + i, nrm(r[8 * i], g0.x, e0.x), nrm(r[8 * i + 1], g0.y, e0.y), nrm(r[8 * i + 2], g0.z, e0.z), nrm(r[8 * i + 3], g0.w, e0.w),
-                         nrm(r[8 * i + 4], g1.x, e1.x), nrm(r[8 * i + 5], g1.y, e1.y), nrm(r[8 * i + 6], g1.z, e1.z), nrm(r[8 * i + 7], g1.w, e1.w));
-            }
-          });
-          epi_arrive();
-        }
-        {                                                            // corr.5 ; net + inp + . ; norm
-          wait_acc();
-          auto add_inp = [&](int c, uint32_t (&v)[32]) { if (irow >= 0) add_half32(v, ip + 32 * c); };
-          float sum, sq, mean, rstd;
-          ingest_state(m0, SP(4), true, add_inp, sum, sq);
-          release_slots();
-          ln_stats(sum, sq, mean, rstd);
-          emit_state(m0, true, mean, rstd, SP(5), SP(6));
-          epi_arrive();
-        }
+        for (int rr = 0; rr < 2; ++rr) irow[rr] = live[rr] ? (a.inp_index ? a.inp_index[grow[rr]] : grow[rr]) : -1;
+        add_bias(SP(4)); add_state(live, grow); add_row16(a.inp16, irow);
+        layer_norm(SP(5), SP(6));
+        emit_state(live, grow, true);
       } else if constexpr (CHAIN == CHAIN_C) {
-        // parameters: ba | bb (shared)
-        prefetch_rows(tile);
-        epi_relu_act(SP(0));
-        {
-          wait_acc();
-          auto none = [&](int, uint32_t (&)[32]) {};
-          float sum, sq;
-          ingest_state(m0, SP(1), true, none, sum, sq);
-          release_slots();
-          emit_state(m0, false, 0.f, 1.f, nullptr, nullptr);
-          epi_arrive();
-        }
+        // parameters: ba | bb
+        mma_gathered(ti);
+        add_bias(SP(0)); relu_all(); store_act();
+        mma_slots();
+        warp_arrive(&bars->slots_free);
+        add_bias(SP(1)); add_state(live, grow);
+        emit_state(live, grow, true);
       } else {
-        // parameters (shared): g0 | be0 | bg1 | ba1 | bb1 | g2 | be2 | bg2 | ba2 | bb2 | W4[4][384] | b4[4]
-        float ctr0 = 0.f, ctr1 = 0.f;
-        if (h == 0 && live && a.coords) { ctr0 = a.coords[grow * 2 * a.PP + a.centre]; ctr1 = a.coords[grow * 2 * a.PP + a.PP + a.centre]; }
-        {                                                            // prologue: x = LN(net + h_ij[group]); the operand slots are dead, stage in them
-          if (ti == 0) prefetch_rows(tile);
-          prefetch_rows(tile + gridDim.x);
-          const int grp = (live && a.group_of) ? a.group_of[grow] : -1;
-          const int grk = (live && a.group_kk) ? a.group_kk[grow] : -1;
-          const __half* hp = a.hij16 + (int64_t)(grp >= 0 ? grp : 0) * CH_DIM + colbase;
-          const __half* hk = a.hkk16 + (int64_t)(grk >= 0 ? grk : 0) * CH_DIM + colbase;
-          auto add_h = [&](int c, uint32_t (&v)[32]) {
-            if (grk >= 0) add_half32(v, hk + 32 * c);
-            if (grp >= 0) add_half32(v, hp + 32 * c);
-          };
-          float sum, sq, mean, rstd;
-          ingest_state(m0, nullptr, false, add_h, sum, sq);
-          ln_stats(sum, sq, mean, rstd);
-          for_chunks32([&](int c, uint32_t (&r)[32]) {
-            const float* g = SP(0) + colbase + 32 * c;
-            const float* be = SP(1) + colbase + 32 * c;
+        // parameters: g0 | be0 | bg1 | ba1 | bb1 | g2 | be2 | bg2 | ba2 | bb2 | W4[4][384] | b4[4]
+        {                                                            // prologue: x = LN(net + h_kk[patch] + h_ij[group])
+          int64_t gk[2], gp[2];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float4 g0 = *reinterpret_cast<const float4*>(g + 8 * i), g1 = *reinterpret_cast<const float4*>(g + 8 * i + 4);
-              const float4 e0 = *reinterpret_cast<const float4*>(be + 8 * i), e1 = *reinterpret_cast<const float4*>(be + 8 * i + 4);
-              auto nrm = [&](uint32_t u, float gg, float bb) { return (__uint_as_float(u) - mean) * rstd * gg + bb; };
-              const float y0 = nrm(r[8 * i], g0.x, e0.x), y1 = nrm(r[8 * i + 1], g0.y, e0.y), y2 = nrm(r[8 * i + 2], g0.z, e0.z), y3 = nrm(r[8 * i + 3], g0.w, e0.w);
-              const float y4 = nrm(r[8 * i + 4], g1.x, e1.x), y5 = nrm(r[8 * i + 5], g1.y, e1.y), y6 = nrm(r[8 * i + 6], g1.z, e1.z), y7 = nrm(r[8 * i + 7], g1.w, e1.w);
-              __stcg(x_ptr(8 * c + 2 * i), make_float4(y0, y1, y2, y3));
-              __stcg(x_ptr(8 * c + 2 * i + 1), make_float4(y4, y5, y6, y7));
-              store_act8(4 * c + i, y0, y1, y2, y3, y4, y5, y6, y7);
-            }
-          });
-          epi_arrive();
+          for (int rr = 0; rr < 2; ++rr) {
+            gk[rr] = (live[rr] && a.group_kk) ? a.group_kk[grow[rr]] : -1;
+            gp[rr] = (live[rr] && a.group_of) ? a.group_of[grow[rr]] : -1;
+          }
+#pragma unroll
+          for (int i = 0; i < 96; ++i) acc[i] = 0.f;
+          add_state(live, grow);
+          add_row16(a.hkk16, gk);
+          add_row16(a.hij16, gp);
+          layer_norm(SP(0), SP(1));
+          save_x();
+          store_act();
         }
 #pragma unroll 1
         for (int blk = 0; blk < 2; ++blk) {
           const int pv = 2 + 5 * blk;                                // bg | ba | bb | (g | be of the LayerNorm that follows block 0)
-          {                                                          // gate = sigmoid(x Wg + bg) -> scratch
-            wait_acc_own_half();
-            for_chunks32([&](int c, uint32_t (&r)[32]) {
-              add_vec32(r, SP(pv) + colbase + 32 * c);
+          mma_slots();                                               // gate = sigmoid(x Wg + bg) -> scratch
+          add_bias(SP(pv));
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                uint4 o;
-                *reinterpret_cast<__half2*>(&o.x) = sigmoid_tanh_h2(__uint_as_float(r[8 * i]), __uint_as_float(r[8 * i + 1]));
-                *reinterpret_cast<__half2*>(&o.y) = sigmoid_tanh_h2(__uint_as_float(r[8 * i + 2]), __uint_as_float(r[8 * i + 3]));
-                *reinterpret_cast<__half2*>(&o.z) = sigmoid_tanh_h2(__uint_as_float(r[8 * i + 4]), __uint_as_float(r[8 * i + 5]));
-                *reinterpret_cast<__half2*>(&o.w) = sigmoid_tanh_h2(__uint_as_float(r[8 * i + 6]), __uint_as_float(r[8 * i + 7]));
-                __stcg(gate_ptr(4 * c + i), o);
-              }
-            });
-            wait_acc_other_half();
-            epi_arrive();
-          }
-          epi_relu_act(SP(pv + 1));                                  // r1 = relu(x Wa + ba) -> operand tile (x is not needed as an operand again)
-          wait_acc();                                                // r2 = r1 Wb + bb
-          // v = x + gate * r2 for a 16-column chunk; the scratch operands of chunk c+1 are fetched while chunk c is computed
-          float4 xq[4]; uint4 gq[2];
-          auto fetch = [&](int c) {
+          for (int j = 0; j < 24; ++j)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) xq[i] = __ldcg(x_ptr(4 * c + i));
-            gq[0] = __ldcg(gate_ptr(2 * c)); gq[1] = __ldcg(gate_ptr(2 * c + 1));
-          };
-          auto gated = [&](int c, const uint32_t (&r)[16], float (&v)[16]) {
-            const float* bb = SP(pv + 2) + colbase + 16 * c;
-            const uint32_t gw[8] = {gq[0].x, gq[0].y, gq[0].z, gq[0].w, gq[1].x, gq[1].y, gq[1].z, gq[1].w};
-            const float xs[16] = {xq[0].x, xq[0].y, xq[0].z, xq[0].w, xq[1].x, xq[1].y, xq[1].z, xq[1].w,
-                                  xq[2].x, xq[2].y, xq[2].z, xq[2].w, xq[3].x, xq[3].y, xq[3].z, xq[3].w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float2 g = __half22float2(*reinterpret_cast<const __half2*>(&gw[j]));
-              const float2 b2v = *reinterpret_cast<const float2*>(bb + 2 * j);
-              v[2 * j] = xs[2 * j] + g.x * (__uint_as_float(r[2 * j]) + b2v.x);
-              v[2 * j + 1] = xs[2 * j + 1] + g.y * (__uint_as_float(r[2 * j + 1]) + b2v.y);
+            for (int rr = 0; rr < 2; ++rr) {
+              const __half2 g = sigmoid_tanh_h2(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1]);
+              __stcg(reinterpret_cast<unsigned int*>(sc_gate + sidx(j, rr)), *reinterpret_cast<const unsigned int*>(&g));
             }
-            if (c + 1 < 12) fetch(c + 1);                            // xq / gq are dead from here on
-          };
-          fetch(0);
-          if (blk == 0) {
-            // x' = LN(x + gate * r2): new fp32 x -> scratch, fp16 -> operand tile
-            float sum = 0.f, sq = 0.f, mean, rstd;
-            for_chunks16([&](int c, uint32_t (&r)[16]) {
-              float v[16];
-              gated(c, r, v);
-              uint32_t w[16];
+          mma_slots();                                               // r1 = relu(x Wa + ba) -> operand tile (x is not needed as an operand again)
+          add_bias(SP(pv + 1)); relu_all(); store_act();
+          mma_slots();                                               // r2 = r1 Wb + bb;  v = x + gate * r2
+          add_bias(SP(pv + 2));
 #pragma unroll
-              for (int j = 0; j < 16; ++j) { sum += v[j]; sq += v[j] * v[j]; w[j] = __float_as_uint(v[j]); }
-              tc_st16(tacc + 16 * c, w);
-            });
-            tc_st_wait();
-            ln_stats(sum, sq, mean, rstd);
-            for_chunks32([&](int c, uint32_t (&r)[32]) {
-              const float* g = SP(pv + 3) + colbase + 32 * c;
-              const float* be = SP(pv + 4) + colbase + 32 * c;
+          for (int j = 0; j < 24; ++j)
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float4 g0 = *reinterpret_cast<const float4*>(g + 8 * i), g1 = *reinterpret_cast<const float4*>(g + 8 * i + 4);
-                const float4 e0 = *reinterpret_cast<const float4*>(be + 8 * i), e1 = *reinterpret_cast<const float4*>(be + 8 * i + 4);
-                auto nrm = [&](uint32_t u, float gg, float bb) { return (__uint_as_float(u) - mean) * rstd * gg + bb; };
-                const float y0 = nrm(r[8 * i], g0.x, e0.x), y1 = nrm(r[8 * i + 1], g0.y, e0.y), y2 = nrm(r[8 * i + 2], g0.z, e0.z), y3 = nrm(r[8 * i + 3], g0.w, e0.w);
-                const float y4 = nrm(r[8 * i + 4], g1.x, e1.x), y5 = nrm(r[8 * i + 5], g1.y, e1.y), y6 = nrm(r[8 * i + 6], g1.z, e1.z), y7 = nrm(r[8 * i + 7], g1.w, e1.w);
-                __stcg(x_ptr(8 * c + 2 * i), make_float4(y0, y1, y2, y3));
-                __stcg(x_ptr(8 * c + 2 * i + 1), make_float4(y4, y5, y6, y7));
-                store_act8(4 * c + i, y0, y1, y2, y3, y4, y5, y6, y7);
-              }
-            });
-            epi_arrive();
-          } else {
-            // net = x + gate * r2 -> global (TMA stores staged in the dead operand slots, 3 x 4 KB); heads on relu(net)
+            for (int rr = 0; rr < 2; ++rr) {
+              const float2 x = __ldcg(sc_x + sidx(j, rr));
+              const unsigned int gu = __ldcg(reinterpret_cast<const unsigned int*>(sc_gate + sidx(j, rr)));
+              const float2 g = __half22float2(*reinterpret_cast<const __half2*>(&gu));
+              acc[4 * j + 2 * rr] = x.x + g.x * acc[4 * j + 2 * rr];
+              acc[4 * j + 2 * rr + 1] = x.y + g.y * acc[4 * j + 2 * rr + 1];
+            }
+          if (blk == 0) {                                            // x' = LN(x + gate * r2): fp32 -> scratch, fp16 -> operand tile
+            layer_norm(SP(pv + 3), SP(pv + 4));
+            save_x();
+            store_act();
+          } else {                                                   // net = x + gate * r2 -> global; heads on relu(net)
+            emit_state(live, grow, false);
             const float* W4 = SP(10);
-            float hd[4] = {0.f, 0.f, 0.f, 0.f};
-            for_chunks16([&](int c, uint32_t (&r)[16]) {
-              float v[16];
-              gated(c, r, v);
+            float hd[2][4];
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+              for (int o = 0; o < 4; ++o) hd[rr][o] = 0.f;
+#pragma unroll
+            for (int j = 0; j < 24; ++j)
 #pragma unroll
               for (int o = 0; o < 4; ++o) {
-                const float* wp = W4 + o * CH_DIM + colbase + 16 * c;
-                float s = 0.f;
+                const float2 wv = *reinterpret_cast<const float2*>(W4 + o * CH_DIM + colbase + 8 * j + cl);
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const float4 wv = *reinterpret_cast<const float4*>(wp + 4 * i);
-                  s += fmaxf(v[4 * i], 0.f) * wv.x + fmaxf(v[4 * i + 1], 0.f) * wv.y + fmaxf(v[4 * i + 2], 0.f) * wv.z + fmaxf(v[4 * i + 3], 0.f) * wv.w;
-                }
-                hd[o] += s;
+                for (int rr = 0; rr < 2; ++rr) hd[rr][o] += fmaxf(acc[4 * j + 2 * rr], 0.f) * wv.x + fmaxf(acc[4 * j + 2 * rr + 1], 0.f) * wv.y;
               }
-              // two 16-column chunks make one 32-column store box
-              unsigned char* o32 = piece((c >> 1) % 3);
-              if (c >= 6 && !(c & 1)) { if (lane == 0) bulk_wait_read<2>(); __syncwarp(); }
-              {
-                unsigned char* dst = o32 + lane * 128;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(dst + ((((c & 1) * 4 + i) ^ (lane & 7)) << 4)) = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+            for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+              for (int o = 0; o < 4; ++o) {
+                hd[rr][o] += __shfl_xor_sync(0xffffffffu, hd[rr][o], 1);
+                hd[rr][o] += __shfl_xor_sync(0xffffffffu, hd[rr][o], 2);
               }
-              if (c & 1) {
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) { tma_store_2d(&tmNet, colbase + 16 * (c - 1), m0 + q * 32, smem_u32(o32)); bulk_commit(); }
-              }
-            });
-            epi_arrive();
-            xch[h * CH_M + row] = make_float4(hd[0], hd[1], hd[2], hd[3]);
-            named_bar_sync(1 + q, 64);
-            if (h == 0 && live) {
-              const float4 o = xch[CH_M + row];
-              const float* b4 = W4 + 4 * CH_DIM;
-              *reinterpret_cast<float2*>(a.delta + grow * 2) = make_float2(hd[0] + o.x + b4[0] + ctr0, hd[1] + o.y + b4[1] + ctr1);   // target = centre + delta (dpvo.py:341)
-              *reinterpret_cast<float2*>(a.weight + grow * 2) = make_float2(sigmoid_fast(hd[2] + o.z + b4[2]), sigmoid_fast(hd[3] + o.w + b4[3]));
+            if ((lane & 3) == 0) {
+#pragma unroll
+              for (int rr = 0; rr < 2; ++rr) xch[h * CH_M + rl + 8 * rr] = make_float4(hd[rr][0], hd[rr][1], hd[rr][2], hd[rr][3]);
             }
-            named_bar_sync(1 + q, 64);
-            if (lane == 0) bulk_wait_read<0>();                      // the next prologue stages loads in the same buffers
-            __syncwarp();
+            pair_sync();
+            if (h == 0 && (lane & 3) == 0) {
+              const float* b4 = W4 + 4 * CH_DIM;
+#pragma unroll
+              for (int rr = 0; rr < 2; ++rr) {
+                if (!live[rr]) continue;
+                const float4 o = xch[CH_M + rl + 8 * rr];
+                float ctr0 = 0.f, ctr1 = 0.f;
+                if (a.coords) { ctr0 = a.coords[grow[rr] * 2 * a.PP + a.centre]; ctr1 = a.coords[grow[rr] * 2 * a.PP + a.PP + a.centre]; }
+                // target = centre + delta (dpvo.py:341)
+                *reinterpret_cast<float2*>(a.delta + grow[rr] * 2) = make_float2(hd[rr][0] + o.x + b4[0] + ctr0, hd[rr][1] + o.y + b4[1] + ctr1);
+                *reinterpret_cast<float2*>(a.weight + grow[rr] * 2) = make_float2(sigmoid_fast(hd[rr][2] + o.z + b4[2]), sigmoid_fast(hd[rr][3] + o.w + b4[3]));
+              }
+            }
+            pair_sync();
           }
         }
       }
     }
-    if (lane == 0) bulk_wait<0>();                                   // every state row has left shared memory and reached global
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == CH_MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "n"(512));
   }
 }
 
@@ -795,7 +540,7 @@ static int ch_tmap(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int 
   return DPVO_OK;
 }
 
-struct ChainMaps { CUtensorMap X, W0, W, Net, N16, Pf; };
+struct ChainMaps { CUtensorMap X, W0, W; };
 
 template <int CHAIN>
 static int chain_launch(const ChainMaps& m, const ChainArgs& a, cudaStream_t st) {
@@ -803,44 +548,9 @@ static int chain_launch(const ChainMaps& m, const ChainArgs& a, cudaStream_t st)
   const unsigned grid = (unsigned)std::min<int64_t>(tiles, sm_count());
   cudaError_t e = cudaFuncSetAttribute(chain_kernel<CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ChainCfg<CHAIN>::SMEM);
   if (e != cudaSuccess) return check_cuda(e, "update chain: cudaFuncSetAttribute");
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-  static long long* dbg = nullptr;
-  const bool timing = getenv("DPVO_B200_CHAIN_TIMING") != nullptr;
-  ChainArgs at = a;
-  if (timing) {
-    if (!dbg) cudaMalloc(&dbg, 256 * sizeof(long long));
-    cudaMemsetAsync(dbg, 0, 256 * sizeof(long long), st);
-    at.dbg = dbg;
-  }
-  chain_kernel<CHAIN><<<grid, chain_threads(CHAIN), ChainCfg<CHAIN>::SMEM, st>>>(m.X, m.W0, m.W, m.Net, m.N16, m.Pf, at);
-  DPVO_LAUNCH_CHECK("chain_kernel");
-  if (timing) {
-    long long hbuf[256];
-    cudaStreamSynchronize(st);
-    cudaMemcpy(hbuf, dbg, sizeof(hbuf), cudaMemcpyDeviceToHost);
-    long long t0 = 0;
-    for (int i = 0; i < 96; ++i) if (hbuf[i] && (!t0 || hbuf[i] < t0)) t0 = hbuf[i];
-    fprintf(stderr, "[chain %d, CTA 0, SM cycles from the first stamp] step: mma begin / issued | epilogue begin / done\n", CHAIN);
-    for (int t = 0; t < 3; ++t)
-      for (int l = 0; l < 8; ++l) {
-        const long long* r = hbuf + ((t * 8 + l) << 2);
-        if (r[0] || r[1] || r[2] || r[3])
-          fprintf(stderr, "   tile %d step %d: %8lld %8lld | %8lld %8lld\n", t, l, r[0] ? r[0] - t0 : -1, r[1] ? r[1] - t0 : -1, r[2] ? r[2] - t0 : -1, r[3] ? r[3] - t0 : -1);
-      }
-    for (int l = 0; l < 8; ++l) {
-      const long long* r = hbuf + 96 + l * 16;
-      if (!r[0]) continue;
-      fprintf(stderr, "   tile 1 epilogue %d chunk starts:", l);
-      for (int k = 0; k < 16 && r[k]; ++k) fprintf(stderr, " %lld", r[k] - t0);
-      fprintf(stderr, "\n");
-    }
-  }
-  return DPVO_OK;
-#else
-  chain_kernel<CHAIN><<<grid, chain_threads(CHAIN), ChainCfg<CHAIN>::SMEM, st>>>(m.X, m.W0, m.W, m.Net, m.N16, m.Pf, a);
+  chain_kernel<CHAIN><<<grid, CH_THREADS, ChainCfg<CHAIN>::SMEM, st>>>(m.X, m.W0, m.W, a);
   DPVO_LAUNCH_CHECK("chain_kernel");
   return DPVO_OK;
-#endif
 }
 
 static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
@@ -857,12 +567,10 @@ extern "C" int dpvo_update_corr_norm(const void* corr16, int64_t ld_corr, const 
   int rc = ch_tmap(&m.X, corr16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, E, CH_K0, ld_corr, 64, CH_M, CU_TENSOR_MAP_SWIZZLE_128B);
   if (!rc) rc = ch_tmap(&m.W0, W0, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, CH_DIM, CH_K0, CH_K0, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
   if (!rc) rc = ch_tmap(&m.W, W25, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.Net, net32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, E, CH_DIM, CH_DIM, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.N16, net16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, E, CH_DIM, CH_DIM, 32, 32, CU_TENSOR_MAP_SWIZZLE_64B);
   if (rc) return rc;
   ChainArgs a;
   memset(&a, 0, sizeof(a));
-  a.rows = E; a.state = net32; a.p = params; a.n_params = 7 * CH_DIM; a.inp16 = (const __half*)inp16; a.inp_index = inp_index;
+  a.rows = E; a.state = net32; a.state16 = (__half*)net16; a.p = params; a.n_params = 7 * CH_DIM; a.inp16 = (const __half*)inp16; a.inp_index = inp_index;
   return chain_launch<CHAIN_A>(m, a, (cudaStream_t)stream);
 }
 
@@ -876,13 +584,11 @@ extern "C" int dpvo_update_neighbor_mlp(const void* net16_in, const int64_t* ind
   ChainMaps m;
   memset(&m, 0, sizeof(m));
   int rc = ch_tmap(&m.W, Wab, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.Net, net32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, E, CH_DIM, CH_DIM, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.N16, net16_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, E, CH_DIM, CH_DIM, 32, 32, CU_TENSOR_MAP_SWIZZLE_64B);
   if (rc) return rc;
-  m.X = m.W; m.W0 = m.W; m.Pf = m.W;
+  m.X = m.W; m.W0 = m.W;
   ChainArgs a;
   memset(&a, 0, sizeof(a));
-  a.rows = E; a.state = net32; a.p = params; a.n_params = 2 * CH_DIM; a.x16 = (const __half*)net16_in; a.gidx = index;
+  a.rows = E; a.state = net32; a.state16 = (__half*)net16_out; a.p = params; a.n_params = 2 * CH_DIM; a.x16 = (const __half*)net16_in; a.gidx = index;
   return chain_launch<CHAIN_C>(m, a, (cudaStream_t)stream);
 }
 
@@ -902,9 +608,8 @@ extern "C" int dpvo_update_gru_heads(float* net32, const void* hij16, const int3
   ChainMaps m;
   memset(&m, 0, sizeof(m));
   int rc = ch_tmap(&m.W, W6, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 6 * CH_DIM, CH_DIM, CH_DIM, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.Net, net32, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, E, CH_DIM, CH_DIM, 32, 32, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
-  m.X = m.W; m.W0 = m.W; m.Pf = m.W; m.N16 = m.Net;
+  m.X = m.W; m.W0 = m.W;
   ChainArgs a;
   memset(&a, 0, sizeof(a));
   a.rows = E; a.state = net32; a.p = params; a.n_params = 14 * CH_DIM + 4; a.hij16 = (const __half*)hij16; a.group_of = group_of; a.hkk16 = (const __half*)hkk16; a.group_kk = group_kk; a.coords = coords;

@@ -14,6 +14,6 @@ void set_error(const char* fmt, ...) {
 }
 }  // namespace dpvo
 
-extern "C" const char* dpvo_version(void) { return "dpvo_b200 0.1 (sm_100a)"; }
+extern "C" const char* dpvo_version(void) { return "dpvo_b200 0.1 (sm_90a)"; }
 extern "C" const char* dpvo_last_error(void) { return dpvo::g_err; }
 extern "C" int64_t dpvo_launch_count(void) { return (int64_t)dpvo::g_launches.load(); }

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels behind include/dpvo_b200.h.
+// Shared helpers for the sm_90a kernels behind include/dpvo_b200.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -47,8 +47,8 @@ inline int sm_count() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 132;
   }
   return n;
 }

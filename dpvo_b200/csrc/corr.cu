@@ -1,4 +1,4 @@
-// Patch <-> frame local correlation (altcorr) for sm_100a.
+// Patch <-> frame local correlation (altcorr) for sm_90a.
 //
 // Replaces dpvo/altcorr/correlation_kernel.cu:82-136 (raw 8x8 taps), :221-230 (bilinear blend,
 // ~15 ATen launches over a [E,8,8,3,3] temporary) and :232 (permute) with ONE launch.
@@ -266,7 +266,7 @@ corr_fwd_mma(const CorrArgs a) {
   extern __shared__ __align__(16) unsigned char mma_smem_raw[];
   MmaWarpSmem& sm = reinterpret_cast<MmaWarpSmem*>(mma_smem_raw)[threadIdx.x >> 5];
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  // list mode (edges the tcgen05 kernel could not box): an item is ONE patch pixel of a listed edge -- its own 8x8
+  // list mode (edges the wgmma kernel could not box): an item is ONE patch pixel of a listed edge -- its own 8x8
   // window on both levels and its 49 outputs -- so that the nine passes of a stretched edge spread over nine warps
   // instead of serialising in one (a handful of such edges used to cost 30 us of single-warp latency)
   const int64_t nitems = a.list ? (int64_t)*a.list_count * 9 : (int64_t)a.B * a.M;
@@ -793,7 +793,7 @@ extern "C" int dpvo_corr_forward_pyramid2(const void* fmap1, const int64_t* fmap
   a.coords = coords; a.ii = ii; a.jj = jj; a.out = out; a.out_stride = 2;
   a.out_offset[0] = 0; a.out_offset[1] = 1; a.nlev = 2; a.B = B; a.M = M; a.C = C; a.P = P; a.R = radius;
   a.out_row = out_row_stride;
-  // tcgen05 + TMA path: fp16 channels-last rings, batch 1, caller-provided scratch for the edge list
+  // wgmma + TMA path: fp16 channels-last rings, batch 1, caller-provided scratch for the edge list
   if (workspace && workspace_bytes >= dpvo_corr_pyramid2_workspace_bytes(M) && B == 1 && S1 > 0 && S2 > 0 &&
       mma_eligible(a, dtype)) {
     const int rc = corr_tc_forward(fmap1, a.s1, S1, fmap2_l0, a.s2[0], H0, W0, fmap2_l1, a.s2[1], H1, W1, S2, lvl1_div, coords, ii, jj,

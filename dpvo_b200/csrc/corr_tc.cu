@@ -1,4 +1,4 @@
-// Patch <-> frame correlation on tcgen05 + TMA (sm_100a), both pyramid levels in one launch.
+// Patch <-> frame correlation on wgmma + TMA (sm_90a), both pyramid levels in one launch.
 //
 // Per edge and level the nine 8x8 tap windows are covered by one (8+sx) x (8+sy) pixel box, sx/sy = spread of the
 // nine anchors (2 at unit patch scale, 0..1 on the quarter-resolution level).  Boxes of up to 128 pixels on level 0
@@ -11,14 +11,15 @@
 //     which is exactly the reference's "out-of-bounds taps contribute 0" (correlation_kernel.cu:121-122)
 //     -- no predicates, no per-lane address arithmetic
 //   * the landed tile IS the canonical K-major SWIZZLE_128B operand: rows = box pixels, K = channels.
-//     tcgen05.mma (M=128 rows incl. padding, N=16 patch pixels incl. padding, K=16 x 8) accumulates
-//     <box pixel, patch pixel> for all pairs into 16 TMEM columns per level
-//   * groups of four epilogue warps pull the accumulator with tcgen05.ld (lane = box pixel), transpose it through
-//     shared memory and apply the bilinear blend + (x,y) ordering + level interleave, writing fp16 pairs
-// Roles per CTA (persistent, one per SM): warps 0-1 producers (alternate edges, coords prefetched two edges ahead), warp 2 MMA
-// issuer, warps 3.. epilogue (TC_NG groups of four); a 3-stage shared-memory ring and a TC_NG-stage TMEM ring
-// keep TMA, tensor pipe and epilogue overlapped.
+//     Two wgmma.m64n16k16 per k-step (rows 0-63 and 64-127 incl. padding, N=16 patch pixels incl. padding, K=16 x 8)
+//     accumulate <box pixel, patch pixel> for all pairs in the registers of the warpgroup that owns the edge
+//   * that warpgroup transposes the accumulator through shared memory and applies the bilinear blend + (x,y) ordering
+//     + level interleave, writing fp16 pairs
+// Roles per CTA (persistent, one per SM): warps 0.. consumers (TC_NG warpgroups taking edges round-robin, each issuing
+// its own MMAs), then TC_NP producer warps (alternate edges, coords prefetched two edges ahead); one shared-memory
+// stage per warpgroup, refilled as soon as its MMAs have retired, keeps TMA, tensor pipe and the blends overlapped.
 #include "common.cuh"
+#include "tc.cuh"
 #include <cuda.h>
 #include <cstring>
 #include <cmath>
@@ -34,14 +35,16 @@ constexpr int TC_WIN1_BYTES = 13 * 1024;       // level 1: <= 100 rows, rounded 
 constexpr int TC_PAT_BYTES = 16 * 128;         // patch half: 16 rows (9 loaded) x 64 channels
 constexpr int TC_PAT_TX = 9 * 128;
 constexpr int TC_STAGE_BYTES = 2 * TC_WIN0_BYTES + 2 * TC_WIN1_BYTES + 2 * TC_PAT_BYTES;
-constexpr int TC_STAGES = 3;
-constexpr int TC_NG = 2;                       // epilogue groups == TMEM accumulator stages
-constexpr int TC_META = 16;                    // meta ring (> smem stages + accumulator stages + 1)
+// one stage per consumer warpgroup: a stage is then always consumed by the same group, in order (with stages shared
+// round-robin a group could wait on a stage two phases ahead of it, which a parity wait cannot tell apart)
+constexpr int TC_STAGES = 2;
+constexpr int TC_NG = 2;                       // consumer warpgroups
+constexpr int TC_META = 16;                    // meta ring (> smem stages + consumer groups + 1)
 constexpr int TC_NP = 2;                       // producer warps (alternate edges; must not exceed TC_STAGES, see the kernel)
-constexpr int TC_THREADS = (TC_NP + 1 + 4 * TC_NG) * 32;
+constexpr int TC_THREADS = (4 * TC_NG + TC_NP) * 32;
 static_assert(TC_NP <= TC_STAGES, "a producer may run at most one phase ahead of the stage it waits for");
+static_assert(TC_STAGES == TC_NG, "each consumer warpgroup owns one stage");
 constexpr int TC_RAWP = 129;                   // floats per patch pixel row of the transposed accumulator
-static_assert(TC_NG == 1 || TC_NG == 2 || TC_NG == 4, "TMEM allocation must be a power of two >= 32 columns");
 static_assert(TC_STAGE_BYTES % 1024 == 0, "stages must keep the 1024 B swizzle alignment");
 
 struct TcMaps {
@@ -67,8 +70,7 @@ struct __align__(16) TcMeta {   // what the producer hands to the other roles, p
 };
 
 struct TcBars {
-  uint64_t full[TC_STAGES], empty[TC_STAGES], tmem_full[TC_NG], tmem_empty[TC_NG];
-  uint32_t tmem_base;
+  uint64_t full[TC_STAGES], empty[TC_STAGES];
 };
 
 __device__ __forceinline__ uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -97,29 +99,6 @@ __device__ __forceinline__ void tc_tma_2d(uint32_t dst, const void* tmap, int c0
                "l"(tmap), "r"(c0), "r"(c1), "r"(tc_smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tc_commit_(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(tc_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc),
-      "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld16_(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ uint64_t tc_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// D fp32, A/B fp16 K-major, N = 16, M = 128
-constexpr uint32_t TC_IDESC = (1u << 4) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-
 // level-1 coordinate: x / div (correlation is sampled at coords / 4, dpvo.py:206); a power-of-two divisor is
 // applied as an exact multiplication
 template <bool POW2> __device__ __forceinline__ float tc_level1(float x, const TcArgs& a) { return POW2 ? x * a.inv1 : x / a.div1; }
@@ -137,20 +116,14 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) { tc_mbar_init(&bars->full[s], 1); tc_mbar_init(&bars->empty[s], 1); }
-    for (int i = 0; i < TC_NG; ++i) { tc_mbar_init(&bars->tmem_full[i], 1); tc_mbar_init(&bars->tmem_empty[i], 128); }
+    // a stage is handed back by lane 0 of each of the four warps of the consuming warpgroup
+    for (int s = 0; s < TC_STAGES; ++s) { tc_mbar_init(&bars->full[s], 1); tc_mbar_init(&bars->empty[s], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (warp == TC_NP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tc_smem_u32(&bars->tmem_base)), "n"(TC_NG * 32));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp < TC_NP) {
+  if (warp >= 4 * TC_NG) {
+    const int pw = warp - 4 * TC_NG;                 // producer index
     // ================================================================================ producers
     // TC_NP warps take edges alternately.  Parity waits stay unambiguous because a producer that has issued
     // edge i (stage free => MMA of edge i - STAGES retired) next waits for the stage of edge i + NP, whose
@@ -167,10 +140,10 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
     };
     float c0, c1, c2; int i0, i1, i2;
     const int G = gridDim.x * TC_NP;
-    const int e_first = blockIdx.x + warp * gridDim.x;
+    const int e_first = blockIdx.x + pw * gridDim.x;
     fetch(e_first, c0, i0);
     fetch(e_first + G, c1, i1);
-    uint32_t it = warp;
+    uint32_t it = pw;
     for (int e = e_first; e < a.M; e += G, it += TC_NP) {
       fetch(e + 2 * G, c2, i2);
       const uint32_t s = it % TC_STAGES, ph = (it / TC_STAGES) & 1;
@@ -223,52 +196,16 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
       __syncwarp();
       c0 = c1; i0 = i1; c1 = c2; i1 = i2;
     }
-  } else if (warp == TC_NP) {
-    // ================================================================================ MMA issuer
-    uint32_t it = 0;
-    for (int e = blockIdx.x; e < a.M; e += gridDim.x, ++it) {
-      const uint32_t s = it % TC_STAGES, ph = (it / TC_STAGES) & 1;
-      const uint32_t acc = it % TC_NG, aph = (it / TC_NG) & 1;
-      tc_mbar_wait(&bars->tmem_empty[acc], aph ^ 1);
-      tc_mbar_wait(&bars->full[s], ph);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-      if (lane == 0) {
-        if (meta[it % TC_META].uni) {
-          const uint32_t st = tc_smem_u32(stages + (size_t)s * TC_STAGE_BYTES);
-          const uint32_t pa = st + 2 * TC_WIN0_BYTES + 2 * TC_WIN1_BYTES;
-#pragma unroll
-          for (int lev = 0; lev < 2; ++lev) {
-            const uint32_t d = tmem_base + acc * 32 + lev * 16;
-            const uint32_t wa = lev == 0 ? st : st + 2 * TC_WIN0_BYTES;
-            const uint32_t wstep = lev == 0 ? TC_WIN0_BYTES : TC_WIN1_BYTES;
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-              const uint64_t ad = tc_desc_sw128(wa + half * wstep);
-              const uint64_t bd = tc_desc_sw128(pa + half * TC_PAT_BYTES);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) tc_mma_(d, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), TC_IDESC, (half | k) != 0);
-            }
-          }
-        }
-        tc_commit_(&bars->empty[s]);
-        tc_commit_(&bars->tmem_full[acc]);
-      }
-      __syncwarp();
-    }
   } else {
-    // ================================================================================ epilogue
-    // TC_NG groups of four warps take edges round-robin; a group owns one TMEM accumulator stage and one
-    // transpose tile.  Thread -> (patch pixel p, taps t0 + 14k): constant for the kernel, so weights / base
-    // are read once per edge.
-    const int eg = (warp - TC_NP - 1) >> 2;
-    const int et = ((warp - TC_NP - 1) & 3) * 32 + lane;
-    const int quarter = warp & 3;                    // TMEM lane quarter this warp may read
-    const int r = quarter * 32 + lane;               // box pixel owned by this thread
+    // ================================================================================ consumers
+    // TC_NG warpgroups take edges round-robin; a group issues the MMAs of its edge, owns one transpose tile and
+    // hands the stage back as soon as its MMAs have retired.  Thread -> (patch pixel p, taps t0 + 14k): constant for the
+    // kernel, so weights / base are read once per edge.
+    const int eg = warp >> 2, wq = warp & 3;
+    const int et = threadIdx.x & 127;
     // Thread -> (patch pixel p, tap row y, half of the tap columns): the 7 taps of a row share their bilinear corners
     // (tap x uses columns x, x+1 of rows y, y+1), so a thread that owns a run of taps reads each window value once --
-    // 36 shared-memory loads per (p, y) and level pair instead of 56 when every tap was blended on its own; the kernel
-    // is bound by shared-memory bandwidth (TMA fills + UMMA operand reads + these loads), and the loads of the blend
-    // were replayed 3.4x by bank conflicts (ncu: 14.9 M conflict wavefronts of 21.1 M).
+    // 36 shared-memory loads per (p, y) and level pair instead of 56 when every tap was blended on its own.
     const int u = et % 63, hx = et / 63;             // hx = 0: tap columns 0..3, hx = 1: tap columns 4..6
     const int p = u % 9, yrow = u / 9;
     const int x0 = hx * 4, nx = 4 - hx;
@@ -276,10 +213,10 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
     uint32_t it = 0;
     for (int e = blockIdx.x; e < a.M; e += gridDim.x, ++it) {
       if ((int)(it % TC_NG) != eg) continue;
-      const uint32_t aph = (it / TC_NG) & 1;
+      const uint32_t s = it % TC_STAGES, ph = (it / TC_STAGES) & 1;
       const TcMeta& mt = meta[it % TC_META];
       // this thread's patch pixel: anchor and bilinear weights per level (independent of the box, so the
-      // loads and the arithmetic overlap the wait for the accumulator)
+      // loads and the arithmetic overlap the wait for the stage)
       const float xr = __ldg(a.coords + (int64_t)e * 18 + p), yr = __ldg(a.coords + (int64_t)e * 18 + 9 + p);
       int ax[2], ay[2];
       float4 w[2];
@@ -290,28 +227,55 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
         const float fx = x - floorf(x), fy = y - floorf(y);
         w[lev] = make_float4((1.f - fx) * (1.f - fy), fx * (1.f - fy), (1.f - fx) * fy, fx * fy);
       }
-      tc_mbar_wait(&bars->tmem_full[eg], aph);
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+      tc_mbar_wait(&bars->full[s], ph);
       const int4 org = *reinterpret_cast<const int4*>(&mt.bx[0]);        // bx0 bx1 by0 by1
       const int4 shp = *reinterpret_cast<const int4*>(&mt.pitch[0]);     // pitch0 pitch1 uni edge
       if (!shp.z) {                                   // finished by the list kernel: just hand the stage back
-        asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-        tc_mbar_arrive(&bars->tmem_empty[eg]);
+        __syncwarp();
+        if (lane == 0) tc_mbar_arrive(&bars->empty[s]);
         continue;
       }
-      uint32_t v0[16], v1[16];
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + eg * 32;
-      tc_ld16_(taddr, v0);
-      tc_ld16_(taddr + 16, v1);
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-      tc_mbar_arrive(&bars->tmem_empty[eg]);
-      // transpose: raw[lev][p][r]   (rows past the box are padding)
+      float acc[2][2][8];                             // [level][rows 0-63 | 64-127][fragment]
+      {
+        const uint32_t st = tc_smem_u32(stages + (size_t)s * TC_STAGE_BYTES);
+        const uint32_t pa = st + 2 * TC_WIN0_BYTES + 2 * TC_WIN1_BYTES;
+        wgmma_fence();
 #pragma unroll
-      for (int pp = 0; pp < 9; ++pp) {
-        rw[pp * TC_RAWP + r] = __uint_as_float(v0[pp]);
-        rw[(9 + pp) * TC_RAWP + r] = __uint_as_float(v1[pp]);
+        for (int lev = 0; lev < 2; ++lev) {
+          const uint32_t wa = lev == 0 ? st : st + 2 * TC_WIN0_BYTES;
+          const uint32_t wstep = lev == 0 ? TC_WIN0_BYTES : TC_WIN1_BYTES;
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const uint64_t bd = wgmma_desc_sw128(pa + half * TC_PAT_BYTES);
+#pragma unroll
+            for (int rh = 0; rh < 2; ++rh) {
+              const uint64_t ad = wgmma_desc_sw128(wa + half * wstep + rh * 64 * 128);
+#pragma unroll
+              for (int k = 0; k < 4; ++k) wgmma_m64n16k16(acc[lev][rh], ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (half | k) != 0);
+            }
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int lev = 0; lev < 2; ++lev)
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) wgmma_fence_regs(acc[lev][rh]);
+        __syncwarp();
+        if (lane == 0) tc_mbar_arrive(&bars->empty[s]);
       }
+      // transpose: raw[lev][p][r]   (rows past the box are padding); fragment i of row half rh: box pixel
+      // r = 64 rh + 16 wq + lane / 4 + 8 ((i / 2) % 2), patch pixel 8 (i / 4) + 2 (lane % 4) + i % 2
+#pragma unroll
+      for (int lev = 0; lev < 2; ++lev)
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const int r = rh * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+            const int pp = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+            if (pp < 9) rw[(lev * 9 + pp) * TC_RAWP + r] = acc[lev][rh][i];
+          }
       asm volatile("bar.sync %0, 128;\n" ::"r"(1 + eg) : "memory");
       if (et < 126) {
         __half2* orow = reinterpret_cast<__half2*>(a.out + (int64_t)e * a.out_row);
@@ -338,12 +302,6 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
     }
   }
 
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  if (warp == TC_NP) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "n"(TC_NG * 32));
-  }
 }
 
 typedef CUresult (*TcEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,

@@ -1,42 +1,38 @@
-// Dense layers of the update operator on the 5th-generation tensor cores (tcgen05 + TMEM).
+// Dense layers of the update operator on the Hopper tensor cores (wgmma, sm_90a).
 //
 //   Y[rows, N] = epilogue( X[rows, K] @ W[N, K]^T + bias )        fp16 operands, fp32 accumulate
 //
-// Persistent, warp-specialised kernel (one CTA per SM):
-//   warps 0-3  epilogue     tcgen05.ld the 128 x 192 fp32 accumulator tile out of TMEM (each warp owns
-//                           its 32-lane quarter), bias / activation / residual, fp16 or fp32 store
-//   warp  4    MMA issuer   one elected thread issues tcgen05.mma.cta_group::1.kind::f16
-//                           (M=128, N=192, K=16) on shared-memory descriptors, accumulators in TMEM,
-//                           double buffered (2 x 192 of the 512 columns) so the epilogue of tile i
-//                           overlaps the main loop of tile i+1; tcgen05.commit releases smem stages and
-//                           publishes finished accumulators through mbarriers
-//   warps 5-8  producers    stage X and W k-blocks (64 halves = one 128-byte swizzle atom per row) into a
-//                           5-deep shared-memory ring with 16-byte cp.async in the SWIZZLE_128B K-major
-//                           layout the UMMA descriptors expect; X rows may be gathered through an index
+// Persistent, warp-specialised kernel (one CTA per SM), tiles of 128 x 192:
+//   warps 0-7  consumers    two warpgroups; warpgroup g issues wgmma.m64n192k16 for rows 64 g .. 64 g + 63 of the tile
+//                           on shared-memory descriptors, keeps the 64 x 192 fp32 accumulator in registers and runs
+//                           the epilogue (bias / activation / residual / gate, fp16 or fp32 store) straight from them
+//   warps 8-11 producers    stage X and W k-blocks (64 halves = one 128-byte swizzle atom per row) into a
+//                           5-deep shared-memory ring in the SWIZZLE_128B K-major layout the descriptors expect: by TMA
+//                           (one elected thread), or with 16-byte cp.async when X rows are gathered through an index
 //                           (net.py:84-85 `net[:, ix]` with mask) so the gather never touches HBM twice
-// The weights (<= 0.7 MB per layer) stay L2 resident; X is read once per 192-column half.
+// The weights (<= 0.7 MB per layer) stay L2 resident; X is read once per 192-column slice.
 #include "common.cuh"
 #include "tc.cuh"
 #include <cuda.h>          // CUtensorMap types only; the encoder is fetched from the driver at run time
 
 namespace dpvo {
 
-constexpr int GM_M = 128;            // rows per tile == TMEM lanes
-constexpr int GM_N = 192;            // columns per tile (UMMA N, multiple of 16)
+constexpr int GM_M = 128;            // rows per tile (two warpgroups of 64)
+constexpr int GM_N = 192;            // columns per tile (wgmma N)
 constexpr int GM_K = 64;             // halves per k-block: 128 bytes, one swizzle atom
-constexpr int GM_UK = 16;            // UMMA K for 16-bit operands
+constexpr int GM_UK = 16;            // wgmma K for 16-bit operands
 constexpr int GM_STAGES = 5;
-constexpr int GM_LOOK = 4;           // cp.async groups in flight per producer thread (gather mode, < GM_STAGES)
-constexpr int GM_EPI_WARPS = 8;      // two warps per TMEM lane quarter, each owning half of the tile's columns
-constexpr int GM_EPI_THREADS = GM_EPI_WARPS * 32, GM_PROD_THREADS = 128;
-constexpr int GM_MMA_WARP = GM_EPI_WARPS;
-constexpr int GM_THREADS = GM_EPI_THREADS + 32 + GM_PROD_THREADS;
+// cp.async groups in flight per producer thread (gather mode).  A consumer returns the stage of k-block i - 1 only
+// after it has issued the MMAs of k-block i, and a producer signals k-block i only once it has issued k-block
+// i + LOOK, so LOOK must stay below ring depth - 1.
+constexpr int GM_LOOK = GM_STAGES - 2;
+constexpr int GM_CONS_WARPS = 8;     // two consumer warpgroups
+constexpr int GM_CONS_THREADS = GM_CONS_WARPS * 32, GM_PROD_THREADS = 128;
+constexpr int GM_THREADS = GM_CONS_THREADS + GM_PROD_THREADS;
 constexpr int GM_A_BYTES = GM_M * 128, GM_B_BYTES = GM_N * 128;
-constexpr int GM_TMEM_COLS = 512;
 constexpr int GM_WS_MAXKB = 6;       // weight-stationary mode: K <= 384 (6 k-blocks of the weight slice stay in smem)
 constexpr int GM_WS_ASTAGES = 4;     // activation ring depth in weight-stationary mode
 constexpr int GM_OUT_F16 = 0, GM_OUT_F32 = 1, GM_OUT_F32_F16 = 2;   // result: fp16 | fp32 | fp32 plus an fp16 copy
-constexpr int GM_STG_FLOATS = 32 * 16; // per-warp epilogue staging tile: 32 rows x 16 columns fp32 (2 KB)
 
 struct GemmArgs {
   const __half* X; int64_t ldx;
@@ -49,40 +45,19 @@ struct GemmArgs {
   __half* Y16;                 // optional fp16 copy of the result (row stride ldy16)
   int64_t ldy16;
   int64_t rows; int N; int K; int epilogue;
-  int prefetch;                // residual / gate tensor maps are valid: prefetch their tiles into L2
-  int exp_flags;               // perf experiments only (DPVO_B200_GEMM_EXP): 1 no residual load, 2 no gate load, 4 no Y store, 8 no Y16 store
-  long long* dbg;              // optional per-role timestamps of CTA 0 (DPVO_B200_GEMM_TIMING), NULL = off
 };
 
-// instruction descriptor (InstrDescriptor): D fp32, A/B fp16 K-major, N>>3 at bit 17, M>>4 at bit 24
-constexpr uint32_t GM_IDESC = (1u << 4) | ((uint32_t)(GM_N >> 3) << 17) | ((uint32_t)(GM_M >> 4) << 24);
-
 struct GemmBars {
-  uint64_t full[GM_STAGES], empty[GM_STAGES], tmem_full[2], tmem_empty[2], wfull;
-  uint32_t tmem_base;
+  uint64_t full[GM_STAGES], empty[GM_STAGES], wfull;
 };
 
 // GATHER = false: X and W tiles arrive by TMA (one elected thread, hardware swizzle, OOB rows zero).
 // GATHER = true : X rows are fetched through an index with cp.async by 128 producer threads (W too).
 // WS = true (weight stationary, K <= 384): a CTA works on ONE 192-column slice of the layer for its whole
-// life, loads that slice of W once (<= 144 KB, resident) and streams only activation tiles.  Streaming both
-// operands needs (128+192)*128 B per 128x192x64 MACs = 107 B/clk/SM at the tensor-pipe rate, 2.5x what L2
-// delivers per SM; with W resident it is 43 B/clk/SM.
-// debug timestamps: dbg[role * 16 + tile] for the first 16 tiles of CTA 0.  roles: 0 MMA tile begin, 1 MMA accumulator
-// stage free, 2 MMA tile issued, 3 epilogue accumulator ready, 4 epilogue tile done, 5 kernel begin / weights landed
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-#define GM_STAMP(role, t) do { if (a.dbg && blockIdx.x == 0 && lane == 0 && (t) < 16) a.dbg[(role) * 16 + (t)] = clock64(); } while (0)
-#define GM_EXP(bit) (a.exp_flags & (bit))
-#else
-#define GM_STAMP(role, t) do { } while (0)
-#define GM_EXP(bit) false
-#endif
-
+// life, loads that slice of W once (<= 144 KB, resident) and streams only activation tiles.
 template <bool GATHER, bool WS, int EPI, int OUT>
 __global__ void __launch_bounds__(GM_THREADS, 1)
-linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmG,
-                  const __grid_constant__ CUtensorMap tmY, const GemmArgs a) {
+linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs a) {
   extern __shared__ unsigned char gm_smem_raw[];
   constexpr int NST = WS ? GM_WS_ASTAGES : GM_STAGES;
   // 1024-byte alignment by pointer arithmetic on the shared array (an integer round trip would demote every
@@ -90,8 +65,7 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   unsigned char* base = gm_smem_raw + ((1024u - (smem_u32(gm_smem_raw) & 1023u)) & 1023u);
   unsigned char* sA = base;
   unsigned char* sB = base + NST * GM_A_BYTES;
-  unsigned char* sStage = sB + (WS ? GM_WS_MAXKB : GM_STAGES) * GM_B_BYTES;       // [GM_EPI_WARPS][GM_STG_FLOATS] fp32
-  GemmBars* bars = reinterpret_cast<GemmBars*>(sStage + GM_EPI_WARPS * GM_STG_FLOATS * 4);
+  GemmBars* bars = reinterpret_cast<GemmBars*>(sB + (WS ? GM_WS_MAXKB : GM_STAGES) * GM_B_BYTES);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles_n = (a.N + GM_N - 1) / GM_N;
@@ -100,35 +74,16 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int KB = a.K / GM_K;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < GM_STAGES; ++s) { mbar_init(&bars->full[s], GATHER ? GM_PROD_THREADS : 1); mbar_init(&bars->empty[s], 1); }
+    for (int s = 0; s < GM_STAGES; ++s) { mbar_init(&bars->full[s], GATHER ? GM_PROD_THREADS : 1); mbar_init(&bars->empty[s], GM_CONS_WARPS); }
     mbar_init(&bars->wfull, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&bars->tmem_full[i], 1); mbar_init(&bars->tmem_empty[i], GM_EPI_THREADS); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (warp == GM_MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&bars->tmem_base)), "n"(GM_TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  // Optional (DPVO_B200_GEMM_PREFETCH=1): pull the residual / gate tiles the epilogue of a tile will read into L2
-  // while its MMAs run.  Measured neutral to slightly negative once the epilogue prefetches a chunk ahead, so off
-  // by default.
-  auto prefetch_epilogue_operands = [&](int m0, int n0) {
-    if constexpr (EPI == DPVO_EPI_RESADD || EPI == DPVO_EPI_GATEDRES) {
-      if (a.prefetch) {
-        tma_prefetch_l2_2d(&tmR, n0, m0);
-        if constexpr (EPI == DPVO_EPI_GATEDRES) tma_prefetch_l2_2d(&tmG, n0, m0);
-      }
-    }
-  };
-  if (warp > GM_MMA_WARP) {
+  if (warp >= GM_CONS_WARPS) {
     // =========================================================================== producers
     if constexpr (!GATHER) {
-      if (warp == GM_MMA_WARP + 1 && lane == 0) {
+      if (warp == GM_CONS_WARPS && lane == 0) {
         uint32_t it = 0;
         if constexpr (WS) {                  // the CTA's weight slice, once
           const int n0 = (int)(blockIdx.x % n_tiles_n) * GM_N;
@@ -138,7 +93,6 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
           const int m0 = (int)((tile / n_tiles_n) * GM_M);
           const int n0 = (int)(tile % n_tiles_n) * GM_N;
-          prefetch_epilogue_operands(m0, n0);
           for (int kb = 0; kb < KB; ++kb, ++it) {
             const uint32_t s = it % NST, ph = (it / NST) & 1;
             mbar_wait(&bars->empty[s], ph ^ 1);
@@ -149,9 +103,9 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     } else {
-      const int pt = threadIdx.x - (GM_EPI_THREADS + 32);
+      const int pt = threadIdx.x - GM_CONS_THREADS;
       uint32_t it = 0;                       // k-block counter over all tiles of this CTA
-      constexpr int LOOK = WS ? GM_WS_ASTAGES - 1 : GM_LOOK;
+      constexpr int LOOK = WS ? GM_WS_ASTAGES - 2 : GM_LOOK;
       if constexpr (WS) {
         if (pt == 0) {
           const int n0 = (int)(blockIdx.x % n_tiles_n) * GM_N;
@@ -175,9 +129,7 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       };
       fetch_rows(blockIdx.x);
       for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t m0 = (tile / n_tiles_n) * GM_M;
         const int n0 = (int)(tile % n_tiles_n) * GM_N;
-        if (pt == 0) prefetch_epilogue_operands((int)m0, n0);
         const __half* arow[8]; uint32_t aoff[8], abytes[8];
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -221,263 +173,72 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       fence_proxy_async();
       for (uint32_t j = (it >= LOOK ? it - LOOK : 0); j < it; ++j) mbar_arrive(&bars->full[j % NST]);
     }
-  } else if (warp == GM_MMA_WARP) {
-    // =========================================================================== MMA issuer
-    uint32_t it = 0, tcount = 0;
-    GM_STAMP(5, 0);
+  } else {
+    // =========================================================================== consumers: MMA + epilogue
+    const int wg = warp >> 2, wq = warp & 3;
+    uint32_t it = 0;
+    float acc[96];
     if constexpr (WS) mbar_wait(&bars->wfull, 0);
-    GM_STAMP(5, 1);
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-      const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-      GM_STAMP(0, tcount);
-      mbar_wait(&bars->tmem_empty[acc], aph ^ 1);
-      tc_fence_after();
-      GM_STAMP(1, tcount);
-      const uint32_t d_tmem = tmem_base + acc * GM_N;
+    auto release = [&](uint32_t s) { __syncwarp(); if (lane == 0) mbar_arrive(&bars->empty[s]); };
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      const int64_t m0 = (tile / n_tiles_n) * GM_M;
+      const int n0 = (int)(tile % n_tiles_n) * GM_N;
+      uint32_t prev = 0;
       for (int kb = 0; kb < KB; ++kb, ++it) {
         const uint32_t s = it % NST, ph = (it / NST) & 1;
         mbar_wait(&bars->full[s], ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint64_t ad = umma_desc_sw128(smem_u32(sA + s * GM_A_BYTES));
-          const uint64_t bd = umma_desc_sw128(smem_u32(sB + (WS ? kb : (int)s) * GM_B_BYTES));
+        const uint64_t ad = wgmma_desc_sw128(smem_u32(sA + s * GM_A_BYTES + wg * 64 * 128));
+        const uint64_t bd = wgmma_desc_sw128(smem_u32(sB + (WS ? kb : (int)s) * GM_B_BYTES));
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < GM_K / GM_UK; ++k)
-            tc_mma_f16(d_tmem, ad + (uint64_t)(k * GM_UK * 2 / 16), bd + (uint64_t)(k * GM_UK * 2 / 16), GM_IDESC, (kb | k) != 0);
-          tc_commit(&bars->empty[s]);                      // smem stage reusable once these MMAs retire
-          if (kb == KB - 1) tc_commit(&bars->tmem_full[acc]);   // accumulator complete
-        }
-        __syncwarp();
+        for (int k = 0; k < GM_K / GM_UK; ++k) wgmma_m64n192k16(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_commit();
+        if (kb > 0) { wgmma_wait<1>(); release(prev); }     // the previous k-block's MMAs have read their stage
+        prev = s;
       }
-      GM_STAMP(2, tcount);
-    }
-  } else {
-    // =========================================================================== epilogue
-    // TMEM hands every thread one accumulator ROW (lane = row); a warp may only touch the lane quarter
-    // warp % 4.  Eight warps share a tile: warps q and q+4 own the left / right 96 columns of quarter q.
-    // Row-per-thread global accesses cost one LSU wavefront per lane (32 rows x 16 B scattered over 32
-    // lines) and made the fused residual layers 3x slower than their MMAs, so every 32 x 16 accumulator
-    // block is transposed through a 2 KB per-warp staging tile (16-byte chunks, XOR-swizzled: conflict-free
-    // both ways) and all global traffic -- bias, residual, gate, fp32 / fp16 results -- is issued with
-    // lane = (row, 4 consecutive columns): 8 rows x 64 contiguous bytes per instruction.
-    uint32_t tcount = 0;
-    const int quarter = warp & 3, half = warp >> 2;
-    if constexpr (OUT == GM_OUT_F16 && EPI != DPVO_EPI_RESADD && EPI != DPVO_EPI_GATEDRES) {
-      // ---- fp16 result without epilogue operands: TMEM -> registers -> shared -> TMA store --------------------
-      // Every lane owns one accumulator row (the TMEM layout as it is): 32 columns at a time are biased / activated
-      // / packed in registers and written as four 16-byte chunks into a 32 x 32 fp16 staging tile in the
-      // SWIZZLE_64B pattern of the result's tensor map (chunk ^ ((row >> 1) & 3): the eight lanes of a
-      // shared-memory wavefront hit eight different 16-byte slots), and one lane hands the tile to the TMA unit.
-      // No transposition round trip, no per-lane global addressing, no LSU wavefronts for the result: the
-      // epilogue of a 128 x 192 tile dropped from ~4.7 k to the ~1 k cycles the MMAs of the next tile hide.
-      unsigned char* stile = sStage + warp * (GM_STG_FLOATS * 4);          // 2 KB per warp, 1024-byte aligned base
-      const uint32_t stile_u = smem_u32(stile);
-      const uint32_t my_row = stile_u + lane * 64;
-      const int sw = (lane >> 1) & 3;
-      for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-        const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-        const int m0 = (int)((tile / n_tiles_n) * GM_M) + quarter * 32;
-        const int n0 = (int)(tile % n_tiles_n) * GM_N + half * (GM_N / 2);
-        const int nch = min(GM_N / 2 / 32, max(0, (a.N - n0) / 32));       // valid 32-column chunks (N % 32 == 0)
-        mbar_wait(&bars->tmem_full[acc], aph);
-        tc_fence_after();
-        GM_STAMP(3, tcount);
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * GM_N + half * (GM_N / 2);
-        uint32_t r[32];
-        if (nch > 0) tc_ld32(taddr, r);
-        else { tc_fence_before(); mbar_arrive(&bars->tmem_empty[acc]); }
-#pragma unroll 1
-        for (int c = 0; c < nch; ++c) {
-          const int col0 = n0 + c * 32;
-          float4 bv[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j)                                     // same address in every lane: one broadcast wavefront each
-            bv[j] = a.bias ? __ldg(reinterpret_cast<const float4*>(a.bias + col0) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-          tc_ld_wait();
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            v[4 * j] = __uint_as_float(r[4 * j]) + bv[j].x; v[4 * j + 1] = __uint_as_float(r[4 * j + 1]) + bv[j].y;
-            v[4 * j + 2] = __uint_as_float(r[4 * j + 2]) + bv[j].z; v[4 * j + 3] = __uint_as_float(r[4 * j + 3]) + bv[j].w;
-          }
-          if (c + 1 < nch) tc_ld32(taddr + (c + 1) * 32, r);
-          else { tc_fence_before(); mbar_arrive(&bars->tmem_empty[acc]); }     // last read of this accumulator stage
-          bool sig = EPI == DPVO_EPI_SIGMOID, relu = EPI == DPVO_EPI_RELU;
-          if constexpr (EPI == DPVO_EPI_SIGMOID_RELU) { sig = col0 < (a.N >> 1); relu = !sig; }   // uniform over the chunk
-          if (sig) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __fdividef(1.0f, 1.0f + __expf(-v[j]));
-          } else if (relu) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          uint4 o[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            *reinterpret_cast<__half2*>(&o[j].x) = __floats2half2_rn(v[8 * j], v[8 * j + 1]);
-            *reinterpret_cast<__half2*>(&o[j].y) = __floats2half2_rn(v[8 * j + 2], v[8 * j + 3]);
-            *reinterpret_cast<__half2*>(&o[j].z) = __floats2half2_rn(v[8 * j + 4], v[8 * j + 5]);
-            *reinterpret_cast<__half2*>(&o[j].w) = __floats2half2_rn(v[8 * j + 6], v[8 * j + 7]);
-          }
-          if (lane == 0) bulk_wait_read<0>();                // the previous store has finished reading the staging tile
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};\n" ::"r"(my_row + ((j ^ sw) << 4)), "r"(o[j].x), "r"(o[j].y), "r"(o[j].z), "r"(o[j].w) : "memory");
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) { tma_store_2d(&tmY, col0, m0, stile_u); bulk_commit(); }
-        }
-        GM_STAMP(4, tcount);
-      }
-      if (lane == 0) bulk_wait<0>();
-    } else {
-    float4* stg = reinterpret_cast<float4*>(sStage) + warp * (GM_STG_FLOATS / 4);
-    const int lrow = lane >> 2, lc4 = lane & 3;              // this lane's row (of 8) / 4-column chunk in the write-out
-    constexpr bool fused = (EPI == DPVO_EPI_RESADD || EPI == DPVO_EPI_GATEDRES);
-    constexpr int NCH = GM_N / 2 / 16;
-    // Everything below is written so that one chunk is straight-line code (no branches on dtypes / optional outputs /
-    // row bounds inside it): its four 8-row steps are independent and only then does the compiler interleave them --
-    // with two epilogue warps per scheduler the dependent-issue latency of serialised steps was the whole cost.
-    constexpr int YB = (OUT == GM_OUT_F16) ? 2 : 4;          // bytes per element of Y
-    const int64_t ystep = 8 * a.ldy * YB, y16step = 8 * a.ldy16 * 2;     // byte strides between the 8-row steps
-    const int64_t rstep = 8 * a.ldres * (a.res_dtype == DPVO_F32 ? 4 : 2), gstep = 8 * a.ldgate * 2;
-    const bool res32 = a.res_dtype == DPVO_F32;
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-      const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-      const int64_t row0 = (tile / n_tiles_n) * GM_M + quarter * 32 + lrow;   // this lane's row in step 0
-      const int n0 = (int)(tile % n_tiles_n) * GM_N + half * (GM_N / 2);
-      const int nch = min(NCH, max(0, (a.N - n0) / 16));     // valid chunks (N is a multiple of 32)
-      bool ok[4];
-#pragma unroll
-      for (int it = 0; it < 4; ++it) ok[it] = row0 + it * 8 < a.rows;
-      const int colL = n0 + lc4 * 4;                          // this lane's first column in chunk 0
-      char* yp = reinterpret_cast<char*>(a.Y) + (row0 * a.ldy + colL) * YB;
-      char* y16p = reinterpret_cast<char*>(a.Y16) + (row0 * a.ldy16 + colL) * 2;
-      const char* rp = reinterpret_cast<const char*>(a.res) + (row0 * a.ldres + colL) * (res32 ? 4 : 2);
-      const char* gp = reinterpret_cast<const char*>(a.gate) + (row0 * a.ldgate + colL) * 2;
-      const float* bp = a.bias ? a.bias + colL : nullptr;
-      // operands of the fused epilogues are fetched one 16-column chunk ahead of their use (and the first chunk
-      // before the accumulator is even ready): with one 16-byte load per lane in flight the layer ran at DRAM
-      // latency.  The residual may alias the output element for element (in-place `net += f(net)`): a thread only
-      // ever prefetches columns it has not written yet.
-      float4 rvA[4], rvB[4]; uint2 gvA[4], gvB[4];
-      auto fetch_operands = [&](int c, float4 (&rv)[4], uint2 (&gv)[4]) {
-        if constexpr (fused) {
-#pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            if (ok[it] && c < nch) {
-              const char* p = rp + it * rstep + c * (res32 ? 64 : 32);
-              if (GM_EXP(1)) rv[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-              else if (res32) rv[it] = *reinterpret_cast<const float4*>(p);
-              else { const uint2 q = *reinterpret_cast<const uint2*>(p); rv[it] = make_float4(__uint_as_float(q.x), __uint_as_float(q.y), 0.f, 0.f); }
-              if constexpr (EPI == DPVO_EPI_GATEDRES) gv[it] = GM_EXP(2) ? make_uint2(0u, 0u) : *reinterpret_cast<const uint2*>(gp + it * gstep + c * 32);
-            }
-          }
-        }
-      };
-      auto fetch_bias = [&](int c) { return (bp && c < nch) ? __ldg(reinterpret_cast<const float4*>(bp + c * 16)) : make_float4(0.f, 0.f, 0.f, 0.f); };
-      float4 bias_next = fetch_bias(0);
-      fetch_operands(0, rvA, gvA);
-      mbar_wait(&bars->tmem_full[acc], aph);
-      tc_fence_after();
-      GM_STAMP(3, tcount);
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * GM_N + half * (GM_N / 2);
-      uint32_t r[16];
-      if (nch > 0) tc_ld16(taddr, r);
-      else { tc_fence_before(); mbar_arrive(&bars->tmem_empty[acc]); }
-      // one 16-column chunk: `use` holds this chunk's operands, `pre` receives the next chunk's
-      auto chunk = [&](int c, float4 (&rv_use)[4], uint2 (&gv_use)[4], float4 (&rv_pre)[4], uint2 (&gv_pre)[4]) {
-        if (c >= nch) return;                                // warp-uniform
-        tc_ld_wait();
-        {                                                    // accumulator row -> staging, chunk j of row `lane`
-          const int sw = (lane >> 1) & 3;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            stg[lane * 4 + (j ^ sw)] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                                   __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-        }
-        if (c + 1 < nch) tc_ld16(taddr + (c + 1) * 16, r);
-        else { tc_fence_before(); mbar_arrive(&bars->tmem_empty[acc]); }     // last read of this accumulator stage
-        const float4 bv = bias_next;
-        bias_next = fetch_bias(c + 1);
-        fetch_operands(c + 1, rv_pre, gv_pre);
-        __syncwarp();
-        float4 v[4];
-#pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int rr = it * 8 + lrow;
-          v[it] = stg[rr * 4 + (lc4 ^ ((rr >> 1) & 3))];
-        }
-        __syncwarp();                                        // staging tile free for the next chunk
-        if constexpr (EPI == DPVO_EPI_SIGMOID_RELU) {
-          // the column half decides the activation; uniform over the chunk (N/2 is a multiple of 16), so a real
-          // branch: evaluating both and selecting made this epilogue slower than the two layers it replaces
-          if (n0 + c * 16 < (a.N >> 1)) {
-#pragma unroll
-            for (int it = 0; it < 4; ++it)
-              v[it] = make_float4(__fdividef(1.0f, 1.0f + __expf(-(v[it].x + bv.x))), __fdividef(1.0f, 1.0f + __expf(-(v[it].y + bv.y))),
-                                  __fdividef(1.0f, 1.0f + __expf(-(v[it].z + bv.z))), __fdividef(1.0f, 1.0f + __expf(-(v[it].w + bv.w))));
-          } else {
-#pragma unroll
-            for (int it = 0; it < 4; ++it)
-              v[it] = make_float4(fmaxf(v[it].x + bv.x, 0.f), fmaxf(v[it].y + bv.y, 0.f), fmaxf(v[it].z + bv.z, 0.f), fmaxf(v[it].w + bv.w, 0.f));
-          }
-        }
-#pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          float4 o4 = v[it];
-          o4.x += bv.x; o4.y += bv.y; o4.z += bv.z; o4.w += bv.w;
-          if constexpr (fused) {
-            float4 rr4 = rv_use[it];
-            {
-              const uint32_t q0 = __float_as_uint(rr4.x), q1 = __float_as_uint(rr4.y);
-              const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&q0)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&q1));
-              rr4 = res32 ? rr4 : make_float4(f0.x, f0.y, f1.x, f1.y);
-            }
-            if constexpr (EPI == DPVO_EPI_GATEDRES) {
-              const uint2 q = gv_use[it];
-              const float2 g0 = __half22float2(*reinterpret_cast<const __half2*>(&q.x)), g1 = __half22float2(*reinterpret_cast<const __half2*>(&q.y));
-              o4.x = rr4.x + g0.x * o4.x; o4.y = rr4.y + g0.y * o4.y; o4.z = rr4.z + g1.x * o4.z; o4.w = rr4.w + g1.y * o4.w;
-            } else {
-              o4.x += rr4.x; o4.y += rr4.y; o4.z += rr4.z; o4.w += rr4.w;
-            }
-          } else if constexpr (EPI == DPVO_EPI_RELU) {
-            o4.x = fmaxf(o4.x, 0.f); o4.y = fmaxf(o4.y, 0.f); o4.z = fmaxf(o4.z, 0.f); o4.w = fmaxf(o4.w, 0.f);
-          } else if constexpr (EPI == DPVO_EPI_SIGMOID) {
-            o4.x = __fdividef(1.0f, 1.0f + __expf(-o4.x)); o4.y = __fdividef(1.0f, 1.0f + __expf(-o4.y));
-            o4.z = __fdividef(1.0f, 1.0f + __expf(-o4.z)); o4.w = __fdividef(1.0f, 1.0f + __expf(-o4.w));
-          } else if constexpr (EPI == DPVO_EPI_SIGMOID_RELU) {
-            o4 = v[it];                                        // activated (with bias) before this loop, see below
-          }
-          uint2 o;
-          *reinterpret_cast<__half2*>(&o.x) = __floats2half2_rn(o4.x, o4.y);
-          *reinterpret_cast<__half2*>(&o.y) = __floats2half2_rn(o4.z, o4.w);
-          if (ok[it]) {
-            if (!GM_EXP(4)) {
-              if constexpr (OUT == GM_OUT_F16) *reinterpret_cast<uint2*>(yp + it * ystep + c * 32) = o;
-              else *reinterpret_cast<float4*>(yp + it * ystep + c * 64) = o4;
-            }
-            if constexpr (OUT == GM_OUT_F32_F16) { if (!GM_EXP(8)) *reinterpret_cast<uint2*>(y16p + it * y16step + c * 32) = o; }
-          }
-        }
-      };
-      static_assert(NCH % 2 == 0, "chunks are processed in pairs (two operand buffers)");
-#pragma unroll 1
-      for (int c = 0; c < NCH; c += 2) {
-        chunk(c, rvA, gvA, rvB, gvB);
-        chunk(c + 1, rvB, gvB, rvA, gvA);
-      }
-      GM_STAMP(4, tcount);
-    }
-    }
-  }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      release(prev);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == GM_MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "n"(GM_TMEM_COLS));
+      // ---- epilogue from the accumulator registers: rows r0, r0 + 8; columns 8 j + 2 (lane % 4) + {0, 1}
+      const int64_t r0 = m0 + wg * 64 + wq * 16 + (lane >> 2);
+      const int cl = 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < GM_N / 8; ++j) {
+        const int col = n0 + 8 * j + cl;
+        if (col >= a.N) continue;                              // N is a multiple of 32: uniform per 8-column block
+        const float2 bv = a.bias ? *reinterpret_cast<const float2*>(a.bias + col) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int64_t row = r0 + 8 * rr;
+          if (row >= a.rows) continue;
+          float v0 = acc[4 * j + 2 * rr] + bv.x, v1 = acc[4 * j + 2 * rr + 1] + bv.y;
+          if constexpr (EPI == DPVO_EPI_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          else if constexpr (EPI == DPVO_EPI_SIGMOID) { v0 = __fdividef(1.0f, 1.0f + __expf(-v0)); v1 = __fdividef(1.0f, 1.0f + __expf(-v1)); }
+          else if constexpr (EPI == DPVO_EPI_SIGMOID_RELU) {
+            if (col < (a.N >> 1)) { v0 = __fdividef(1.0f, 1.0f + __expf(-v0)); v1 = __fdividef(1.0f, 1.0f + __expf(-v1)); }
+            else { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          } else if constexpr (EPI == DPVO_EPI_RESADD || EPI == DPVO_EPI_GATEDRES) {
+            // the residual may alias the output element for element (in-place `net += f(net)`): read before the write
+            float2 rv;
+            if (a.res_dtype == DPVO_F32) rv = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(a.res) + row * a.ldres + col);
+            else rv = __half22float2(*reinterpret_cast<const __half2*>(reinterpret_cast<const __half*>(a.res) + row * a.ldres + col));
+            if constexpr (EPI == DPVO_EPI_GATEDRES) {
+              const float2 g = __half22float2(*reinterpret_cast<const __half2*>(a.gate + row * a.ldgate + col));
+              v0 = rv.x + g.x * v0; v1 = rv.y + g.y * v1;
+            } else {
+              v0 += rv.x; v1 += rv.y;
+            }
+          }
+          if constexpr (OUT == GM_OUT_F16) {
+            *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(a.Y) + row * a.ldy + col) = __floats2half2_rn(v0, v1);
+          } else {
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(a.Y) + row * a.ldy + col) = make_float2(v0, v1);
+            if constexpr (OUT == GM_OUT_F32_F16) *reinterpret_cast<__half2*>(a.Y16 + row * a.ldy16 + col) = __floats2half2_rn(v0, v1);
+          }
+        }
+      }
+    }
   }
 }
 
@@ -515,17 +276,17 @@ static int make_tmap(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols
   return DPVO_OK;
 }
 
-struct GemmMaps { CUtensorMap A, B, R, G, Y; };
+struct GemmMaps { CUtensorMap A, B; };
 
 template <bool GATHER, bool WS, int EPI, int OUT>
 static int launch_out(const GemmMaps& m, const GemmArgs& a, unsigned grid, cudaStream_t st) {
   const size_t smem = (WS ? (size_t)GM_WS_ASTAGES * GM_A_BYTES + (size_t)GM_WS_MAXKB * GM_B_BYTES
-                          : (size_t)GM_STAGES * (GM_A_BYTES + GM_B_BYTES)) + (size_t)GM_EPI_WARPS * GM_STG_FLOATS * 4 + sizeof(GemmBars) + 1024;
+                          : (size_t)GM_STAGES * (GM_A_BYTES + GM_B_BYTES)) + sizeof(GemmBars) + 1024;
   // the opt-in is a per-device function attribute: set it on every launch (a cached flag would be wrong on the
   // second GPU of a process and is not worth a lock)
   cudaError_t e = cudaFuncSetAttribute(linear_f16_kernel<GATHER, WS, EPI, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return check_cuda(e, "linear_f16: cudaFuncSetAttribute");
-  linear_f16_kernel<GATHER, WS, EPI, OUT><<<grid, GM_THREADS, smem, st>>>(m.A, m.B, m.R, m.G, m.Y, a);
+  linear_f16_kernel<GATHER, WS, EPI, OUT><<<grid, GM_THREADS, smem, st>>>(m.A, m.B, a);
   DPVO_LAUNCH_CHECK("linear_f16_kernel");
   return DPVO_OK;
 }
@@ -549,43 +310,10 @@ static int launch_variant(const GemmMaps& m, const GemmArgs& a, unsigned grid, c
   }
 }
 
-// fp16 result [rows, N], row stride ld: 32-row x 32-column store boxes in the SWIZZLE_64B pattern the epilogue writes
-static int make_store_tmap(CUtensorMap* m, void* ptr, int64_t rows, int64_t cols, int64_t ld) {
-  EncodeTiledFn fn = encode_tiled();
-  if (!fn) { set_error("linear_f16: cuTensorMapEncodeTiled is not available from the driver"); return DPVO_ERR_CUDA; }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("linear_f16: cuTensorMapEncodeTiled (result map) failed (%d)", (int)r); return DPVO_ERR_CUDA; }
-  return DPVO_OK;
-}
-
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-// plain (unswizzled) 2-D map over an epilogue operand, used only for L2 prefetches of GM_M x GM_N tiles
-static bool make_prefetch_tmap(CUtensorMap* m, const void* ptr, int dtype, int64_t rows, int64_t cols, int64_t ld) {
-  EncodeTiledFn fn = encode_tiled();
-  const int es = dtype == DPVO_F32 ? 4 : 2;
-  if (!fn || ((uintptr_t)ptr & 15) || (ld * es) % 16) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * es};
-  cuuint32_t box[2] = {(cuuint32_t)std::min<int64_t>(cols, GM_N), (cuuint32_t)GM_M};
-  cuuint32_t estr[2] = {1, 1};
-  return fn(m, dtype == DPVO_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides,
-            box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-#endif
-
 static int linear_launch(GemmArgs& a, cudaStream_t st) {
   const int n_tiles_n = (a.N + GM_N - 1) / GM_N;
   const int64_t tiles = ((a.rows + GM_M - 1) / GM_M) * n_tiles_n;
-  bool ws = (a.K / GM_K) <= GM_WS_MAXKB;
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-  if (getenv("DPVO_B200_GEMM_STREAM")) ws = false;
-#endif
+  const bool ws = (a.K / GM_K) <= GM_WS_MAXKB;
   // weight-stationary CTAs keep their column slice: the grid must be a multiple of the slice count
   int64_t grid = std::min<int64_t>(tiles, sm_count());
   if (ws) grid = std::max<int64_t>(n_tiles_n, grid / n_tiles_n * n_tiles_n);
@@ -593,19 +321,6 @@ static int linear_launch(GemmArgs& a, cudaStream_t st) {
   memset(&m, 0, sizeof(m));
   int rc = make_tmap(&m.B, a.W, a.N, a.K, a.ldw, GM_N);
   if (rc) return rc;
-  a.prefetch = 0;
-  const bool fused = a.epilogue == DPVO_EPI_RESADD || a.epilogue == DPVO_EPI_GATEDRES;
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-  if (fused && getenv("DPVO_B200_GEMM_PREFETCH")) {
-    bool ok = make_prefetch_tmap(&m.R, a.res, a.res_dtype, a.rows, a.N, a.ldres);
-    if (ok && a.epilogue == DPVO_EPI_GATEDRES) ok = make_prefetch_tmap(&m.G, a.gate, DPVO_F16, a.rows, a.N, a.ldgate);
-    a.prefetch = ok ? 1 : 0;
-  }
-#endif
-  if (!fused && a.y_dtype == DPVO_F16) {                     // the result leaves through the TMA unit
-    rc = make_store_tmap(&m.Y, a.Y, a.rows, a.N, a.ldy);
-    if (rc) return rc;
-  }
   if (a.gather) return ws ? launch_variant<true, true>(m, a, (unsigned)grid, st) : launch_variant<true, false>(m, a, (unsigned)grid, st);
   rc = make_tmap(&m.A, a.X, a.rows, a.K, a.ldx, GM_M);
   if (rc) return rc;
@@ -644,33 +359,5 @@ extern "C" int dpvo_linear_f16(const void* X, int64_t ldx, const int64_t* gather
   a.Y16 = (__half*)Y16; a.ldy16 = ldy16;
   a.Y = Y; a.y_dtype = y_dtype; a.ldy = ldy; a.rows = rows; a.N = N; a.K = K; a.epilogue = epilogue;
 
-  a.dbg = nullptr;
-  a.exp_flags = 0;
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-  // perf-attribution switches (tools/ only; never compiled into the release library): per-role timestamps of CTA 0
-  // and dropping operand loads / result stores
-  static long long* dbg = nullptr;
-  const bool timing = getenv("DPVO_B200_GEMM_TIMING") != nullptr;
-  if (timing && !dbg) cudaMalloc(&dbg, 96 * sizeof(long long));
-  a.dbg = timing ? dbg : nullptr;
-  {
-    const char* ex = getenv("DPVO_B200_GEMM_EXP");
-    a.exp_flags = ex ? atoi(ex) : 0;
-  }
-  if (timing) cudaMemsetAsync(dbg, 0, 96 * sizeof(long long), (cudaStream_t)stream);
-#endif
-  const int rc = linear_launch(a, (cudaStream_t)stream);
-#ifdef DPVO_B200_PERF_EXPERIMENTS
-  if (timing && rc == DPVO_OK) {
-    long long h[96];
-    cudaStreamSynchronize((cudaStream_t)stream);
-    cudaMemcpy(h, dbg, sizeof(h), cudaMemcpyDeviceToHost);
-    const long long t0 = h[5 * 16];
-    fprintf(stderr, "[linear_f16 CTA 0, SM cycles from kernel begin] rows=%lld N=%d K=%d epi=%d  weights landed %lld\n", (long long)rows, N, K, epilogue, h[5 * 16 + 1] - t0);
-    for (int t = 0; t < 16 && h[t]; ++t)
-      fprintf(stderr, "   tile %d: mma begin %lld  acc free %lld  issued %lld | epi ready %lld  done %lld\n", t, h[t] - t0, h[16 + t] - t0,
-              h[32 + t] - t0, h[48 + t] - t0, h[64 + t] - t0);
-  }
-#endif
-  return rc;
+  return linear_launch(a, (cudaStream_t)stream);
 }

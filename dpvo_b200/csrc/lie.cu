@@ -1,4 +1,4 @@
-// lietorch_backends for sm_100a: SO3, RxSO3, SE3, Sim3, float and double, forward + backward.
+// lietorch_backends for sm_90a: SO3, RxSO3, SE3, Sim3, float and double, forward + backward.
 // Replaces dpvo/lietorch/src/lietorch_gpu.cu:20-601 (Eigen template kernels) with register math
 // from lie.cuh.  One group element per thread, grid-stride, outputs fully written (the reference
 // allocates with torch::zeros and overwrites; the unused last gradient component stays 0).

@@ -323,7 +323,7 @@ Tensor corr_pyramid2(Tensor fmap1, Tensor fmap2_l0, Tensor fmap2_l1, Tensor coor
   const int B = coords.size(0), M = coords.size(1), P = coords.size(3), C = fmap1.size(2), O = 2 * radius + 1;
   const int64_t feat = (int64_t)O * O * P * P * 2;
   const int64_t row = pad_to > feat ? pad_to : feat;
-  // padded rows ([B, M, row], zero tail) feed the tcgen05 dense layer directly; unpadded keep the 7-d view
+  // padded rows ([B, M, row], zero tail) feed the wgmma dense layer directly; unpadded keep the 7-d view
   // out_buf: a caller-owned [B, M, row] buffer whose padding columns are already zero (reused every update)
   Tensor out;
   if (out_buf.has_value()) {
@@ -551,7 +551,7 @@ Tensor softagg_reduce(Tensor fg, Tensor order, Tensor group_start, Tensor n_grou
   return y;
 }
 
-// Y = epilogue(X @ W^T + bias) on tcgen05; X [.., rows, K] fp16 (row stride may exceed K), W [N, K] fp16
+// Y = epilogue(X @ W^T + bias) on wgmma; X [.., rows, K] fp16 (row stride may exceed K), W [N, K] fp16
 Tensor linear_f16(Tensor x, Tensor w, c10::optional<Tensor> bias, int64_t epilogue, c10::optional<Tensor> res,
                   c10::optional<Tensor> gate, c10::optional<Tensor> gather, bool out_f32, c10::optional<Tensor> out,
                   c10::optional<Tensor> out16) {
@@ -814,7 +814,7 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("softagg_reduce", &softagg_reduce, "segment softmax-weighted sum");
   m.def("update_heads", &update_heads, "delta / weight heads (optionally emitting the BA target)", py::arg("net32"), py::arg("W4"),
         py::arg("b4"), py::arg("coords") = py::none(), py::arg("gate") = py::none(), py::arg("res") = py::none());
-  m.def("linear_f16", &linear_f16, "tcgen05 dense layer", py::arg("x"), py::arg("w"), py::arg("bias") = py::none(),
+  m.def("linear_f16", &linear_f16, "wgmma dense layer", py::arg("x"), py::arg("w"), py::arg("bias") = py::none(),
         py::arg("epilogue") = 0, py::arg("res") = py::none(), py::arg("gate") = py::none(), py::arg("gather") = py::none(),
         py::arg("out_f32") = false, py::arg("out") = py::none(), py::arg("out16") = py::none());
   m.def("update_corr_norm", &update_corr_norm, "fused corr MLP + context add + LayerNorm (net.py:76-77)", py::arg("corr16"), py::arg("W0"), py::arg("W25"),

@@ -1,4 +1,4 @@
-"""The recurrent update operator (dpvo/net.py:27-92, dpvo/blocks.py:15-48) on sm_100a kernels.
+"""The recurrent update operator (dpvo/net.py:27-92, dpvo/blocks.py:15-48) on sm_90a kernels.
 
 `Update` keeps the reference's sub-module names, so a DPVO checkpoint's "update.*" state_dict keys
 load unchanged (update.c1.0.weight, update.agg_kk.f.weight, update.gru.1.gate.0.weight, ...).
@@ -10,9 +10,8 @@ Data flow is fp32 for the carried state `net`, fp16 for every GEMM operand (what
 autocast does, dpvo.py:332), with the fp16 copies produced inside the fused row kernels.  The edge
 groupings come from ONE device radix-sort launch each (no host sync, no torch.unique, no D2H sort).
 
-Every dense layer runs on hand-written tcgen05 kernels (csrc/chain.cu: the three fused layer chains; csrc/gemm.cu:
-dpvo_linear_f16 for the four SoftAgg layers); there is no library GEMM and no other backend in the product (a cuBLAS
-comparison lives in tools/bench_gemm.py only).
+Every dense layer runs on hand-written wgmma kernels (csrc/chain.cu: the three fused layer chains; csrc/gemm.cu:
+dpvo_linear_f16 for the four SoftAgg layers); there is no library GEMM and no other backend.
 """
 import torch
 import torch.nn as nn
@@ -138,7 +137,7 @@ class Update(nn.Module):
         P = {}
         P["corr0"], P["corr2"], P["corr5"] = lin(self.corr[0]), lin(self.corr[2]), lin(self.corr[5])
         # the first dense layer consumes correlation rows padded from 882 to 896 columns (one 64-wide
-        # k-block of the tcgen05 kernel); the extra weight columns are zero
+        # k-block of the wgmma kernel); the extra weight columns are zero
         w0, b0 = P["corr0"]
         P["corr0"] = (F.pad(w0, (0, CORR_PAD - w0.shape[1])).contiguous(), b0)
         P["c1a"], P["c1b"], P["c2a"], P["c2b"] = lin(self.c1[0]), lin(self.c1[2]), lin(self.c2[0]), lin(self.c2[2])
@@ -218,7 +217,7 @@ class Update(nn.Module):
         return self._forward_chains(net, inp, corr, groups_kk, groups_ij)
 
     def _forward_chains(self, net, inp, corr, groups_kk, groups_ij):
-        """The row-local stretches of net.py:74-92 as one tcgen05 chain kernel each (csrc/chain.cu): corr MLP + context
+        """The row-local stretches of net.py:74-92 as one wgmma chain kernel each (csrc/chain.cu): corr MLP + context
         add + LayerNorm; c1 and c2 on the masked temporal neighbours; group add + GRU + heads.  Between them only the two
         SoftAgg reductions (which mix rows of a group) run as separate kernels."""
         ex = extensions()[3]

@@ -1,4 +1,4 @@
-"""One DPVO `update()` iteration on the sm_100a kernels -- the public call a user makes.
+"""One DPVO `update()` iteration on the sm_90a kernels -- the public call a user makes.
 
 Mirrors DPVO.update (dpvo/dpvo.py:328-360):
     reproject -> correlation (2 levels) -> context gather -> update operator -> target/weight ->

@@ -1,5 +1,5 @@
 /*
- * dpvo_b200.h -- C-ABI of the B200-native DPVO update hot path.
+ * dpvo_b200.h -- C-ABI of the H100-native DPVO update hot path.
  *
  * Every entry point takes plain device pointers, sizes/strides and a CUDA stream and
  * returns an int status (DPVO_OK == 0).  No torch types cross this boundary.  The three
@@ -13,7 +13,7 @@
  *   Update operator    dpvo/net.py:27-92, dpvo/blocks.py:15-48 (pieces: LayerNorm, SoftAgg, GEMMs)
  *
  * All pointers are DEVICE pointers unless stated otherwise.  `stream` is a cudaStream_t
- * passed as void* (NULL = legacy default stream).  Kernels are compiled for sm_100a only;
+ * passed as void* (NULL = legacy default stream).  Kernels are compiled for sm_90a only;
  * there is no CPU fallback: a call on a machine without a usable device returns DPVO_ERR_CUDA.
  */
 #ifndef DPVO_B200_H
@@ -96,7 +96,7 @@ int dpvo_corr_forward_pyramid2(const void* fmap1, const int64_t* fmap1_strides,
                                int dtype, int B, int M, int C, int P,
                                int S1, int S2, int radius,
                                void* workspace, int64_t workspace_bytes, void* stream);
-/* Scratch for the tcgen05/TMA kernel of dpvo_corr_forward_pyramid2 (list of edges whose nine tap windows do
+/* Scratch for the wgmma/TMA kernel of dpvo_corr_forward_pyramid2 (list of edges whose nine tap windows do
  * not fit one 10x10 box, finished by the mma.sync kernel).  workspace may be NULL: the call then runs the
  * mma.sync kernel for every edge.  S1 / S2 are the slot counts of the patch-feature and frame-feature rings
  * (extents of the TMA tensor maps). */
@@ -383,7 +383,7 @@ int dpvo_update_heads(void* net32, const void* gate16, int64_t ld_gate, const vo
                       float* delta, float* weight, int64_t rows, int dim, void* stream);
 
 /*
- * Dense layer on tensor cores (tcgen05.mma, fp16 operands, fp32 accumulation in TMEM):
+ * Dense layer on tensor cores (wgmma, fp16 operands, fp32 accumulation in registers):
  *   Y = epilogue( X[rows, K] @ W[N, K]^T + bias[N] )
  * X, W fp16 row-major (K contiguous, rows 16-byte aligned), bias fp32 (may be NULL).
  * gather (optional, int64 [rows]): row r of X is read from X[gather[r]], or taken as zero when
@@ -413,8 +413,8 @@ int dpvo_linear_f16(const void* X, int64_t ldx, const int64_t* gather, const voi
                     int64_t rows, int N, int K, int epilogue, void* stream);
 
 /* ---- Update operator, fused layer chains (dpvo_b200/csrc/chain.cu) -------------------------------------------------
- * The row-local stretches of Update.forward (dpvo/net.py:74-92) as one tcgen05 kernel each: a 128-edge tile runs
- * through every dense layer of the stretch on chip (operand tile in shared memory, fp32 accumulator in TMEM),
+ * The row-local stretches of Update.forward (dpvo/net.py:74-92) as one wgmma kernel each: a 64-edge tile runs
+ * through every dense layer of the stretch on chip (operand tile in shared memory, fp32 accumulator in registers),
  * LayerNorm / gating / heads in the epilogues.  DIM = 384 (net.py:24), E = edges, all weights fp16 row-major
  * [out, in], all parameters fp32, `net32` is the fp32 recurrent state [E, 384] updated IN PLACE.
  *

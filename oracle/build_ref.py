@@ -1,4 +1,4 @@
-"""ORACLE (test infrastructure): compile the REFERENCE's own CUDA extensions for sm_100a into
+"""ORACLE (test infrastructure): compile the REFERENCE's own CUDA extensions for sm_90a into
 oracle/_ref/ so the GPU box can compare our kernels against the reference's kernels directly.
 
 Sources are read where they lie under /root/reference; nothing is copied into the repository.  The
@@ -15,7 +15,7 @@ directory:
 lietorch_backends cannot be built (every kernel is Eigen template code): no _ref for it.
 
 Outputs: oracle/_ref/ref_cuda_corr<EXT>, oracle/_ref/ref_cuda_ba<EXT> (module names prefixed so they
-can be imported next to ours).  git-ignored, not gpurun-ignored.  Run: python oracle/build_ref.py
+can be imported next to ours).  git-ignored.  Run: python oracle/build_ref.py
 
 stage_python(): the reference's *Python* package (dpvo/*.py, altcorr/, fastba/, lietorch/ wrappers,
 config/*.yaml -- interpreted code, no build step) packed UNMODIFIED into oracle/_ref/dpvo_ref_py.zip so that the GPU
@@ -30,6 +30,7 @@ import subprocess
 import sys
 import sysconfig
 import tempfile
+from concurrent.futures import ThreadPoolExecutor
 
 REF = "/root/reference/dpvo"
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -76,7 +77,7 @@ def build(force=False):
     if not force and os.path.exists(t_corr) and os.path.exists(t_ba):
         return True
     inc, abi, link = _flags()
-    nv = ["nvcc", "-O3", "-std=c++17", "--expt-relaxed-constexpr", "-gencode", "arch=compute_100a,code=sm_100a",
+    nv = ["nvcc", "-O3", "-std=c++17", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a",
           "-Xcompiler", "-fPIC", abi] + inc
     with tempfile.TemporaryDirectory(prefix="dpvo_ref_") as tmp:
         # ---- cuda_corr
@@ -84,9 +85,6 @@ def build(force=False):
         src, n = re.subn(r"\.type\(\), \"", ".scalar_type(), \"", src)
         assert n == 4, "expected 4 dispatch sites, found %d" % n
         open(os.path.join(tmp, "correlation_kernel.cu"), "w").write(src)
-        _sh(nv + ["-DTORCH_EXTENSION_NAME=ref_cuda_corr", "-c", os.path.join(tmp, "correlation_kernel.cu"), "-o", os.path.join(tmp, "ck.o")])
-        _sh(nv + ["-DTORCH_EXTENSION_NAME=ref_cuda_corr", "-x", "cu", "-c", os.path.join(REF, "altcorr", "correlation.cpp"), "-o", os.path.join(tmp, "cc.o")])
-        _sh(["nvcc", "-shared", "-o", t_corr, os.path.join(tmp, "ck.o"), os.path.join(tmp, "cc.o")] + link)
         # ---- cuda_ba
         lines = open(os.path.join(REF, "fastba", "ba.cpp")).read().split("\n")
         keep = [l for i, l in enumerate(lines, 1) if not (i in (6, 7) or 99 <= i <= 180 or i == 187)]
@@ -97,9 +95,17 @@ def build(force=False):
         assert n == 1, "IndexLookup typedef not found"
         open(os.path.join(tmp, "block_e.cu"), "w").write(be)
         fb = ["-I", os.path.join(REF, "fastba")]
-        _sh(nv + fb + ["-DTORCH_EXTENSION_NAME=ref_cuda_ba", "-c", os.path.join(REF, "fastba", "ba_cuda.cu"), "-o", os.path.join(tmp, "bk.o")])
-        _sh(nv + fb + ["-DTORCH_EXTENSION_NAME=ref_cuda_ba", "-c", os.path.join(tmp, "block_e.cu"), "-o", os.path.join(tmp, "be.o")])
-        _sh(nv + fb + ["-DTORCH_EXTENSION_NAME=ref_cuda_ba", "-x", "cu", "-c", os.path.join(tmp, "ba.cpp"), "-o", os.path.join(tmp, "bc.o")])
+        corr = nv + ["-DTORCH_EXTENSION_NAME=ref_cuda_corr"]
+        ba = nv + fb + ["-DTORCH_EXTENSION_NAME=ref_cuda_ba"]
+        # the five translation units are independent (and each takes minutes): compile them concurrently
+        compiles = [corr + ["-c", os.path.join(tmp, "correlation_kernel.cu"), "-o", os.path.join(tmp, "ck.o")],
+                    corr + ["-x", "cu", "-c", os.path.join(REF, "altcorr", "correlation.cpp"), "-o", os.path.join(tmp, "cc.o")],
+                    ba + ["-c", os.path.join(REF, "fastba", "ba_cuda.cu"), "-o", os.path.join(tmp, "bk.o")],
+                    ba + ["-c", os.path.join(tmp, "block_e.cu"), "-o", os.path.join(tmp, "be.o")],
+                    ba + ["-x", "cu", "-c", os.path.join(tmp, "ba.cpp"), "-o", os.path.join(tmp, "bc.o")]]
+        with ThreadPoolExecutor(max_workers=len(compiles)) as ex:
+            list(ex.map(_sh, compiles))
+        _sh(["nvcc", "-shared", "-o", t_corr, os.path.join(tmp, "ck.o"), os.path.join(tmp, "cc.o")] + link)
         _sh(["nvcc", "-shared", "-o", t_ba, os.path.join(tmp, "bk.o"), os.path.join(tmp, "be.o"), os.path.join(tmp, "bc.o")] + link)
     return True
 

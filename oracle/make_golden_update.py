@@ -30,7 +30,7 @@ from oracle import refimport  # noqa: E402
 GOLD = os.path.join(ROOT, "tests", "golden")
 CASES = {
     # name: (M patches/frame, lifetime, removal, frames, weight seed, data seed)
-    "a": (6, 5, 8, 10, 1234, 71),
+    "a": (6, 5, 8, 8, 1234, 71),
     "b": (4, 3, 5, 12, 99, 72),
 }
 

@@ -3,11 +3,11 @@ dpvo/dpvo.py with dpvo/net.py:VONet -- driven on a synthetic image stream, on to
 of native modules:
 
     native="ours"   cuda_corr / cuda_ba / lietorch_backends = dpvo_b200/_ext   (the drop-in, exercised)
-    native="ref"    cuda_corr / cuda_ba = oracle/_ref (the reference's own kernels compiled for sm_100a);
+    native="ref"    cuda_corr / cuda_ba = oracle/_ref (the reference's own kernels compiled for sm_90a);
                     lietorch_backends stays ours: the reference's is Eigen template code and Eigen is
                     not in the image (SURVEY 8(c)) -- it only serves pops.transform / the motion model here
     update="reference"  dpvo/net.py:Update in torch under autocast (dpvo.py:332), torch_scatter restated
-    update="ours"       dpvo_b200.net.Update (tcgen05 kernels) loaded with the same state_dict
+    update="ours"       dpvo_b200.net.Update (wgmma kernels) loaded with the same state_dict
 
 Used by tests/test_dropin_gpu.py (parity of one DPVO.update() from an identical state, ours vs the
 reference kernels) and by bench.py's `reference_cuda` leg (the same-box denominator of north_star's

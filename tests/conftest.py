@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 @pytest.fixture(scope="session")
 def ext():
-    """(cuda_corr, cuda_ba, lietorch_backends, dpvo_b200_ext) -- the real sm_100a build."""
+    """(cuda_corr, cuda_ba, lietorch_backends, dpvo_b200_ext) -- the real sm_90a build."""
     import dpvo_b200
     return dpvo_b200.extensions()
 

@@ -24,7 +24,7 @@ def test_every_declared_symbol_is_exported():
 
 def test_version_and_error_text():
     lib = dpvo_b200.library()
-    assert b"sm_100a" in lib.dpvo_version()
+    assert b"sm_90a" in lib.dpvo_version()
     assert isinstance(lib.dpvo_last_error(), bytes)
     assert lib.dpvo_launch_count() >= 0
 

@@ -33,7 +33,7 @@ def _close(a, b, tol, what):
     assert err <= tol * max(ref, 1.0), "%s: max err %.3g (ref scale %.3g)" % (what, err, ref)
 
 
-@pytest.mark.parametrize("E", [47712, 128, 77, 1000, 148 * 128 + 5])
+@pytest.mark.parametrize("E", [47712, 128, 77, 1000, 148 * 128 + 5, 132 * 64, 132 * 64 + 5])
 def test_corr_norm_chain(E):
     ex = _ext()
     g = torch.Generator(device="cuda").manual_seed(E)
@@ -62,7 +62,7 @@ def test_corr_norm_chain(E):
     assert torch.equal(n16.reshape(E, DIM), net32.half()), "the fp16 copy is the rounded fp32 state"
 
 
-@pytest.mark.parametrize("E", [47712, 128, 77, 1000, 148 * 128 + 5])
+@pytest.mark.parametrize("E", [47712, 128, 77, 1000, 148 * 128 + 5, 132 * 64, 132 * 64 + 5])
 def test_neighbor_mlp_chain(E):
     ex = _ext()
     g = torch.Generator(device="cuda").manual_seed(E + 1)
@@ -82,7 +82,7 @@ def test_neighbor_mlp_chain(E):
     assert torch.equal(n16.reshape(E, DIM), net32.half())
 
 
-@pytest.mark.parametrize("E", [47712, 128, 77, 1000, 148 * 128 + 5])
+@pytest.mark.parametrize("E", [47712, 128, 77, 1000, 148 * 128 + 5, 132 * 64, 132 * 64 + 5])
 @pytest.mark.parametrize("with_groups", [True, False])
 def test_gru_heads_chain(E, with_groups):
     ex = _ext()

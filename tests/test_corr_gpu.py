@@ -95,7 +95,7 @@ def _pyramid_inputs(dtype, M, seed=7, S1=50, S2=4, H=32, W=48, stretch_every=0, 
     offs = torch.arange(3).float() - 1
     sx, sy = torch.ones(M), torch.ones(M)
     if stretch_every:
-        sx[::stretch_every] = fx              # 2.7: the nine tap windows no longer fit any box of the tcgen05 kernel
+        sx[::stretch_every] = fx              # 2.7: the nine tap windows no longer fit any box of the wgmma kernel
         sy[::stretch_every] = fy
     coords[0, :, 0] = (torch.rand(M, generator=g) * (W + 8) - 4)[:, None, None] + offs[None, None, :] * sx[:, None, None]
     coords[0, :, 1] = (torch.rand(M, generator=g) * (H + 8) - 4)[:, None, None] + offs[None, :, None] * sy[:, None, None]
@@ -115,7 +115,7 @@ def test_corr_pyramid2_matches_two_calls(ext, dtype):
     if dtype == torch.float32:
         assert torch.equal(fused, ref)
     else:
-        # fp16 features: the fused call runs on tcgen05 (fp32 accumulation in another order than mma.sync),
+        # fp16 features: the fused call runs on wgmma (fp32 accumulation in another order than mma.sync),
         # results agree to fp16 rounding
         assert torch.allclose(fused.float(), ref.float(), atol=2e-3, rtol=2e-3)
 
@@ -124,7 +124,7 @@ def test_corr_pyramid2_matches_two_calls(ext, dtype):
                                                  (3000, 2, 896, 1.4, 1.4), (3000, 2, 896, 1.9, 1.0), (3000, 3, 0, 0.6, 1.9),
                                                  (2000, 2, 0, 1.9, 1.9), (2000, 2, 0, 0.3, 0.3)])
 def test_corr_tcgen05_vs_oracle(ext, M, stretch, pad, fx, fy):
-    """tcgen05/TMA kernel (every box shape 8..12 x 8..12 up to 128 pixels, the stretched-edge list finished by
+    """wgmma/TMA kernel (every box shape 8..12 x 8..12 up to 128 pixels, the stretched-edge list finished by
     the mma.sync kernel, out-of-map boxes zero-filled by TMA, padded rows) against the fp64 restatement of
     correlation_kernel.cu:78-137"""
     f1, l0, l1, coords, ii, jj = _pyramid_inputs(torch.half, M, seed=11 + M, stretch_every=stretch, fx=fx, fy=fy)

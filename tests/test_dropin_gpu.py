@@ -152,7 +152,7 @@ def test_reference_transform_jacobians_on_our_lietorch(refpy):
 @pytest.mark.parametrize("config,n_frames", [("fast", 14)])
 def test_reference_update_module_vs_ours_same_weights(refpy, ext, config, n_frames):
     """dpvo/net.py:Update (torch, autocast as dpvo.py:332, calling OUR cuda_ba.neighbors) vs dpvo_b200.net.Update
-    (tcgen05) with the same state_dict, both against the reference module in fp32: ours no worse than 2x the
+    (wgmma) with the same state_dict, both against the reference module in fp32: ours no worse than 2x the
     reference's own mixed-precision error"""
     from dpvo_b200.net import Update
     st = synthetic.make_state(config, n_frames, device="cpu", features=False)

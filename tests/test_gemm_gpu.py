@@ -1,4 +1,4 @@
-"""tcgen05 dense layer (dpvo_linear_f16) vs an fp32 torch reference of the same op."""
+"""wgmma dense layer (dpvo_linear_f16) vs an fp32 torch reference of the same op."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -149,7 +149,7 @@ def test_write_golden_fixtures_from_reference_kernels(ref):
     grad = torch.randn(1, 48, 7, 7, 3, 3, generator=g)
     g1, g2 = ref[0].backward(f1.to(DEV), f2.to(DEV), coords.to(DEV), ii.to(DEV), jj.to(DEV), grad.to(DEV), 3)
     torch.save(dict(fmap1=f1, fmap2=f2, coords=coords, ii=ii, jj=jj, radius=3, out=c.cpu(), grad=grad,
-                    fmap1_grad=g1.cpu(), fmap2_grad=g2.cpu(), source="ref_cuda_corr (correlation_kernel.cu) on B200"),
+                    fmap1_grad=g1.cpu(), fmap2_grad=g2.cpu(), source="ref_cuda_corr (correlation_kernel.cu)"),
                os.path.join(out_dir, "corr_ref_fp32.pt"))
     st = synthetic.make_state("fast", 12, device="cpu", features=False, seed=53, buffer=16)
     coords2 = OB.fastba_reproject(st.poses.double(), st.patches.double(), st.intrinsics.double(), st.ii, st.jj, st.kk)
@@ -167,5 +167,5 @@ def test_write_golden_fixtures_from_reference_kernels(ref):
                     target=target, weight=weight, ii=st.ii, jj=st.jj, kk=st.kk, t0=st.t0, t1=st.n,
                     poses_out=poses[0, :st.n].cpu(), depth_out=patches[0, :st.n * 48, 2, 0, 0].cpu(), live=live,
                     neighbors_ix=ix.cpu(), neighbors_jx=jx.cpu(), reproject=rep.cpu().half(),
-                    source="ref_cuda_ba (ba_cuda.cu, ba.cpp) on B200"),
+                    source="ref_cuda_ba (ba_cuda.cu, ba.cpp)"),
                os.path.join(out_dir, "ba_ref_fast12.pt"))

@@ -12,7 +12,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 @pytest.fixture()
 def gpu_tests(monkeypatch):
     sys.path.insert(0, os.path.join(HERE, "..", "oracle", "shims"))
-    import lietorch_backends as LB
+    # by file: once the real extension module is imported under this name, `import lietorch_backends` returns it
+    _spec = importlib.util.spec_from_file_location("oracle_lietorch_backends", os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "shims", "lietorch_backends.py"))
+    LB = importlib.util.module_from_spec(_spec)
+    _spec.loader.exec_module(LB)
     import dpvo_b200.lietorch.groups as Gm
     import dpvo_b200.projective_ops as pops
     monkeypatch.setattr(Gm, "_B", LB)

@@ -1,5 +1,5 @@
 """The step the bench times -- UpdateRunner.step(): reproject_clamped -> corr_fwd_tc on the real feature ring ->
-tcgen05 Update -> grouped BA -- end to end on BASELINE configs[1] (default, E = 47,712) and configs[2] (fast,
+wgmma Update -> grouped BA -- end to end on BASELINE configs[1] (default, E = 47,712) and configs[2] (fast,
 E = 14,496), eager and as a CUDA graph, against
   (1) the composed fp32 oracle (oracle/ba.py transform + oracle/corr.py + oracle/update.py + fastba_forward fp64), and
   (2) the reference CUDA pipeline (oracle/ref_pipeline.py:RefCudaStep: the reference's own correlation and BA

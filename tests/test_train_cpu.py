@@ -1,13 +1,13 @@
 """Training-path host code without a GPU: the differentiable bundle adjustment of dpvo_b200/ba.py against the
-REFERENCE's own dpvo/ba.py:BA (imported unmodified from /root/reference, lietorch served by the CPU oracle on
-both sides), outputs and gradients in fp64; and the sequence loss on a hand-checkable case."""
+REFERENCE's own dpvo/ba.py:BA (run once by oracle/make_golden_reference.py with lietorch served by the CPU oracle;
+outputs and gradients in fp64 stored in tests/golden/reference_cpu.pt); and the sequence loss on a hand-checkable case."""
+import importlib.util
 import os
 import sys
 
 import pytest
 import torch
 
-from oracle import refimport
 from dpvo_b200 import synthetic
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -24,7 +24,10 @@ class _UniqueGroups:
 @pytest.fixture()
 def cpu_ops(monkeypatch):
     sys.path.insert(0, os.path.join(HERE, "..", "oracle", "shims"))
-    import lietorch_backends as LB
+    # by file: once the real extension module is imported under this name, `import lietorch_backends` returns it
+    _spec = importlib.util.spec_from_file_location("oracle_lietorch_backends", os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "shims", "lietorch_backends.py"))
+    LB = importlib.util.module_from_spec(_spec)
+    _spec.loader.exec_module(LB)
     import dpvo_b200.lietorch.groups as Gm
     import dpvo_b200.ba as ba
     monkeypatch.setattr(Gm, "_B", LB)
@@ -47,37 +50,41 @@ def _problem(seed, structure_only=False):
     return st, poses, patches, intr, target, weight
 
 
-@pytest.mark.skipif(not refimport.available(), reason="/root/reference not mounted")
-@pytest.mark.parametrize("structure_only", [False, True])
-def test_differentiable_ba_matches_the_reference_ba_forward_and_backward(cpu_ops, structure_only):
-    from dpvo_b200.lietorch import SE3
+GOLD = os.path.join(HERE, "golden", "reference_cpu.pt")
+BA_OUTPUTS = ("poses", "patches", "d/dtarget", "d/dweight", "d/dpatches")
+
+
+def run_ba(BA, SE3cls, structure_only, lm=1e-4):
+    """two BA iterations on _problem(3) and the gradients of a seeded linear loss of their result"""
     st, poses, patches, intr, target, weight = _problem(3)
     bounds = [-64, -64, 80 + 64, 60 + 64]
-    h, w = 60, 80
+    t = target.clone().requires_grad_(True)
+    wt = weight.clone().requires_grad_(True)
+    q = patches.clone().requires_grad_(True)
+    G, Q = SE3cls(poses.clone()), q
+    for _ in range(2):
+        G, Q = BA(G, Q, intr, t, wt, lm, st.ii, st.jj, st.kk, bounds, ep=10.0, fixedp=1, structure_only=structure_only)
+    g = torch.Generator().manual_seed(9)
+    cp = torch.randn(G.data.shape, generator=g).double()
+    cq = torch.randn(Q.shape, generator=g).double()
+    loss = (G.data * cp).sum() + (Q * cq).sum()
+    gt, gw, gq = torch.autograd.grad(loss, (t, wt, q))
+    return G.data.detach(), Q.detach(), gt, gw, gq
 
-    def run(BA, SE3cls, lm):
-        t = target.clone().requires_grad_(True)
-        wt = weight.clone().requires_grad_(True)
-        q = patches.clone().requires_grad_(True)
-        G, Q = SE3cls(poses.clone()), q
-        for _ in range(2):
-            G, Q = BA(G, Q, intr, t, wt, lm, st.ii, st.jj, st.kk, bounds, ep=10.0, fixedp=1, structure_only=structure_only)
-        g = torch.Generator().manual_seed(9)
-        cp = torch.randn(G.data.shape, generator=g).double()
-        cq = torch.randn(Q.shape, generator=g).double()
-        loss = (G.data * cp).sum() + (Q * cq).sum()
-        gt, gw, gq = torch.autograd.grad(loss, (t, wt, q))
-        return G.data.detach(), Q.detach(), gt, gw, gq
 
-    mine = run(cpu_ops.BA, SE3, 1e-4)
-    with refimport.reference_modules():
-        import dpvo.ba as RB
-        from dpvo.lietorch import SE3 as RSE3
-        theirs = run(RB.BA, RSE3, 1e-4)
-    for a, b, nm in zip(mine, theirs, ("poses", "patches", "d/dtarget", "d/dweight", "d/dpatches")):
+@pytest.mark.parametrize("structure_only", [False, True])
+def test_differentiable_ba_matches_the_reference_ba_forward_and_backward(cpu_ops, structure_only):
+    """against the REFERENCE's dpvo/ba.py:BA run on the same problem (tests/golden/reference_cpu.pt, written by
+    oracle/make_golden_reference.py)"""
+    from dpvo_b200.lietorch import SE3
+    mine = run_ba(cpu_ops.BA, SE3, structure_only)
+    theirs = torch.load(GOLD)["train_ba"][str(structure_only)]
+    for a, nm in zip(mine, BA_OUTPUTS):
+        b = theirs[nm]
         scale = max(1.0, b.abs().max().item())
         assert (a - b).abs().max().item() <= 1e-8 * scale, (nm, (a - b).abs().max().item())
     if not structure_only:
+        poses = _problem(3)[1]
         assert (mine[0] - poses).abs().max().item() > 1e-4          # the step moved the poses
 
 

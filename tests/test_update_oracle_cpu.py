@@ -1,12 +1,12 @@
 """oracle/update.py held to the REFERENCE's own dpvo/net.py:Update -- through the committed fixtures
 (tests/golden/update_ref_*.pt, written by oracle/make_golden_update.py from the imported reference
-module) and, when /root/reference is mounted, live against the imported module itself."""
+module) and against the reference module run with this oracle's own weights (tests/golden/reference_cpu.pt)."""
 import os
 
 import pytest
 import torch
 
-from oracle import update as OU, refimport
+from oracle import update as OU
 from oracle.make_golden_update import CASES, make_inputs, small_graph, loop_scatter_softmax_sum
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -45,21 +45,20 @@ def test_scatter_restatement_against_loop_definition():
     assert (y - loop_scatter_softmax_sum(fx, gx, key)).abs().max().item() < 1e-12
 
 
-@pytest.mark.skipif(not refimport.available(), reason="/root/reference not mounted")
 def test_update_oracle_equals_imported_reference_module_live():
+    """against the REFERENCE's dpvo/net.py:Update with the same weights (tests/golden/reference_cpu.pt, written by
+    oracle/make_golden_reference.py)"""
     ii, jj, kk = small_graph(5, 4, 6, 9)
     net, inp, corr, _ = make_inputs(ii.numel(), 123)
     torch.manual_seed(7)
     mine = OU.Update(3).eval()
-    with refimport.reference_modules():
-        import dpvo.net as RN
-        theirs = RN.Update(3).eval()
-        theirs.load_state_dict(mine.state_dict())          # identical key names
-        with torch.no_grad():
-            rn, (rd, rw, _) = theirs(net, inp, corr, None, ii, jj, kk)
+    ref = torch.load(os.path.join(GOLD, "reference_cpu.pt"))["update_live"]
     with torch.no_grad():
         on, (od, ow, _) = mine(net, inp, corr, None, ii, jj, kk)
-    assert torch.equal(on, rn) and torch.equal(od, rd) and torch.equal(ow, rw)
+    # same fp32 op sequence as the reference module; equal up to the BLAS summation order of the host
+    assert (on - ref["net"]).abs().max().item() <= 2e-6 * ref["net"].abs().max().item()
+    assert (od - ref["delta"]).abs().max().item() <= 2e-6 * max(1.0, ref["delta"].abs().max().item())
+    assert (ow - ref["weight"]).abs().max().item() <= 2e-6
 
 
 def test_packed_inference_weights_follow_the_parameters():
