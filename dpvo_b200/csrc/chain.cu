@@ -9,21 +9,28 @@
 // and read back from global memory, one LayerNorm / gating / heads pass over the fp32 state per step, one launch
 // (with its tail wave) per layer.
 //
-// One persistent CTA per SM, warp-specialised:
+// One persistent CTA per SM, in clusters of CH_CL CTAs that work on CH_CL neighbouring tiles at a time and share
+// every weight k-block: each CTA loads 1/CH_CL of its rows from L2 and multicasts them into the weight rings of all CTAs
+// of the cluster, so L2 sends each weight byte once per cluster instead of once per CTA (at one 64-row tile per CTA a
+// weight byte feeds only 64 FLOP: unshared, the weight feed asks more of L2 than the tensor pipe asks of it).  Roles:
 //   warps 0-7  consumers   two warpgroups, warpgroup h owns column half h (192 columns) of the 64-row tile: it issues
 //                          wgmma.m64n192k16 on shared-memory descriptors (a layer is 6 k-blocks x 4 instructions), keeps the
 //                          64 x 192 fp32 accumulator in registers and runs the epilogue from them: bias, activation,
 //                          LayerNorm (row statistics exchanged between the two warps that share a row), gating, heads; the
 //                          fp16 result is written straight into the shared-memory operand tile of the NEXT layer in the
 //                          SWIZZLE_128B K-major layout the descriptors expect.  All parameters sit in shared memory.
-//   warp  8    W producer  streams the weight k-blocks (192 x 64 fp16 = 24 KB) of every layer of every tile through a
-//                          4-deep TMA ring, alternating the column halves; it depends on no data, so it runs ahead across
-//                          layers and tiles
+//                          A stage of the weight ring is handed back to every CTA of the cluster once its MMAs retired.
+//   warp  8    W producer  streams its share of the weight k-blocks (192 x 64 fp16 = 24 KB each) of every layer of every
+//                          tile through a 6-deep TMA ring, alternating the column halves; it depends on no data, so it
+//                          runs ahead across layers and tiles, as far as the slowest CTA of the cluster has freed stages
 //   warp  9    (chain A)   streams the 14 k-blocks of the 896-column correlation rows through the operand slots
 //   warps 9-10 (chain C)   gather the neighbour rows net[ix] (masked) into the operand slots with cp.async
 //   (warps 8-11 form the producer warpgroup; they hand most of their registers to the consumers)
+// Every role of every CTA walks the same tile groups.  When the last group has fewer tiles than the cluster has CTAs,
+// the CTAs without a tile still load their share of every weight k-block, and their consumers wait for and release each
+// stage without computing.
 // Shared memory: 6 operand slots of 64 rows x 64 halves (48 KB, one K=384 activation tile, overwritten in place by the
-// layer's own output once both warpgroups' MMAs have retired), the weight ring (96 KB), the parameter vectors, 2 KB of
+// layer's own output once both warpgroups' MMAs have retired), the weight ring (144 KB), the parameter vectors, 2 KB of
 // exchange.  The fp32 recurrent state is read and written by the consumers directly: a warp's accesses cover 8 rows x
 // 32 contiguous bytes, whole sectors.
 // Row-private intermediates of chain G (the sigmoid gate, the fp32 LayerNorm output that the gated residual adds to)
@@ -33,13 +40,24 @@
 #include "common.cuh"
 #include "tc.cuh"
 #include <cuda.h>
+#include <algorithm>
+#include <atomic>
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
 
 namespace dpvo {
 
 constexpr int CH_M = 64, CH_DIM = 384, CH_KB = 6, CH_NH = 192;
 constexpr int CH_SLOT = CH_M * 128;            // one k-block of the operand tile: 64 rows x 128 bytes
 constexpr int CH_WSTAGE = CH_NH * 128;         // one weight k-block of a column half: 192 rows x 128 bytes
-constexpr int CH_WST = 4;                      // weight ring depth (even: each column half keeps to its own stages)
+constexpr int CH_WST = 6;                      // weight ring depth (even: each column half keeps to its own stages)
+constexpr int CH_CL = 2;                       // CTAs per cluster, sharing every weight k-block
+constexpr int CH_WBOX = CH_NH / CH_CL;         // rows of a weight k-block that one CTA of the cluster loads
+static_assert(CH_WST % 2 == 0, "the column halves alternate through the weight ring");
+// a CTA's share must be whole 8-row SWIZZLE_128B atoms at a 1024-byte aligned offset: the assembled stage is then
+// byte-identical to one 192-row load
+static_assert(CH_NH % CH_CL == 0 && CH_WBOX % 8 == 0, "weight share per CTA");
 constexpr int CH_K0 = 896, CH_KB0 = CH_K0 / 64;
 constexpr int CH_CONS_WARPS = 8, CH_CONS = CH_CONS_WARPS * 32, CH_W_WARP = 8, CH_A_WARP = 9;
 constexpr int CH_GATHER_THREADS = 64;
@@ -56,6 +74,8 @@ struct ChainBars {
 };
 template <int CHAIN> struct ChainCfg {
   static constexpr int NPARAM = CHAIN == 0 ? 7 * CH_DIM : (CHAIN == 1 ? 2 * CH_DIM : 14 * CH_DIM + 8);   // fp32 parameters kept in shared memory
+  // weight k-blocks per tile and column half: A = the K = 896 first layer + 2 layers, C = 2 layers, G = 6 layers
+  static constexpr int KBLOCKS = CHAIN == 0 ? CH_KB0 + 2 * CH_KB : (CHAIN == 1 ? 2 : 6) * CH_KB;
   static constexpr int XCH_BYTES = 2 * CH_M * 16;
   static constexpr int OFF_WRING = CH_KB * CH_SLOT;
   static constexpr int OFF_XCH = OFF_WRING + CH_WST * CH_WSTAGE;
@@ -100,7 +120,7 @@ __device__ __forceinline__ __half2 sigmoid_tanh_h2(float a, float b) {
 }
 
 template <int CHAIN>
-__global__ void __launch_bounds__(CH_THREADS, 1)
+__global__ void __cluster_dims__(CH_CL, 1, 1) __launch_bounds__(CH_THREADS, 1)
 chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW0, const __grid_constant__ CUtensorMap tmW,
              const ChainArgs a) {
   using Cfg = ChainCfg<CHAIN>;
@@ -112,19 +132,24 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
   ChainBars* bars = reinterpret_cast<ChainBars*>(ch_smem + Cfg::OFF_BARS);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t n_tiles = (a.rows + CH_M - 1) / CH_M;
-  constexpr int NLAYERS = CHAIN == CHAIN_A ? 3 : (CHAIN == CHAIN_C ? 2 : 6);
+  const int n_tiles = (int)((a.rows + CH_M - 1) / CH_M);                 // rows < 2^31 (the launchers check)
+  // the CTAs of a cluster are consecutive in blockIdx.x, so the tiles blockIdx.x + k gridDim.x that a CTA takes are, for
+  // each k, one group of CH_CL neighbouring tiles shared by its cluster.  Every role of every CTA walks the tile count
+  // rounded up to whole groups: the CTAs of a cluster share the weight stages and must all run the same number of tiles
+  cg::cluster_group cluster = cg::this_cluster();
+  const uint32_t rank = cluster.block_rank();
+  const int n_walk = (n_tiles + CH_CL - 1) / CH_CL * CH_CL;
 
   if (threadIdx.x == 0) {
     if ((smem_u32(ch_smem) & 1023u) != 0) { printf("chain_kernel: shared memory base is not 1024-byte aligned\n"); __trap(); }
-    // consumer-side arrivals come from lane 0 of every warp that read the stage: 4 per column half, 8 for both
-    for (int s = 0; s < CH_WST; ++s) { mbar_init(&bars->w_full[s], 1); mbar_init(&bars->w_empty[s], 4); }
+    // a stage is released by every warp that read it, in every CTA of the cluster: 4 per column half and CTA
+    for (int s = 0; s < CH_WST; ++s) { mbar_init(&bars->w_full[s], 1); mbar_init(&bars->w_empty[s], 4 * CH_CL); }
     for (int s = 0; s < CH_KB; ++s) { mbar_init(&bars->a_full[s], CHAIN == CHAIN_C ? CH_GATHER_THREADS : 1); mbar_init(&bars->a_empty[s], CH_CONS_WARPS); }
     mbar_init(&bars->slots_free, CH_CONS_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   for (int i = threadIdx.x; i < Cfg::NPARAM; i += blockDim.x) sparam[i] = i < a.n_params ? a.p[i] : 0.f;
-  __syncthreads();
+  cluster.sync();                                                    // no peer multicasts or arrives before the barriers exist
   // 168 registers per thread at launch (3 warpgroups); the consumers hold a 96-register accumulator next to their epilogue
   if (warp >= CH_CONS_WARPS) {
   warpgroup_reg_dealloc<56>();
@@ -132,22 +157,24 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     // ===================================================================== weight producer
     if (lane == 0) {
       uint32_t wit = 0;
-      auto wload = [&](const CUtensorMap* tm, int kcol, int nrow) {
-        const uint32_t s = wit % CH_WST, ph = (wit / CH_WST) & 1;
-        mbar_wait_bounded(&bars->w_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&bars->w_full[s], CH_WSTAGE);
-        tma_load_2d(smem_u32(wring + s * CH_WSTAGE), tm, kcol, nrow, &bars->w_full[s]);
-        ++wit;
-      };
-      for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        if constexpr (CHAIN == CHAIN_A) {
-          for (int kb = 0; kb < CH_KB0; ++kb)
-            for (int h = 0; h < 2; ++h) wload(&tmW0, kb * 64, h * CH_NH);
-        }
-        for (int l = (CHAIN == CHAIN_A ? 1 : 0); l < NLAYERS; ++l) {
-          const int wrow = (CHAIN == CHAIN_A ? l - 1 : l) * CH_DIM;      // row block of the stacked K=384 weights
-          for (int kb = 0; kb < CH_KB; ++kb)
-            for (int h = 0; h < 2; ++h) wload(&tmW, kb * 64, wrow + h * CH_NH);
+      // also a tile past the end: the peers need this CTA's share of its weights
+      for (int tile = blockIdx.x; tile < n_walk; tile += gridDim.x) {
+        for (int i = 0; i < Cfg::KBLOCKS; ++i) {
+          // chain A: the 14 k-blocks of the K = 896 first layer (tmW0), then the K = 384 layers stacked in tmW
+          const bool first = CHAIN == CHAIN_A && i < CH_KB0;
+          const int j = (CHAIN == CHAIN_A && !first) ? i - CH_KB0 : i;
+          const CUtensorMap* tm = first ? &tmW0 : &tmW;
+          const int kcol = (first ? j : j % CH_KB) * 64, wrow = first ? 0 : j / CH_KB * CH_DIM;
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t s = wit % CH_WST, ph = (wit / CH_WST) & 1;
+            mbar_wait_bounded(&bars->w_empty[s], ph ^ 1);              // every CTA of the cluster has released the stage
+            // armed for the whole k-block, this CTA's share and the peers'; a peer's share may complete bytes on this
+            // phase before it is armed
+            mbar_arrive_expect_tx(&bars->w_full[s], CH_WSTAGE);
+            tma_load_2d_multicast(smem_u32(wring + s * CH_WSTAGE + rank * CH_WBOX * 128), tm, kcol, wrow + h * CH_NH + (int)rank * CH_WBOX,
+                                  &bars->w_full[s], (uint16_t)((1u << CH_CL) - 1));
+            ++wit;
+          }
         }
       }
     }
@@ -155,7 +182,8 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     // ===================================================================== chain A: correlation rows, 14 k-blocks
     if (lane == 0) {
       uint32_t ait = 0, ti = 0;
-      for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
+      for (int tile = blockIdx.x; tile < n_walk; tile += gridDim.x, ++ti) {
+        if (tile >= n_tiles) continue;                               // past the end: nothing to load
         if (ti > 0) mbar_wait_bounded(&bars->slots_free, (ti - 1) & 1);   // the previous tile is done with the slots
         const int m0 = (int)(tile * CH_M);
         for (int kb = 0; kb < CH_KB0; ++kb, ++ait) {
@@ -178,7 +206,8 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     int64_t src[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) src[i] = src_of(blockIdx.x, i);
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
+    for (int tile = blockIdx.x; tile < n_walk; tile += gridDim.x, ++ti) {
+      if (tile >= n_tiles) continue;                                 // past the end: nothing to gather
       if (ti > 0) mbar_wait_bounded(&bars->slots_free, (ti - 1) & 1);
 #pragma unroll
       for (int kb = 0; kb < CH_KB; ++kb) {
@@ -216,13 +245,22 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     auto cons_sync = [&]() { named_bar_sync(1, CH_CONS); };          // both warpgroups
     auto pair_sync = [&]() { named_bar_sync(2 + wq, 64); };          // the two warps that share this thread's rows
     auto warp_arrive = [&](uint64_t* bar) { __syncwarp(); if (lane == 0) mbar_arrive(bar); };
+    // a weight stage is free once this warp of every CTA of the cluster is done with it: lane c arrives on CTA c's barrier
+    auto release_w = [&](uint32_t ws) {
+      __syncwarp();
+      if (lane < CH_CL) mbar_arrive_cluster(&bars->w_empty[ws], lane);
+    };
+    auto next_w = [&]() {                                            // wait for this column half's next weight stage
+      const uint32_t ws = wit % CH_WST;
+      mbar_wait_bounded(&bars->w_full[ws], (wit / CH_WST) & 1);
+      wit += 2;
+      return ws;
+    };
     // one k-block of this column half: 4 MMAs on the operand at a_smem, one weight stage; the previous k-block's
     // stages are handed back once its MMAs have retired
     uint32_t prev_w = 0, prev_a = 0;
     auto mma_kblock = [&](uint32_t a_smem, bool first) {
-      const uint32_t ws = wit % CH_WST;
-      mbar_wait_bounded(&bars->w_full[ws], (wit / CH_WST) & 1);
-      wit += 2;
+      const uint32_t ws = next_w();
       const uint64_t ad = wgmma_desc_sw128(a_smem), bd = wgmma_desc_sw128(smem_u32(wring + ws * CH_WSTAGE));
       wgmma_fence();
 #pragma unroll
@@ -233,35 +271,35 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     auto mma_slots = [&]() {                                         // operand = the six slots
       for (int kb = 0; kb < CH_KB; ++kb) {
         const uint32_t ws = mma_kblock(smem_u32(slots + kb * CH_SLOT), kb == 0);
-        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&bars->w_empty[prev_w]); }
+        if (kb > 0) { wgmma_wait<1>(); release_w(prev_w); }
         prev_w = ws;
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      warp_arrive(&bars->w_empty[prev_w]);
+      release_w(prev_w);
     };
     auto mma_gathered = [&](uint32_t ti) {                           // chain C: wait for each gathered k-block
       for (int kb = 0; kb < CH_KB; ++kb) {
         mbar_wait_bounded(&bars->a_full[kb], ti & 1);
         const uint32_t ws = mma_kblock(smem_u32(slots + kb * CH_SLOT), kb == 0);
-        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&bars->w_empty[prev_w]); }
+        if (kb > 0) { wgmma_wait<1>(); release_w(prev_w); }
         prev_w = ws;
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      warp_arrive(&bars->w_empty[prev_w]);
+      release_w(prev_w);
     };
     auto mma_corr = [&]() {                                          // chain A: 14 k-blocks through the slot ring
       for (int kb = 0; kb < CH_KB0; ++kb, ++ait) {
         const uint32_t s = ait % CH_KB;
         mbar_wait_bounded(&bars->a_full[s], (ait / CH_KB) & 1);
         const uint32_t ws = mma_kblock(smem_u32(slots + s * CH_SLOT), kb == 0);
-        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&bars->w_empty[prev_w]); warp_arrive(&bars->a_empty[prev_a]); }
+        if (kb > 0) { wgmma_wait<1>(); release_w(prev_w); warp_arrive(&bars->a_empty[prev_a]); }
         prev_w = ws; prev_a = s;
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      warp_arrive(&bars->w_empty[prev_w]);
+      release_w(prev_w);
       warp_arrive(&bars->a_empty[prev_a]);
     };
     // fp16 activation -> operand slots of the next layer (SWIZZLE_128B K-major).  Both warpgroups' MMAs must have
@@ -385,8 +423,14 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     };
 
     uint32_t ti = 0;
-    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++ti) {
-      const int64_t m0 = tile * CH_M;
+    for (int tile = blockIdx.x; tile < n_walk; tile += gridDim.x, ++ti) {
+      if (tile >= n_tiles) {
+        // past the end (only in the last group): every weight stage the tile would have used is filled for the peers,
+        // so wait for each and hand it back, without MMAs, epilogue or global accesses
+        for (int i = 0; i < Cfg::KBLOCKS; ++i) release_w(next_w());
+        continue;
+      }
+      const int64_t m0 = (int64_t)tile * CH_M;
       int64_t grow[2]; bool live[2];
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) { grow[rr] = m0 + rl + 8 * rr; live[rr] = grow[rr] < a.rows; }
@@ -507,6 +551,7 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
       }
     }
   }
+  cluster.sync();                                                    // no peer still arrives on or writes into this CTA
 }
 
 }  // namespace dpvo
@@ -542,12 +587,40 @@ static int ch_tmap(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int 
 
 struct ChainMaps { CUtensorMap X, W0, W; };
 
+// how many CH_CL-CTA clusters of chain_kernel<CHAIN> the current device runs at once; queried once per device, after the
+// shared-memory attribute is set
+template <int CHAIN>
+static int chain_max_clusters(int* n) {
+  constexpr int kDevices = 64;
+  static std::atomic<int> cached[kDevices];                          // 0 = not queried yet
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return check_cuda(e, "update chain: cudaGetDevice");
+  if (dev < kDevices && (*n = cached[dev].load(std::memory_order_relaxed)) > 0) return DPVO_OK;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(CH_CL);
+  cfg.blockDim = dim3(CH_THREADS);
+  cfg.dynamicSmemBytes = ChainCfg<CHAIN>::SMEM;
+  e = cudaOccupancyMaxActiveClusters(n, chain_kernel<CHAIN>, &cfg);
+  if (e != cudaSuccess) return check_cuda(e, "update chain: cudaOccupancyMaxActiveClusters");
+  if (*n < 1) {
+    set_error("update chain: the device cannot run a cluster of %d chain CTAs (%d bytes of shared memory each)", CH_CL, ChainCfg<CHAIN>::SMEM);
+    return DPVO_ERR_CUDA;
+  }
+  if (dev < kDevices) cached[dev].store(*n, std::memory_order_relaxed);
+  return DPVO_OK;
+}
+
 template <int CHAIN>
 static int chain_launch(const ChainMaps& m, const ChainArgs& a, cudaStream_t st) {
-  const int64_t tiles = (a.rows + CH_M - 1) / CH_M;
-  const unsigned grid = (unsigned)std::min<int64_t>(tiles, sm_count());
   cudaError_t e = cudaFuncSetAttribute(chain_kernel<CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ChainCfg<CHAIN>::SMEM);
   if (e != cudaSuccess) return check_cuda(e, "update chain: cudaFuncSetAttribute");
+  int max_clusters = 0;
+  if (int rc = chain_max_clusters<CHAIN>(&max_clusters)) return rc;
+  const int64_t groups = ((a.rows + CH_M - 1) / CH_M + CH_CL - 1) / CH_CL;
+  // at most one CTA per SM: chain G's scratch holds sm_count() CTA slots, indexed by blockIdx.x
+  const int64_t clusters = std::min<int64_t>({groups, (int64_t)max_clusters, (int64_t)(sm_count() / CH_CL)});
+  const unsigned grid = (unsigned)(clusters * CH_CL);
   chain_kernel<CHAIN><<<grid, CH_THREADS, ChainCfg<CHAIN>::SMEM, st>>>(m.X, m.W0, m.W, a);
   DPVO_LAUNCH_CHECK("chain_kernel");
   return DPVO_OK;
@@ -565,8 +638,8 @@ extern "C" int dpvo_update_corr_norm(const void* corr16, int64_t ld_corr, const 
   ChainMaps m;
   memset(&m, 0, sizeof(m));
   int rc = ch_tmap(&m.X, corr16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, E, CH_K0, ld_corr, 64, CH_M, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.W0, W0, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, CH_DIM, CH_K0, CH_K0, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.W, W25, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (!rc) rc = ch_tmap(&m.W0, W0, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, CH_DIM, CH_K0, CH_K0, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (!rc) rc = ch_tmap(&m.W, W25, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   ChainArgs a;
   memset(&a, 0, sizeof(a));
@@ -583,7 +656,7 @@ extern "C" int dpvo_update_neighbor_mlp(const void* net16_in, const int64_t* ind
   DPVO_REQUIRE(al16(net16_in) && al16(Wab) && al16(params) && al16(net32) && al16(net16_out), "update_neighbor_mlp: pointers must be 16-byte aligned");
   ChainMaps m;
   memset(&m, 0, sizeof(m));
-  int rc = ch_tmap(&m.W, Wab, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
+  int rc = ch_tmap(&m.W, Wab, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   m.X = m.W; m.W0 = m.W;
   ChainArgs a;
@@ -607,7 +680,7 @@ extern "C" int dpvo_update_gru_heads(float* net32, const void* hij16, const int3
   DPVO_REQUIRE(!coords || P >= 1, "update_gru_heads: patch size");
   ChainMaps m;
   memset(&m, 0, sizeof(m));
-  int rc = ch_tmap(&m.W, W6, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 6 * CH_DIM, CH_DIM, CH_DIM, 64, CH_NH, CU_TENSOR_MAP_SWIZZLE_128B);
+  int rc = ch_tmap(&m.W, W6, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 6 * CH_DIM, CH_DIM, CH_DIM, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   m.X = m.W; m.W0 = m.W;
   ChainArgs a;

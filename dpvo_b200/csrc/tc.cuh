@@ -48,6 +48,21 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int 
                "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar))
                : "memory");
 }
+// 2-D TMA tile load multicast to the CTAs of the cluster in cta_mask: the tile lands at the same shared-memory offset in
+// each of them and completes its bytes on the mbarrier at the same offset in each
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar, uint16_t cta_mask) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;\n"
+               ::"r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "h"(cta_mask)
+               : "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (the own rank included).  Used to
+// hand back a stage that was read by wgmma (retired by wgmma.wait_group) and is overwritten by TMA: no generic-proxy
+// accesses to order, so the default .release.cta semantics suffice; .release.cluster would add a MEMBAR.GPU per arrive
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile("{\n.reg .b32 ra;\nmapa.shared::cluster.u32 ra, %0, %1;\nmbarrier.arrive.shared::cluster.b64 _, [ra];\n}\n"
+               ::"r"(smem_u32(bar)), "r"(cta)
+               : "memory");
+}
 // L2 prefetch of a 2-D tile (no shared-memory destination, no completion to wait for)
 __device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];\n" ::"l"(tmap), "r"(c0), "r"(c1) : "memory");

@@ -1,5 +1,7 @@
-"""Times the three fused layer chains of the update operator (csrc/chain.cu) alone, CUDA events, E = 47,712."""
-import sys, os
+"""Times the three fused layer chains of the update operator (csrc/chain.cu) alone, CUDA events, E = 47,712, and prints
+the weight bytes each launch streams: every 64-row tile reads every weight k-block (192 rows x 64 fp16 per column half),
+and the CTAs of a cluster share each k-block, so L2 sends it once per group of CLUSTER tiles."""
+import math, re, sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import dpvo_b200
@@ -18,6 +20,9 @@ W6 = rw(6 * DIM, DIM); pG = torch.randn(14 * DIM + 4, generator=g, device="cuda"
 hij = torch.randn(500, DIM, generator=g, device="cuda").half(); gof = torch.randint(0, 500, (E,), generator=g, device="cuda", dtype=torch.int32)
 coords = torch.randn(E, 2, 3, 3, generator=g, device="cuda")
 ws = torch.empty(ex.update_gru_workspace_bytes(), dtype=torch.uint8, device="cuda")
+CLUSTER = int(re.search(r"constexpr int CH_CL = (\d+);", open(os.path.join(os.path.dirname(dpvo_b200.__file__), "csrc", "chain.cu")).read()).group(1))
+KBLOCKS = {"corr_norm": 2 * (14 + 2 * 6), "neighbor_mlp": 2 * 2 * 6, "gru_heads": 2 * 6 * 6}     # per tile, both column halves
+l2_bytes = {n: math.ceil(math.ceil(E / 64) / CLUSTER) * kb * 192 * 64 * 2 for n, kb in KBLOCKS.items()}
 fl = {"corr_norm": 2.0 * E * (896 * 384 + 2 * 384 * 384), "neighbor_mlp": 2.0 * E * 2 * 384 * 384, "gru_heads": 2.0 * E * 6 * 384 * 384}
 fn = {"corr_norm": lambda: ex.update_corr_norm(corr, W0, W25, pA, net, inp, idx, n16),
       "neighbor_mlp": lambda: ex.update_neighbor_mlp(n16, ix, Wab, pC, net, n16b),
@@ -31,4 +36,6 @@ for name, f in fn.items():
         a.record(); f(); b.record()
     torch.cuda.synchronize()
     t = sorted(a.elapsed_time(b) for a, b in evs)
-    print("%-13s median %.1f us  min %.1f us   %.0f TFLOP/s (median)" % (name, t[len(t) // 2] * 1e3, t[0] * 1e3, fl[name] / (t[len(t) // 2] * 1e-3) / 1e12))
+    med = t[len(t) // 2] * 1e-3
+    print("%-13s median %.1f us  min %.1f us   %.0f TFLOP/s   weights %.3f GB into shared memory, %.3f GB from L2 (cluster %d), %.0f GB/s L2 -> SM (median)"
+          % (name, med * 1e6, t[0] * 1e3, fl[name] / med / 1e12, l2_bytes[name] * CLUSTER / 1e9, l2_bytes[name] / 1e9, CLUSTER, l2_bytes[name] / med / 1e9))
