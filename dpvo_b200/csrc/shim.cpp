@@ -551,6 +551,39 @@ Tensor softagg_reduce(Tensor fg, Tensor order, Tensor group_start, Tensor n_grou
   return y;
 }
 
+// x: [.., E, dim] fp16; w [2*dim, dim] fp16 / bias [2*dim] fp32 with the f and g rows interleaved by 96-channel slice
+Tensor softagg_fused(Tensor x, Tensor order, Tensor group_of, Tensor group_start, Tensor n_groups, int64_t max_groups, Tensor w,
+                     Tensor bias, c10::optional<Tensor> workspace) {
+  need_cuda(x, "x");
+  c10::cuda::CUDAGuard guard(x.device());
+  TORCH_CHECK(x.scalar_type() == at::kHalf && x.stride(-1) == 1, "softagg_fused: x must be float16 with contiguous rows");
+  const int dim = x.size(-1);
+  Tensor x2 = x.dim() == 2 ? x : x.reshape({-1, dim});
+  const int64_t E = x2.size(0);
+  TORCH_CHECK(w.is_cuda() && w.scalar_type() == at::kHalf && w.is_contiguous() && w.dim() == 2 && w.size(0) == 2 * dim && w.size(1) == dim,
+              "softagg_fused: w must be a contiguous float16 CUDA tensor [2*dim, dim]");
+  TORCH_CHECK(bias.is_cuda() && bias.scalar_type() == at::kFloat && bias.is_contiguous() && bias.numel() == 2 * dim,
+              "softagg_fused: bias must be a contiguous float32 CUDA tensor [2*dim]");
+  for (const Tensor* t : {&order, &group_of})
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == E,
+                "softagg_fused: order and group_of must be contiguous int32 CUDA tensors with one entry per row of x");
+  TORCH_CHECK(group_start.is_cuda() && group_start.scalar_type() == at::kInt && group_start.is_contiguous() && group_start.numel() >= max_groups + 1,
+              "softagg_fused: group_start must be int32 with at least max_groups + 1 entries");
+  TORCH_CHECK(n_groups.is_cuda() && n_groups.scalar_type() == at::kInt && n_groups.numel() == 1, "softagg_fused: n_groups must be a device int32 scalar");
+  TORCH_CHECK(max_groups >= 0 && max_groups <= E, "softagg_fused: max_groups must be in [0, E]");
+  const int64_t wsb = dpvo_softagg_fused_workspace_bytes(E);
+  Tensor ws = workspace.has_value() ? *workspace : byte_ws(wsb, x);
+  TORCH_CHECK(ws.is_cuda() && ws.is_contiguous() && (int64_t)(ws.numel() * ws.element_size()) >= wsb, "softagg_fused: workspace too small");
+  Tensor y = torch::empty({1, max_groups, dim}, x.options());   // rows past the group count are zeroed by the op itself
+  check(dpvo_softagg_fused(x2.data_ptr(), x2.stride(0), order.data_ptr<int>(), group_of.data_ptr<int>(), group_start.data_ptr<int>(),
+                           n_groups.data_ptr<int>(), w.data_ptr(), bias.data_ptr<float>(), E, max_groups, y.data_ptr(),
+                           ws.data_ptr(), wsb, dim, stream()),
+        "dpvo_b200_ext.softagg_fused");
+  return y;
+}
+
+int64_t softagg_fused_workspace_bytes(int64_t E) { return dpvo_softagg_fused_workspace_bytes(E); }
+
 // Y = epilogue(X @ W^T + bias) on wgmma; X [.., rows, K] fp16 (row stride may exceed K), W [N, K] fp16
 Tensor linear_f16(Tensor x, Tensor w, c10::optional<Tensor> bias, int64_t epilogue, c10::optional<Tensor> res,
                   c10::optional<Tensor> gate, c10::optional<Tensor> gather, bool out_f32, c10::optional<Tensor> out,
@@ -812,6 +845,10 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("residual_sum16", &residual_sum16, "fp16(net + u[group]) without updating net", py::arg("net32"), py::arg("u"), py::arg("group_of") = py::none());
   m.def("gated_residual", &gated_residual, "x + sigmoid(g) * r");
   m.def("softagg_reduce", &softagg_reduce, "segment softmax-weighted sum");
+  m.def("softagg_fused", &softagg_fused, "SoftAgg f|g layer fused with its segment softmax-weighted sum", py::arg("x"), py::arg("order"),
+        py::arg("group_of"), py::arg("group_start"), py::arg("n_groups"), py::arg("max_groups"), py::arg("w"), py::arg("bias"),
+        py::arg("workspace") = py::none());
+  m.def("softagg_fused_workspace_bytes", &softagg_fused_workspace_bytes, "scratch bytes of softagg_fused for E rows");
   m.def("update_heads", &update_heads, "delta / weight heads (optionally emitting the BA target)", py::arg("net32"), py::arg("W4"),
         py::arg("b4"), py::arg("coords") = py::none(), py::arg("gate") = py::none(), py::arg("res") = py::none());
   m.def("linear_f16", &linear_f16, "wgmma dense layer", py::arg("x"), py::arg("w"), py::arg("bias") = py::none(),

@@ -10,8 +10,9 @@ Data flow is fp32 for the carried state `net`, fp16 for every GEMM operand (what
 autocast does, dpvo.py:332), with the fp16 copies produced inside the fused row kernels.  The edge
 groupings come from ONE device radix-sort launch each (no host sync, no torch.unique, no D2H sort).
 
-Every dense layer runs on hand-written wgmma kernels (csrc/chain.cu: the three fused layer chains; csrc/gemm.cu:
-dpvo_linear_f16 for the four SoftAgg layers); there is no library GEMM and no other backend.
+Every dense layer runs on hand-written wgmma kernels (csrc/chain.cu: the three fused layer chains; csrc/softagg.cu:
+each SoftAgg's f|g layer fused with its segment softmax; csrc/gemm.cu: dpvo_linear_f16 for the two SoftAgg h layers);
+there is no library GEMM and no other backend.
 """
 import torch
 import torch.nn as nn
@@ -50,7 +51,7 @@ class GatedResidual(nn.Module):
 
 
 class SoftAgg(nn.Module):
-    """blocks.py:31-48.  Inference: parameters only, the reduction runs in dpvo_softagg_reduce.  Training:
+    """blocks.py:31-48.  Inference: parameters only, f|g and the reduction run in dpvo_softagg_fused.  Training:
     `forward(x, group_of, n_groups)` is the differentiable fp32 form -- a per-group softmax of g(x) weighting f(x),
     summed per group, mapped by h and handed back to every member; group ids come from the device grouping kernel
     (no torch.unique), the per-group max / sums are index reductions."""
@@ -142,9 +143,14 @@ class Update(nn.Module):
         P["corr0"] = (F.pad(w0, (0, CORR_PAD - w0.shape[1])).contiguous(), b0)
         P["c1a"], P["c1b"], P["c2a"], P["c2b"] = lin(self.c1[0]), lin(self.c1[2]), lin(self.c2[0]), lin(self.c2[2])
         for nm, agg in (("kk", self.agg_kk), ("ij", self.agg_ij)):
-            # f and g share their input: one GEMM with N = 768
+            # f and g stacked for one linear_f16 with N = 768: the two-kernel form (linear_f16 + softagg_reduce) that the
+            # fused op is tested and timed against
             P["fg_" + nm] = (torch.cat([agg.f.weight, agg.g.weight], 0).detach().half().contiguous(),
                              torch.cat([agg.f.bias, agg.g.bias], 0).detach().float().contiguous())
+            # dpvo_softagg_fused: the f and g rows interleaved by 96-channel slice, [f 0..95; g 0..95; f 96..191; ...]
+            def il(f, g):
+                return torch.stack([f.reshape(DIM // 96, 96, -1), g.reshape(DIM // 96, 96, -1)], 1).reshape(2 * DIM, -1).detach()
+            P["fgi_" + nm] = (il(agg.f.weight, agg.g.weight).half().contiguous(), il(agg.f.bias, agg.g.bias).reshape(-1).float().contiguous())
             P["h_" + nm] = lin(agg.h)
         for i, blk in ((1, self.gru[1]), (3, self.gru[3])):
             P["gr%d_g" % i], P["gr%d_a" % i], P["gr%d_b" % i] = lin(blk.gate[0]), lin(blk.res[0]), lin(blk.res[2])
@@ -219,7 +225,7 @@ class Update(nn.Module):
     def _forward_chains(self, net, inp, corr, groups_kk, groups_ij):
         """The row-local stretches of net.py:74-92 as one wgmma chain kernel each (csrc/chain.cu): corr MLP + context
         add + LayerNorm; c1 and c2 on the masked temporal neighbours; group add + GRU + heads.  Between them only the two
-        SoftAgg reductions (which mix rows of a group) run as separate kernels."""
+        SoftAgg aggregations (which mix rows of a group) run as separate kernels."""
         ex = extensions()[3]
         P = self.packed()
         inplace = net.dtype == torch.float32 and net.is_contiguous() and self.inplace_state
@@ -244,12 +250,14 @@ class Update(nn.Module):
         ix, jx = ex.neighbors_from_groups(groups_kk.order, groups_kk.group_of)
         n16b = timed(ex.update_neighbor_mlp, n16, ix, P["C1_W"], P["C1_p"], net32)
         n16 = timed(ex.update_neighbor_mlp, n16b, jx, P["C2_W"], P["C2_p"], net32, n16)
-        y = ex.softagg_reduce(L(n16, "fg_kk"), groups_kk.order, groups_kk.group_start, groups_kk.n, groups_kk.max_groups)
+        def agg(x, grp, name):                            # the f|g layer and its segment softmax in one op
+            return timed(ex.softagg_fused, x, grp.order, grp.group_of, grp.group_start, grp.n, grp.max_groups, *P[name])
+        y = agg(n16, groups_kk, "fgi_kk")
         # net + agg_kk(net) is only needed as the fp16 operand of the next aggregation; the fp32 state itself takes both
         # aggregation results in the prologue of the GRU chain (net.py:87-88), one pass over the state instead of two
         h_kk = L(y, "h_kk").reshape(-1, DIM)
         n16 = ex.residual_sum16(net32, h_kk, groups_kk.group_of)
-        y = ex.softagg_reduce(L(n16, "fg_ij"), groups_ij.order, groups_ij.group_start, groups_ij.n, groups_ij.max_groups)
+        y = agg(n16, groups_ij, "fgi_ij")
         h_ij = L(y, "h_ij")
         delta, weight = timed(ex.update_gru_heads, net32, h_ij.reshape(-1, DIM), groups_ij.group_of, P["G_W6"], P["G_p"], self._coords, None,
                               h_kk, groups_kk.group_of)

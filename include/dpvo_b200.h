@@ -371,6 +371,22 @@ int dpvo_softagg_reduce(const void* f16, const void* g16, int64_t ld, const int3
                         const int32_t* n_groups, int64_t max_groups, void* y16, int dim, void* stream);
 
 /*
+ * SoftAgg f|g layer fused with its reduction (blocks.py:31-43): y as dpvo_softagg_reduce computes it from
+ *   f = fp16(x Wf^T + bf), gl = fp16(x Wg^T + bg)
+ * without the [E, 2*dim] layer output.  x16 fp16 [E, dim] (row stride ldx, rows 16-byte aligned) is read in the
+ * sorted order of the CSR (order, group_of, group_start; G read from n_groups on the device).  w16 fp16 [2*dim, dim]
+ * and bias fp32 [2*dim] hold the f and g rows interleaved by 96-channel slice: rows 192 s .. 192 s + 95 are
+ * Wf rows 96 s .. 96 s + 95, rows 192 s + 96 .. 192 s + 191 are Wg rows 96 s .. 96 s + 95.  y fp16 [max_groups, dim];
+ * rows G .. max_groups - 1 are zero.  dim = 384.  workspace: dpvo_softagg_fused_workspace_bytes(E) bytes
+ * (partial results of the groups that span more than one 64-row tile).  Two launches give bit-identical results.
+ */
+int64_t dpvo_softagg_fused_workspace_bytes(int64_t E);
+int dpvo_softagg_fused(const void* x16, int64_t ldx, const int32_t* order, const int32_t* group_of,
+                       const int32_t* group_start, const int32_t* n_groups, const void* w16, const float* bias,
+                       int64_t E, int64_t max_groups, void* y16, void* workspace, int64_t workspace_bytes,
+                       int dim, void* stream);
+
+/*
  * The two output heads (net.py:62-71, 92): delta = Wd relu(net) + bd, weight = sigmoid(Ww relu(net) + bw).
  * W4 fp32 [4, dim] = rows (Wd[0], Wd[1], Ww[0], Ww[1]); b4 fp32 [4]; delta, weight fp32 [rows, 2].
  * coords (optional, fp32 [rows, 2, P, P]): when given, `delta` receives the BA target
