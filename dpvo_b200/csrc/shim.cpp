@@ -788,6 +788,101 @@ std::vector<Tensor> pgraph_new_edges(Tensor n_dev, int64_t M, int64_t r) {
   return {ii, jj, kk};
 }
 
+// ------------------------------------------------------------------------------ frame encoders
+struct EncShape { int ks, s, cin, cout; };
+const EncShape kEncShapes[] = {{7, 2, 3, 32}, {3, 1, 32, 32}, {3, 2, 32, 64}, {1, 2, 32, 64}, {3, 1, 64, 64}, {1, 1, 64, 128}, {1, 1, 64, 384}};
+
+void enc_f16(const Tensor& t, const char* name) {
+  need_cuda(t, name);
+  TORCH_CHECK(t.scalar_type() == at::kHalf && t.is_contiguous(), "encoder_conv: ", name, " must be a contiguous float16 CUDA tensor");
+}
+void enc_f32(const Tensor& t, int64_t n, const char* name) {
+  need_cuda(t, name);
+  TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == n, "encoder_conv: ", name,
+              " must be a contiguous float32 CUDA tensor of ", n, " elements");
+}
+
+// one layer of one encoder; returns (y [Ho, Wo, cout], stats [2, cout] or None, joined [H, W, cin] or None, pool or None)
+std::vector<c10::optional<Tensor>> encoder_conv(int64_t shape, Tensor x, Tensor w, Tensor bias, c10::optional<Tensor> x_stats, bool x_relu,
+                                                c10::optional<Tensor> skip, c10::optional<Tensor> skip_stats, bool skip_relu,
+                                                bool want_joined, bool want_stats, bool want_pool, double scale) {
+  TORCH_CHECK(shape >= 0 && shape < 7, "encoder_conv: unknown shape ", shape);
+  const EncShape sh = kEncShapes[shape];
+  const bool stem = shape == DPVO_ENC_STEM;
+  need_cuda(x, "x");
+  int H, W;
+  dpvo_encoder_conv_io io{};
+  if (stem) {
+    TORCH_CHECK(x.scalar_type() == at::kByte && x.dim() == 3 && x.size(0) == 3, "encoder_conv: the stem takes a uint8 image [3, H, W]");
+    H = (int)x.size(1); W = (int)x.size(2);
+    io.x_strides[0] = x.stride(0); io.x_strides[1] = x.stride(1); io.x_strides[2] = x.stride(2);
+  } else {
+    enc_f16(x, "x");
+    TORCH_CHECK(x.dim() == 3 && x.size(2) == sh.cin, "encoder_conv: x must be NHWC [H, W, ", sh.cin, "]");
+    H = (int)x.size(0); W = (int)x.size(1);
+  }
+  const int Ho = (H + 2 * (sh.ks / 2) - sh.ks) / sh.s + 1, Wo = (W + 2 * (sh.ks / 2) - sh.ks) / sh.s + 1;
+  enc_f16(w, "w");
+  const int64_t taps = stem ? 1 : sh.ks * sh.ks, kc = stem ? 20 : sh.cin / 8;
+  TORCH_CHECK(w.numel() == taps * kc * sh.cout * 8, "encoder_conv: w must hold the packed layer (", taps * kc * sh.cout * 8, " halves)");
+  enc_f32(bias, sh.cout, "bias");
+  Tensor xs, ss, sk;
+  if (x_stats.has_value()) { xs = *x_stats; enc_f32(xs, 2 * sh.cin, "x_stats"); }
+  if (skip.has_value()) { sk = *skip; enc_f16(sk, "skip"); TORCH_CHECK(sk.sizes() == x.sizes(), "encoder_conv: skip must match x"); }
+  if (skip_stats.has_value()) { ss = *skip_stats; enc_f32(ss, 2 * sh.cin, "skip_stats"); }
+  auto opt16 = x.options().dtype(at::kHalf);
+  Tensor y = torch::empty({Ho, Wo, sh.cout}, opt16);
+  c10::optional<Tensor> st, jn, pl;
+  if (want_stats) st = torch::empty({2, sh.cout}, x.options().dtype(at::kFloat));
+  if (want_joined) jn = torch::empty({H, W, sh.cin}, opt16);
+  if (want_pool) pl = torch::empty({Ho / 4, Wo / 4, sh.cout}, opt16);
+  io.x = x.data_ptr(); io.x_stats = xs.defined() ? xs.data_ptr<float>() : nullptr; io.x_relu = x_relu;
+  io.skip = sk.defined() ? sk.data_ptr() : nullptr; io.skip_stats = ss.defined() ? ss.data_ptr<float>() : nullptr; io.skip_relu = skip_relu;
+  io.joined = jn ? jn->data_ptr() : nullptr;
+  io.w = w.data_ptr(); io.bias = bias.data_ptr<float>();
+  io.y = y.data_ptr(); io.y_sy = (int64_t)Wo * sh.cout; io.y_sx = sh.cout;
+  io.pool = pl ? pl->data_ptr() : nullptr; io.pool_sy = (int64_t)(Wo / 4) * sh.cout; io.pool_sx = sh.cout;
+  io.stats = st ? st->data_ptr<float>() : nullptr; io.scale = (float)scale;
+  const int64_t wsb = dpvo_encoder_conv_workspace_bytes((int)shape, H, W);
+  Tensor ws = byte_ws(wsb, x);
+  const c10::cuda::CUDAGuard guard(x.device());
+  check(dpvo_encoder_conv((int)shape, H, W, 1, &io, ws.data_ptr(), wsb, stream()), "dpvo_b200_ext.encoder_conv");
+  return {y, st, jn, pl};
+}
+
+void encode_frame(Tensor image, Tensor w16, Tensor b32, Tensor coords, Tensor fmap1, Tensor fmap2, Tensor gmap, Tensor imap,
+                  Tensor patches, Tensor workspace) {
+  for (auto* t : {&image, &w16, &b32, &coords, &fmap1, &fmap2, &gmap, &imap, &patches, &workspace})
+    TORCH_CHECK(t->is_cuda(), "encode_frame: every tensor must be a CUDA tensor (this build has no CPU path)");
+  TORCH_CHECK(image.scalar_type() == at::kByte && image.dim() == 3 && image.size(0) == 3, "encode_frame: image must be uint8 [3, H, W]");
+  const int H = (int)image.size(1), W = (int)image.size(2);
+  const int h = ((H - 1) / 2 + 1 - 1) / 2 + 1, w = ((W - 1) / 2 + 1 - 1) / 2 + 1;
+  TORCH_CHECK(w16.scalar_type() == at::kHalf && w16.is_contiguous(), "encode_frame: w16 must be contiguous float16");
+  TORCH_CHECK(b32.scalar_type() == at::kFloat && b32.is_contiguous() && b32.numel() == 2 * 11 * 384, "encode_frame: b32 must be float32 [2, 11, 384]");
+  TORCH_CHECK(coords.scalar_type() == at::kFloat && coords.is_contiguous() && coords.dim() == 2 && coords.size(1) == 2, "encode_frame: coords must be contiguous float32 [M, 2]");
+  const int64_t M = coords.size(0);
+  TORCH_CHECK(fmap1.scalar_type() == at::kHalf && fmap1.dim() == 3 && fmap1.size(2) == 128 && fmap1.stride(2) == 1,
+              "encode_frame: fmap1 must be a channels-last float16 slot [h, w, 128]");
+  TORCH_CHECK(fmap1.size(0) == h && fmap1.size(1) == w, "encode_frame: a ", H, "x", W, " image encodes to ", h, "x", w,
+              ", the fmap1 slot is ", fmap1.size(0), "x", fmap1.size(1));
+  TORCH_CHECK(fmap2.scalar_type() == at::kHalf && fmap2.dim() == 3 && fmap2.size(0) == h / 4 && fmap2.size(1) == w / 4 && fmap2.size(2) == 128 &&
+              fmap2.stride(2) == 1, "encode_frame: fmap2 must be a channels-last float16 slot [h/4, w/4, 128]");
+  TORCH_CHECK(gmap.scalar_type() == at::kHalf && gmap.dim() == 4 && gmap.size(0) == M && gmap.size(1) == 3 && gmap.size(2) == 3 &&
+              gmap.size(3) == 128 && gmap.stride(3) == 1, "encode_frame: gmap must be a channels-last float16 slot [M, 3, 3, 128]");
+  TORCH_CHECK(imap.scalar_type() == at::kHalf && imap.dim() == 2 && imap.size(0) == M && imap.size(1) == 384 && imap.stride(1) == 1,
+              "encode_frame: imap must be float16 [M, 384] with contiguous rows");
+  TORCH_CHECK(patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() == M * 27, "encode_frame: patches must be contiguous float32 [M, 3, 3, 3]");
+  TORCH_CHECK(workspace.is_contiguous(), "encode_frame: workspace must be contiguous");
+  const c10::cuda::CUDAGuard guard(image.device());
+  check(dpvo_encode_frame(image.data_ptr<uint8_t>(), image.stride(0), image.stride(1), image.stride(2), H, W, w16.data_ptr(), b32.data_ptr<float>(),
+                          coords.data_ptr<float>(), (int)M, fmap1.data_ptr(), fmap1.stride(0), fmap1.stride(1), fmap2.data_ptr(), fmap2.stride(0),
+                          fmap2.stride(1), gmap.data_ptr(), gmap.stride(0), gmap.stride(1), gmap.stride(2), imap.data_ptr(), imap.stride(0),
+                          patches.data_ptr<float>(), workspace.data_ptr(), workspace.numel() * workspace.element_size(), stream()),
+        "dpvo_b200_ext.encode_frame");
+}
+
+int64_t encode_frame_workspace_bytes(int64_t H, int64_t W) { return dpvo_encode_frame_workspace_bytes((int)H, (int)W); }
+
 int64_t launch_count() { return dpvo_launch_count(); }
 std::string version() { return dpvo_version(); }
 
@@ -867,6 +962,14 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
         py::arg("new_jj"), py::arg("new_kk"), py::arg("enable"), py::arg("state"), py::arg("n_active"), py::arg("overflow"));
   m.def("pgraph_new_edges", &pgraph_new_edges, "steady-state forward + backward edges of the newest frame");
   m.def("neighbors_from_groups", &neighbors_from_groups, "temporal neighbours from a kk/jj grouping");
+  m.def("encoder_conv", &encoder_conv, "one frame-encoder convolution (tensor cores, fused norm / join prologue)", py::arg("shape"),
+        py::arg("x"), py::arg("w"), py::arg("bias"), py::arg("x_stats") = py::none(), py::arg("x_relu") = false, py::arg("skip") = py::none(),
+        py::arg("skip_stats") = py::none(), py::arg("skip_relu") = false, py::arg("want_joined") = false, py::arg("want_stats") = false,
+        py::arg("want_pool") = false, py::arg("scale") = 1.0);
+  m.def("encode_frame", &encode_frame, "both frame encoders: uint8 image -> fmap1, fmap2, gmap, imap, patches slots", py::arg("image"),
+        py::arg("w16"), py::arg("b32"), py::arg("coords"), py::arg("fmap1"), py::arg("fmap2"), py::arg("gmap"), py::arg("imap"),
+        py::arg("patches"), py::arg("workspace"));
+  m.def("encode_frame_workspace_bytes", &encode_frame_workspace_bytes, "scratch bytes of encode_frame for an H x W image");
   m.def("launch_count", &launch_count, "kernel launches issued by libdpvo_b200 so far");
   m.def("version", &version, "library version string");
 }

@@ -13,16 +13,19 @@ from . import extensions
 from . import altcorr, fastba
 from . import projective_ops as pops
 from .net import Update, EdgeGroups, DIM
+from .frontend import encoder_output_size
 
 
 class UpdateRunner:
-    def __init__(self, state, update=None, ba_iterations=2, seed=1234, graph=None):
-        """graph: optional DevicePatchGraph (patchgraph.py).  With it the edge lists and the recurrent state are the
+    def __init__(self, state, update=None, ba_iterations=2, seed=1234, graph=None, encoder=None):
+        """encoder: optional frontend.FrameEncoder, which `ingest_image` runs.
+        graph: optional DevicePatchGraph (patchgraph.py).  With it the edge lists and the recurrent state are the
         store's fixed-capacity arrays: every kernel runs over all `cap` slots, parked slots are dummy edges in groups of
         their own whose confidence weights are zeroed before bundle adjustment, and a captured CUDA graph of step()
         stays valid while edges are appended and removed between replays."""
         self.s = state
         self.pg = graph
+        self.encoder = encoder
         dev = state.poses.device
         if update is None:
             torch.manual_seed(seed)                    # evaluate_tartan.py:173
@@ -148,6 +151,33 @@ class UpdateRunner:
         s.patches[(s.n - 1) * self.M:s.n * self.M].copy_(hf["patches"], non_blocking=True)
         s.poses[s.n - 1].copy_(hf["pose"], non_blocking=True)
         return sum(v.numel() * v.element_size() for v in hf.values())
+
+    @torch.no_grad()
+    def ingest_image(self, image, depth=None, coords=None):
+        """Encode a uint8 camera image [3, H, W] (CHW or HWC strides) straight into the slots `ingest_frame` writes:
+        fmap1 / fmap2 slot (n-1) % mem, gmap / imap slot (n-1) % pmem, patches[(n-1) M : n M] (dpvo.py:389-438).
+        Centroids are drawn as Patchifier.forward draws them, unless `coords` [M, 2] is given (CUDA-graph capture);
+        the patch depths are then one torch.rand draw (dpvo.py:427), or `depth` (the median the caller computes once
+        initialised, dpvo.py:429-431).  Poses, intrinsics and the motion model stay with the caller.  Returns the
+        centroids."""
+        if self.encoder is None:
+            raise RuntimeError("ingest_image: this UpdateRunner was built without an encoder")
+        s, M = self.s, self.M
+        h, w = s.fmap1.shape[3], s.fmap1.shape[4]
+        if image.dim() != 3 or encoder_output_size(image.shape[1], image.shape[2]) != (h, w):
+            raise RuntimeError("ingest_image: a %s image encodes to %s features, the rings hold %dx%d"
+                               % (tuple(image.shape), encoder_output_size(*image.shape[-2:]) if image.dim() >= 2 else None, h, w))
+        slot = (s.n - 1) % self.mem
+        pslot = (s.n - 1) % self.pmem
+        patches = s.patches[(s.n - 1) * M:s.n * M]
+        coords = self.encoder.encode_into(image, M, self.encoder.strategy, s.fmap1[0, slot].permute(1, 2, 0),
+                                          s.fmap2[0, slot].permute(1, 2, 0),
+                                          s.gmap[0, pslot * M:(pslot + 1) * M].permute(0, 2, 3, 1),
+                                          s.imap[0, pslot * M:(pslot + 1) * M], patches, coords=coords)
+        if depth is None:
+            depth = torch.rand(M, 1, 1, device=patches.device, dtype=patches.dtype)
+        patches[:, 2] = depth
+        return coords
 
     # A streaming front end has frame t+1 in pinned memory while update t runs: its H2D copy goes to a staging
     # buffer on a copy stream (overlapping the update), and only the short device-to-device move into the ring

@@ -489,6 +489,80 @@ int dpvo_pgraph_append(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* active, i
                        float* state, int32_t* slot_of_new, int32_t* n_active, int32_t* overflow, void* stream);
 int dpvo_pgraph_new_edges(const int64_t* n_dev, int M, int r, int64_t* ii, int64_t* jj, int64_t* kk, void* stream);
 
+/* ---- Frame encoders (dpvo_b200/csrc/encoder.cu) ---------------------------------------------------------------------
+ * BasicEncoder4 (extractor.py:200-264) as used by Patchifier (net.py:95-157) for inference: fnet (instance norm after
+ * every convolution but the last, output 128) and inet (no norm, output 384).  Activations are NHWC fp16, convolutions
+ * run on the tensor cores with fp32 accumulation and round their output to fp16.
+ *
+ * Packed weights (FrameEncoder.pack()):
+ *   w16  fp16 blob: for encoder e = fnet, inet and layer l = 0..10 in the order
+ *          conv1 (stem), layer1.0.conv1, layer1.0.conv2, layer1.1.conv1, layer1.1.conv2, layer2.0.conv1,
+ *          layer2.0.downsample.0, layer2.0.conv2, layer2.1.conv1, layer2.1.conv2, conv2 (output)
+ *        the layer's weight W[cout][cin][ky][kx] as [tap = ky*k + kx][cin / 8][cout][cin % 8], back to back.  The stem
+ *        is one tap with K = (cin*7 + ky)*7 + kx (147, zero-padded to 160) in place of cin.
+ *   b32  fp32 [2][11][384]: the biases, zero-padded.
+ *
+ * dpvo_encoder_conv: one layer for nenc (1 or 2) encoders, io[e] describing encoder e.  shape is a DPVO_ENC_* value.
+ *   prologue: stem: x is the uint8 image [3, H, W] with element strides x_strides (c, y, x), normalised as
+ *                   fp16(2 (x / 255) - 0.5) (dpvo.py:389).
+ *             otherwise x is fp16 NHWC [H, W, cin] dense and is transformed as
+ *                   x' = relu?((x - mean) * rstd)    (x_stats [2][cin] = (mean, rstd), or NULL for none; x_relu)
+ *                   skip given: x' = relu(skip' + x'),  skip' = relu?((skip - mean) * rstd) by skip_stats / skip_relu
+ *             out-of-image taps read 0 after the transform.  joined (3x3 layers with skip): x' of every pixel is also
+ *             written there, fp16 NHWC [H, W, cin].
+ *   epilogue: y = fp16((conv(x') + bias) * scale), pixel strides y_sy, y_sx, channel stride 1.
+ *             pool (optional): fp16 4x4 average of y (F.avg_pool2d order), strides pool_sy, pool_sx.
+ *             stats (optional, cout <= 64): [2][cout] (mean, 1/sqrt(var + 1e-5)) of the fp16 y over the image.
+ *   workspace: dpvo_encoder_conv_workspace_bytes(shape, H, W) bytes when any stats are requested.
+ *   Output size: (H + 2 (k/2) - k) / s + 1.  No float atomics: two launches give identical bits.
+ *
+ * dpvo_encode_frame: both encoders over one uint8 image [3, H, W] (element strides s_c, s_y, s_x), about a dozen
+ * launches, writing a new frame's slots directly (all channels-last, channel stride 1):
+ *   fmap1  fp16 [h, w, 128]     fnet(image) / 4                      (pixel strides f1_sy, f1_sx)
+ *   fmap2  fp16 [h/4, w/4, 128] F.avg_pool2d(fmap1, 4, 4)            (f2_sy, f2_sx)
+ *   imap   fp16 [M, 384]        inet(image) / 4 at the centroids      (row stride i_sm)
+ *   gmap   fp16 [M, 3, 3, 128]  the 3x3 windows of fmap1 at the centroids (strides g_sm, g_sy, g_sx)
+ *   patches fp32 [M, 3, 3, 3]   (x + dx, y + dy, 1) around each centroid, contiguous
+ * coords fp32 [M, 2] (x, y) integer centroids.  h, w = the encoder output size of H, W.
+ * workspace: dpvo_encode_frame_workspace_bytes(H, W) bytes (activations, statistics).
+ */
+#define DPVO_ENC_STEM        0   /* 7x7/2, 3 -> 32   */
+#define DPVO_ENC_C3_32       1   /* 3x3/1, 32 -> 32  */
+#define DPVO_ENC_C3S2_32_64  2   /* 3x3/2, 32 -> 64  */
+#define DPVO_ENC_C1S2_32_64  3   /* 1x1/2, 32 -> 64  */
+#define DPVO_ENC_C3_64       4   /* 3x3/1, 64 -> 64  */
+#define DPVO_ENC_OUT_128     5   /* 1x1/1, 64 -> 128 */
+#define DPVO_ENC_OUT_384     6   /* 1x1/1, 64 -> 384 */
+
+typedef struct dpvo_encoder_conv_io {
+  const void* x;
+  int64_t x_strides[3];
+  const float* x_stats;
+  int x_relu;
+  const void* skip;
+  const float* skip_stats;
+  int skip_relu;
+  void* joined;
+  const void* w;
+  const float* bias;
+  void* y;
+  int64_t y_sy, y_sx;
+  void* pool;
+  int64_t pool_sy, pool_sx;
+  float* stats;
+  float scale;
+} dpvo_encoder_conv_io;
+
+int64_t dpvo_encoder_conv_workspace_bytes(int shape, int H, int W);
+int dpvo_encoder_conv(int shape, int H, int W, int nenc, const dpvo_encoder_conv_io* io, void* workspace,
+                      int64_t workspace_bytes, void* stream);
+int64_t dpvo_encode_frame_workspace_bytes(int H, int W);
+int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y, int64_t s_x, int H, int W,
+                      const void* w16, const float* b32, const float* coords, int M,
+                      void* fmap1, int64_t f1_sy, int64_t f1_sx, void* fmap2, int64_t f2_sy, int64_t f2_sx,
+                      void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm,
+                      float* patches, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
