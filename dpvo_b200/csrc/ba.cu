@@ -16,6 +16,8 @@
 //       * CTA 0 assembles B from the pair records, applies the damping, Cholesky-factors and
 //         solves the 6N x 6N system in shared memory, retracts the poses
 //       * all CTAs back-substitute the depth updates and retract the patches
+//   batched (ba_reduce_batched_kernel, ba_solve_batched_kernel): B streams' independent windows in the same two
+//       launches, each stream on its slice of the shared groupings and scratch, one 8-CTA cluster per stream
 // Results are bit-reproducible run to run (the reference's are not: unordered atomics).
 #include "common.cuh"
 #include "ba_edge.cuh"
@@ -75,9 +77,55 @@ __device__ __forceinline__ int ba_tri(int N6, int r, int c) { return r * N6 - (r
 // to warps statically, a warp applies its items in order, the copies of a CTA are added in warp order and the CTAs'
 // partial systems are summed in CTA order by the solve kernel: still no float atomics, still bit-reproducible.
 // A copy is stored packed (upper triangle row-major, then the gradient): 7.4 KB for 10 free poses.
-template <bool SYSTEM>
-__global__ void __launch_bounds__((SYSTEM ? BA_FAST_WARPS : BA_RED_WARPS) * 32)
-ba_reduce_kernel(const BaArgs a) {
+// Entries [LO, HI) of the 90-float record of a pair: the lanes sum their edges in index order, one warp reduction per
+// entry, lane (k mod 32) keeps entry k in mine[k / 32].  Every entry's sum is independent of the others, so the record
+// comes out bit-identical whether it is formed in one pass or in two (which recomputes each edge's linearisation but
+// holds only half of the accumulators in registers).
+template <int LO, int HI>
+__device__ __forceinline__ void ba_pair_record(const BaArgs& a, int gs, int ge, int lane, float fx, float fy, float cx, float cy,
+                                               float (&mine)[3]) {
+  float acc[HI - LO];
+#pragma unroll
+  for (int k = 0; k < HI - LO; ++k) acc[k] = 0.0f;
+  for (int idx = gs + lane; idx < ge; idx += 32) {
+    EdgeLin L;
+    linearize_edge(a, a.p_order[idx], fx, fy, cx, cy, L);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float w = L.w[r];
+      int o = 0;
+#define BA_ACC(v) do { if (o >= LO && o < HI) acc[o - LO] += (v); ++o; } while (0)
+#pragma unroll
+      for (int x = 0; x < 6; ++x)
+#pragma unroll
+        for (int y = x; y < 6; ++y) BA_ACC(w * L.Ji[r][x] * L.Ji[r][y]);
+#pragma unroll
+      for (int x = 0; x < 6; ++x)
+#pragma unroll
+        for (int y = 0; y < 6; ++y) BA_ACC(-w * L.Ji[r][x] * L.Jj[r][y]);
+#pragma unroll
+      for (int x = 0; x < 6; ++x)
+#pragma unroll
+        for (int y = x; y < 6; ++y) BA_ACC(w * L.Jj[r][x] * L.Jj[r][y]);
+#pragma unroll
+      for (int x = 0; x < 6; ++x) BA_ACC(-w * L.r[r] * L.Ji[r][x]);
+#pragma unroll
+      for (int x = 0; x < 6; ++x) BA_ACC(w * L.r[r] * L.Jj[r][x]);
+#undef BA_ACC
+    }
+  }
+#pragma unroll
+  for (int k = LO; k < HI; ++k) {
+    const float s = warp_sum(acc[k - LO]);
+    if ((k & 31) == lane) mine[k >> 5] = s;
+  }
+}
+
+// Gk / Gp: the patch and pair groups this launch (batched: this stream) reduces; blockIdx.x deals the items.
+// SPLIT_PAIRS: form the pair records in two passes (ba_pair_record) -- the batched fast path, which is held to 128
+// registers by its 512-thread CTAs, then needs no local memory.
+template <bool SYSTEM, bool SPLIT_PAIRS = false>
+__device__ __forceinline__ void ba_reduce_body(const BaArgs& a, const int Gk, const int Gp) {
   constexpr int WARPS = SYSTEM ? BA_FAST_WARPS : BA_RED_WARPS;
   extern __shared__ __align__(16) float red_smem[];
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
@@ -91,7 +139,6 @@ ba_reduce_kernel(const BaArgs a) {
   }
   const float fx = a.intrinsics[0], fy = a.intrinsics[1], cx = a.intrinsics[2], cy = a.intrinsics[3];
   const float lm = a.lmbda[0];
-  const int Gk = *a.k_n, Gp = (a.N > 0) ? *a.p_n : 0;
   const int N = a.N, N6 = 6 * a.N;
   const int nwarps = gridDim.x * WARPS;
 
@@ -188,39 +235,44 @@ ba_reduce_kernel(const BaArgs a) {
       // ------------------------------------------------------------ pair item
       const int p = item - Gk;
       const int gs = a.p_start[p], ge = a.p_start[p + 1];
-      float acc[BA_REC];
-#pragma unroll
-      for (int k = 0; k < BA_REC; ++k) acc[k] = 0.0f;
-      for (int idx = gs + lane; idx < ge; idx += 32) {
-        EdgeLin L;
-        linearize_edge(a, a.p_order[idx], fx, fy, cx, cy, L);
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const float w = L.w[r];
-          int o = 0;
-#pragma unroll
-          for (int x = 0; x < 6; ++x)
-#pragma unroll
-            for (int y = x; y < 6; ++y) acc[o++] += w * L.Ji[r][x] * L.Ji[r][y];
-#pragma unroll
-          for (int x = 0; x < 6; ++x)
-#pragma unroll
-            for (int y = 0; y < 6; ++y) acc[o++] += -w * L.Ji[r][x] * L.Jj[r][y];
-#pragma unroll
-          for (int x = 0; x < 6; ++x)
-#pragma unroll
-            for (int y = x; y < 6; ++y) acc[o++] += w * L.Jj[r][x] * L.Jj[r][y];
-#pragma unroll
-          for (int x = 0; x < 6; ++x) acc[o++] += -w * L.r[r] * L.Ji[r][x];
-#pragma unroll
-          for (int x = 0; x < 6; ++x) acc[o++] += w * L.r[r] * L.Jj[r][x];
-        }
-      }
       float mine[3] = {0.f, 0.f, 0.f};
+      if constexpr (SPLIT_PAIRS) {
+        ba_pair_record<0, BA_REC / 2>(a, gs, ge, lane, fx, fy, cx, cy, mine);
+        ba_pair_record<BA_REC / 2, BA_REC>(a, gs, ge, lane, fx, fy, cx, cy, mine);
+      } else {                                          // one pass: the single-window launches
+        float acc[BA_REC];
 #pragma unroll
-      for (int k = 0; k < BA_REC; ++k) {
-        const float s = warp_sum(acc[k]);
-        if ((k & 31) == lane) mine[k >> 5] = s;
+        for (int k = 0; k < BA_REC; ++k) acc[k] = 0.0f;
+        for (int idx = gs + lane; idx < ge; idx += 32) {
+          EdgeLin L;
+          linearize_edge(a, a.p_order[idx], fx, fy, cx, cy, L);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const float w = L.w[r];
+            int o = 0;
+#pragma unroll
+            for (int x = 0; x < 6; ++x)
+#pragma unroll
+              for (int y = x; y < 6; ++y) acc[o++] += w * L.Ji[r][x] * L.Ji[r][y];
+#pragma unroll
+            for (int x = 0; x < 6; ++x)
+#pragma unroll
+              for (int y = 0; y < 6; ++y) acc[o++] += -w * L.Ji[r][x] * L.Jj[r][y];
+#pragma unroll
+            for (int x = 0; x < 6; ++x)
+#pragma unroll
+              for (int y = x; y < 6; ++y) acc[o++] += w * L.Jj[r][x] * L.Jj[r][y];
+#pragma unroll
+            for (int x = 0; x < 6; ++x) acc[o++] += -w * L.r[r] * L.Ji[r][x];
+#pragma unroll
+            for (int x = 0; x < 6; ++x) acc[o++] += w * L.r[r] * L.Jj[r][x];
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < BA_REC; ++k) {
+          const float s = warp_sum(acc[k]);
+          if ((k & 31) == lane) mine[k >> 5] = s;
+        }
       }
       if constexpr (!SYSTEM) {
         float* rp = a.rec + (int64_t)p * BA_REC;
@@ -279,6 +331,12 @@ ba_reduce_kernel(const BaArgs a) {
   }
 }
 
+template <bool SYSTEM>
+__global__ void __launch_bounds__((SYSTEM ? BA_FAST_WARPS : BA_RED_WARPS) * 32)
+ba_reduce_kernel(const BaArgs a) {
+  ba_reduce_body<SYSTEM>(a, *a.k_n, (a.N > 0) ? *a.p_n : 0);
+}
+
 // ==========================================================================================
 // kernel B: Schur complement, solve, retraction -- one thread-block cluster
 // ==========================================================================================
@@ -306,15 +364,13 @@ struct SolveSmem {
 //      substitution falls out of the factorisation -- and a one-warp back substitution
 //   4. every CTA: depth updates dZ = Q (u - E^T dX) for its patches (one warp per patch, coalesced),
 //      patch retraction; CTA 0: SE3 retraction of the free poses
-__global__ void __cluster_dims__(BA_CLUSTER, 1, 1) __launch_bounds__(BA_SOLVE_THREADS, 1)
-ba_solve_kernel(const BaArgs a) {
+__device__ __forceinline__ void ba_solve_body(const BaArgs& a, const int Gk, const int Gp) {
   extern __shared__ __align__(16) unsigned char solve_smem_raw[];
   SolveSmem& sm = *reinterpret_cast<SolveSmem*>(solve_smem_raw);
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int N = a.N, N6 = 6 * N;
-  const int Gk = *a.k_n;
   const int P = a.P;
   const int per = (Gk + BA_CLUSTER - 1) / BA_CLUSTER;
   const int m0 = min(Gk, rank * per), m1 = min(Gk, m0 + per);
@@ -462,7 +518,6 @@ ba_solve_kernel(const BaArgs a) {
     }
     BA_STAMP(1);
     // ---- 1b. pose blocks from this CTA's share of the pair records (pairs rank, rank+8, ...)
-    const int Gp = *a.p_n;
     const int n_mine = (Gp > rank) ? (Gp - rank + BA_CLUSTER - 1) / BA_CLUSTER : 0;
     for (int c0 = 0; c0 < n_mine; c0 += BA_REC_CHUNK) {
       const int cn = min(BA_REC_CHUNK, n_mine - c0);
@@ -712,6 +767,91 @@ ba_solve_kernel(const BaArgs a) {
   if (N > 0 && rank == 0 && tid < N) {
     retract_pose(a.poses + (int64_t)(a.t0 + tid) * 7, sm.dx + 6 * tid);
   }
+#undef BA_STAMP
+}
+
+__global__ void __cluster_dims__(BA_CLUSTER, 1, 1) __launch_bounds__(BA_SOLVE_THREADS, 1)
+ba_solve_kernel(const BaArgs a) {
+  ba_solve_body(a, *a.k_n, (a.N > 0) ? *a.p_n : 0);
+}
+
+// ==========================================================================================
+// batched: B independent sliding windows in one reduce and one solve launch
+// ==========================================================================================
+// Stream b owns frames [b F, (b+1) F) and patches [b F M, (b+1) F M).  The groupings are built over the concatenated
+// edge list; their keys ascend, so the patch groups and the pair groups of stream b form one contiguous range each.
+// ba_stream_bounds_kernel finds the ranges on the device: bounds[b] = first patch group of stream b (bounds[B] = the
+// number of patch groups), bounds[B + 1 + b] likewise for the pair groups.  No edge joins two streams (the host layer
+// rejects such edge lists), so a stream's groups hold only its own edges and every stream is the single-window
+// problem on a slice of the groupings and of the scratch.
+constexpr int BA_MAX_STREAMS = 64;
+
+struct BaBatch {
+  int B;
+  int64_t F, FM;                       // frames and patches per stream
+  int t0[BA_MAX_STREAMS];              // global index of the first free pose
+  int N[BA_MAX_STREAMS];               // free poses; 0 = the stream is left untouched
+  const int32_t* bounds;               // [2 (B + 1)], written by ba_stream_bounds_kernel
+  int64_t ed_pitch;                    // floats per patch-group row of Ed: 6 max_b N_b
+  int64_t part_stride;                 // floats of partial systems per stream (fast path)
+};
+
+// bounds[b] = the first group whose key belongs to stream >= b.  Each entry is written by exactly one thread: the one
+// at the group where the stream index of the sorted keys steps past b.
+__global__ void __launch_bounds__(256)
+ba_stream_bounds_kernel(const int64_t* __restrict__ k_key, const int32_t* __restrict__ k_n, const int64_t* __restrict__ p_key_i,
+                        const int32_t* __restrict__ p_n, int64_t FM, int64_t F, int B, int32_t* __restrict__ bounds) {
+  const int Gk = *k_n, Gp = p_n ? *p_n : 0;
+  auto stream_of = [&](int64_t key, int64_t per) { const int64_t s = key / per; return (int)(s < 0 ? 0 : (s > B ? B : s)); };
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t <= Gk + 1 + Gp; t += gridDim.x * blockDim.x) {
+    const bool pair = t > Gk;
+    const int g = pair ? t - Gk - 1 : t, G = pair ? Gp : Gk;
+    const int64_t* key = pair ? p_key_i : k_key;
+    const int64_t per = pair ? F : FM;
+    int32_t* out = bounds + (pair ? B + 1 : 0);
+    const int s_prev = (g == 0) ? -1 : stream_of(key[g - 1], per);
+    const int s_cur = (g == G) ? B : stream_of(key[g], per);
+    for (int b = s_prev + 1; b <= s_cur; ++b) out[b] = g;
+  }
+}
+
+// the single-window arguments of stream b: its group ranges, its window, its camera and its slices of the scratch
+__device__ __forceinline__ BaArgs ba_stream_args(const BaArgs& a, const BaBatch& bb, int b, int& Gk, int& Gp) {
+  const int k0 = bb.bounds[b], p0 = bb.bounds[bb.B + 1 + b];
+  Gk = bb.bounds[b + 1] - k0;
+  Gp = bb.bounds[bb.B + 2 + b] - p0;
+  BaArgs s = a;
+  s.t0 = bb.t0[b]; s.N = bb.N[b];
+  s.intrinsics = a.intrinsics + (int64_t)b * bb.F * 4;
+  s.k_start = a.k_start + k0; s.k_key = a.k_key + k0;
+  s.p_start = a.p_start + p0; s.p_key_i = a.p_key_i + p0; s.p_key_j = a.p_key_j + p0;
+  s.Ed = a.Ed + (int64_t)k0 * bb.ed_pitch;
+  s.Qk = a.Qk + k0; s.uk = a.uk + k0;
+  s.rec = a.rec + (int64_t)p0 * BA_REC;
+  s.dX = a.dX + (int64_t)b * 6 * BA_MAX_N;
+  s.part = a.part ? a.part + (int64_t)b * bb.part_stride : nullptr;
+  s.dbg = nullptr;
+  return s;
+}
+
+// grid (partitions per stream, B): blockIdx.y is the stream, blockIdx.x deals that stream's items as the single-window
+// launch deals them, so each stream's partial sums are those of a launch on that stream alone
+template <bool SYSTEM>
+__global__ void __launch_bounds__((SYSTEM ? BA_FAST_WARPS : BA_RED_WARPS) * 32)
+ba_reduce_batched_kernel(const BaArgs a, const BaBatch bb) {
+  int Gk, Gp;
+  const BaArgs s = ba_stream_args(a, bb, blockIdx.y, Gk, Gp);
+  if (s.N == 0 || Gk == 0) return;                   // an empty window or a stream without edges: nothing to do
+  ba_reduce_body<SYSTEM, SYSTEM>(s, Gk, Gp);
+}
+
+// B clusters of 8 CTAs: cluster c solves stream c
+__global__ void __cluster_dims__(BA_CLUSTER, 1, 1) __launch_bounds__(BA_SOLVE_THREADS, 1)
+ba_solve_batched_kernel(const BaArgs a, const BaBatch bb) {
+  int Gk, Gp;
+  const BaArgs s = ba_stream_args(a, bb, blockIdx.x / BA_CLUSTER, Gk, Gp);
+  if (s.N == 0 || Gk == 0) return;                   // uniform over the cluster: no CTA waits at a cluster barrier alone
+  ba_solve_body(s, Gk, Gp);
 }
 
 // ==========================================================================================
@@ -876,6 +1016,94 @@ extern "C" int dpvo_ba_forward_grouped(float* poses, float* patches, const float
   a.rec = (float*)p; p += al256(E * (int64_t)BA_REC * 4);
   a.dX = (float*)p;
   return ba_run(a, iterations, (cudaStream_t)stream);
+}
+
+// batched workspace: the stream bounds, then the grouped layout with Ed rows of 6 max_b N_b floats and one dX per stream,
+// then (every N_b <= BA_FAST_MAX_N) B x sm_count partial reduced systems
+static int64_t ba_batched_part_floats(int max_free_poses) {
+  return (max_free_poses > 0 && max_free_poses <= BA_FAST_MAX_N) ? (int64_t)sm_count() * ba_packed_entries(6 * max_free_poses) : 0;
+}
+
+extern "C" int64_t dpvo_ba_batched_workspace_bytes(int64_t E, int B, int max_free_poses) {
+  if (E < 0) E = 0;
+  if (B < 1) B = 1;
+  return al256(2 * (int64_t)(B + 1) * 4) + al256(E * 6 * (int64_t)std::max(max_free_poses, 1) * 4) + 2 * al256(E * 4) +
+         al256(E * (int64_t)BA_REC * 4) + al256((int64_t)B * 6 * BA_MAX_N * 4) +
+         al256((int64_t)B * ba_batched_part_floats(max_free_poses) * 4) + 256;
+}
+
+extern "C" int dpvo_ba_forward_batched(float* poses, float* patches, const float* intrinsics,
+                                       const float* target, const float* weight, const float* lmbda,
+                                       const int64_t* ii, const int64_t* jj, const int64_t* kk,
+                                       int64_t E, int P, int B, int frames_per_stream, int patches_per_frame,
+                                       const int* t0, const int* t1, int iterations,
+                                       const int32_t* k_order, const int32_t* k_start, const int64_t* k_key, const int32_t* k_n,
+                                       const int32_t* p_order, const int32_t* p_start, const int64_t* p_key_i,
+                                       const int64_t* p_key_j, const int32_t* p_n,
+                                       void* workspace, int64_t workspace_bytes, void* stream) {
+  DPVO_REQUIRE(E >= 0 && P > 0 && iterations >= 0 && B >= 1 && frames_per_stream > 0 && patches_per_frame > 0,
+               "ba_forward_batched: bad sizes");
+  DPVO_REQUIRE(t0 && t1, "ba_forward_batched: null window arrays");
+  if (B > BA_MAX_STREAMS) { set_error("ba_forward_batched: %d streams > %d", B, BA_MAX_STREAMS); return DPVO_ERR_UNSUPPORTED; }
+  BaBatch bb;
+  bb.B = B; bb.F = frames_per_stream; bb.FM = (int64_t)frames_per_stream * patches_per_frame;
+  int max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    const int n = t1[b] - t0[b];
+    DPVO_REQUIRE(n >= 0 && (n == 0 || (t0[b] >= (int64_t)b * frames_per_stream && t1[b] <= (int64_t)(b + 1) * frames_per_stream)),
+                 "ba_forward_batched: window [%d, %d) of stream %d is not inside its frames [%lld, %lld)", t0[b], t1[b], b,
+                 (long long)b * frames_per_stream, (long long)(b + 1) * frames_per_stream);
+    if (n > BA_MAX_N) { set_error("ba_forward_batched: stream %d has %d free poses > %d", b, n, BA_MAX_N); return DPVO_ERR_UNSUPPORTED; }
+    bb.t0[b] = t0[b]; bb.N[b] = n;
+    max_n = std::max(max_n, n);
+  }
+  if (E == 0 || iterations == 0 || max_n == 0) return DPVO_OK;
+  DPVO_REQUIRE(poses && patches && intrinsics && target && weight && lmbda && ii && jj && kk && workspace && k_order &&
+               k_start && k_key && k_n && p_order && p_start && p_key_i && p_key_j && p_n, "ba_forward_batched: null pointer");
+  if (workspace_bytes < dpvo_ba_batched_workspace_bytes(E, B, max_n)) { set_error("ba_forward_batched: workspace too small"); return DPVO_ERR_WORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  char* p = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  int32_t* bounds = (int32_t*)p; p += al256(2 * (int64_t)(B + 1) * 4);
+  BaArgs a;
+  a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
+  a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = 0; a.N = max_n;
+  a.k_order = k_order; a.k_start = k_start; a.k_key = k_key; a.k_n = k_n;
+  a.p_order = p_order; a.p_start = p_start; a.p_key_i = p_key_i; a.p_key_j = p_key_j; a.p_n = p_n;
+  a.Ed = (float*)p; p += al256(E * 6 * (int64_t)max_n * 4);
+  a.Qk = (float*)p; p += al256(E * 4);
+  a.uk = (float*)p; p += al256(E * 4);
+  a.rec = (float*)p; p += al256(E * (int64_t)BA_REC * 4);
+  a.dX = (float*)p; p += al256((int64_t)B * 6 * BA_MAX_N * 4);
+  a.dbg = nullptr;
+  // the fast path applies to the whole batch when every window fits it, the general path otherwise
+  const bool fast = max_n <= BA_FAST_MAX_N;
+  a.part = fast ? (float*)p : nullptr;
+  a.n_part = fast ? sm_count() : 0;
+  bb.part_stride = ba_batched_part_floats(max_n);
+  bb.ed_pitch = 6 * (int64_t)max_n;
+  bb.bounds = bounds;
+  {
+    const int64_t items = E + 2;                 // at most Gk + 1 + Gp + 1 <= E + 2
+    const unsigned grid = (unsigned)std::min<int64_t>((items + 255) / 256, (int64_t)sm_count() * 4);
+    ba_stream_bounds_kernel<<<grid, 256, 0, st>>>(k_key, k_n, p_key_i, p_n, bb.FM, bb.F, B, bounds);
+    DPVO_LAUNCH_CHECK("ba_stream_bounds_kernel");
+  }
+  cudaError_t e = cudaFuncSetAttribute(ba_solve_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SolveSmem));
+  if (e != cudaSuccess) return check_cuda(e, "ba_forward_batched: cudaFuncSetAttribute");
+  // shared memory sized for the widest window of the batch
+  const size_t fast_smem = fast ? (size_t)BA_FAST_WARPS * (6 * BA_MAX_N + 96 + (size_t)ba_packed_entries(6 * max_n)) * sizeof(float) : 0;
+  if (fast) {
+    e = cudaFuncSetAttribute(ba_reduce_batched_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem);
+    if (e != cudaSuccess) return check_cuda(e, "ba_forward_batched: cudaFuncSetAttribute (reduce)");
+  }
+  for (int it = 0; it < iterations; ++it) {
+    if (fast) ba_reduce_batched_kernel<true><<<dim3(a.n_part, B), BA_FAST_WARPS * 32, fast_smem, st>>>(a, bb);
+    else ba_reduce_batched_kernel<false><<<dim3(sm_count() * 4, B), BA_RED_WARPS * 32, BA_RED_WARPS * 6 * BA_MAX_N * sizeof(float), st>>>(a, bb);
+    DPVO_LAUNCH_CHECK("ba_reduce_batched_kernel");
+    ba_solve_batched_kernel<<<BA_CLUSTER * B, BA_SOLVE_THREADS, sizeof(SolveSmem), st>>>(a, bb);
+    DPVO_LAUNCH_CHECK("ba_solve_batched_kernel");
+  }
+  return DPVO_OK;
 }
 
 extern "C" int dpvo_ba_forward(float* poses, float* patches, const float* intrinsics,

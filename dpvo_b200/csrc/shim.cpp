@@ -422,6 +422,44 @@ void ba_forward_grouped(Tensor poses, Tensor patches, Tensor intrinsics, Tensor 
         "dpvo_b200_ext.ba_forward_grouped");
 }
 
+// B streams' sliding windows in one reduce and one solve launch per iteration; t0 / t1 are global frame numbers
+void ba_forward_batched(Tensor poses, Tensor patches, Tensor intrinsics, Tensor target, Tensor weight, Tensor lmbda,
+                        Tensor ii, Tensor jj, Tensor kk, int64_t frames_per_stream, std::vector<int> t0, std::vector<int> t1,
+                        int iterations, Tensor k_order, Tensor k_start, Tensor k_key, Tensor k_n,
+                        Tensor p_order, Tensor p_start, Tensor p_key_i, Tensor p_key_j, Tensor p_n) {
+  need_cuda(poses, "poses"); need_cuda(patches, "patches");
+  c10::cuda::CUDAGuard guard(poses.device());
+  TORCH_CHECK(poses.is_contiguous() && patches.is_contiguous(), "ba_forward_batched updates poses/patches in place: they must be contiguous");
+  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat, "ba_forward_batched: poses/patches must be float32");
+  TORCH_CHECK(t0.size() == t1.size() && !t0.empty(), "ba_forward_batched: t0 and t1 need one entry per stream");
+  const int B = (int)t0.size();
+  const int64_t n_frames = poses.numel() / 7, n_patches = patches.numel() / (3 * patches.size(-1) * patches.size(-1));
+  TORCH_CHECK(frames_per_stream > 0 && n_frames == B * frames_per_stream && n_patches % n_frames == 0,
+              "ba_forward_batched: poses hold ", n_frames, " frames and patches ", n_patches, ", not ", B, " streams of ",
+              frames_per_stream, " frames with the same number of patches each");
+  TORCH_CHECK(intrinsics.numel() == 4 * n_frames, "ba_forward_batched: intrinsics need one row per frame");
+  const int P = patches.size(-1);
+  intrinsics = f32c(intrinsics); target = f32c(target); weight = f32c(weight); lmbda = f32c(lmbda);
+  ii = i64c(ii); jj = i64c(jj); kk = i64c(kk);
+  const int64_t E = ii.numel();
+  int max_n = 0;
+  for (int b = 0; b < B; ++b) max_n = std::max(max_n, t1[b] - t0[b]);
+  const int64_t wsb = dpvo_ba_batched_workspace_bytes(E, B, max_n);
+  Tensor ws = byte_ws(wsb, poses);
+  check(dpvo_ba_forward_batched(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(),
+                                target.data_ptr<float>(), weight.data_ptr<float>(), lmbda.data_ptr<float>(),
+                                ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), E, P, B,
+                                (int)frames_per_stream, (int)(n_patches / n_frames), t0.data(), t1.data(), iterations,
+                                k_order.data_ptr<int>(), k_start.data_ptr<int>(), k_key.data_ptr<int64_t>(), k_n.data_ptr<int>(),
+                                p_order.data_ptr<int>(), p_start.data_ptr<int>(), p_key_i.data_ptr<int64_t>(),
+                                p_key_j.data_ptr<int64_t>(), p_n.data_ptr<int>(), ws.data_ptr(), wsb, stream()),
+        "dpvo_b200_ext.ba_forward_batched");
+}
+
+int64_t ba_batched_workspace_bytes(int64_t E, int64_t B, int64_t max_free_poses) {
+  return dpvo_ba_batched_workspace_bytes(E, (int)B, (int)max_free_poses);
+}
+
 Tensor reproject_clamped(Tensor poses, Tensor patches, Tensor intrinsics, Tensor ii, Tensor jj, Tensor kk) {
   return reproject_impl(poses, patches, intrinsics, ii, jj, kk, 1);
 }
@@ -932,6 +970,9 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("group_edges", &group_edges, "device edge grouping", py::arg("key_a"), py::arg("key_b") = py::none(),
         py::arg("sec") = py::none());
   m.def("ba_forward_grouped", &ba_forward_grouped, "fastba.BA on prebuilt edge groupings");
+  m.def("ba_forward_batched", &ba_forward_batched, "fastba.BA over B streams' windows on prebuilt edge groupings");
+  m.def("ba_batched_workspace_bytes", &ba_batched_workspace_bytes, "scratch bytes of ba_forward_batched (current device)",
+        py::arg("E"), py::arg("B"), py::arg("max_free_poses"));
   m.def("reproject_clamped", &reproject_clamped, "pops.transform-compatible fused reprojection");
   m.def("add_layernorm", &add_layernorm, "fused add + LayerNorm (+ReLU)", py::arg("a"), py::arg("b"), py::arg("c"), py::arg("gamma"),
         py::arg("beta"), py::arg("eps"), py::arg("relu"), py::arg("want32"), py::arg("want16"), py::arg("b_index") = py::none(), py::arg("inplace32") = false, py::arg("c_scale") = py::none());

@@ -23,3 +23,17 @@ def BA_grouped(poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, t0
     return extensions()[3].ba_forward_grouped(poses.data, patches, intrinsics, target, weight, lmbda, ii, jj, kk, t0, t1,
                                               iterations, gk.order, gk.group_start, gk.key_a, gk.n,
                                               gp.order, gp.group_start, gp.key_a, gp.key_b, gp.n)
+
+
+def BA_batched(poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, frames_per_stream, t0s, t1s, iterations,
+               groups_kk, groups_ij):
+    """BA_grouped for B streams in one reduce and one solve launch per iteration.  Stream b owns frames
+    [b F, (b+1) F) and patches [b F M, (b+1) F M) (F = frames_per_stream); its window is [t0s[b], t1s[b]) in global
+    frame numbers and intrinsics row b F is its camera.  The edge lists and groupings span all streams, and no edge may
+    join two streams (streams.StreamBatch builds and checks such lists).  A stream with an empty window or without edges
+    is left untouched."""
+    gk, gp = groups_kk, groups_ij
+    return extensions()[3].ba_forward_batched(poses.data, patches, intrinsics, target, weight, lmbda, ii, jj, kk,
+                                              int(frames_per_stream), [int(t) for t in t0s], [int(t) for t in t1s],
+                                              iterations, gk.order, gk.group_start, gk.key_a, gk.n,
+                                              gp.order, gp.group_start, gp.key_a, gp.key_b, gp.n)

@@ -30,10 +30,45 @@ class DevicePatchGraph:
         self.overflow = torch.zeros(1, dtype=torch.int32, device=dev)
         self.net = torch.zeros(1, self.cap, DIM, device=dev)                  # the recurrent state `net` (dpvo.py:53), fp32
 
+    @classmethod
+    def stacked(cls, B, capacity, M, dummy_frames, device="cuda"):
+        """One store for the B streams of a streams.StreamBatch: B slices of `capacity` slots (rounded up to a multiple of
+        128) in stream order, and B per-stream graphs whose arrays and recurrent state are views of their slice.
+        dummy_frames[b] is stream b's reserved frame in global numbering (e.g. its last pose slot, b F + F - 1): its
+        parked slots point there, so they stay inside stream b's frames and rings.  Appends and removals go through the
+        per-stream graphs, with global frame numbers, and touch only that slice -- removing a keyframe renumbers only
+        that stream's edges; UpdateRunner steps the whole store.  Returns (store, [graph of stream b])."""
+        dummy_frames = [int(f) for f in dummy_frames]
+        if len(dummy_frames) != int(B):
+            raise ValueError("DevicePatchGraph.stacked: one dummy frame per stream")
+        cap = (int(capacity) + 127) // 128 * 128
+        store = cls(B * cap, M, dummy_frames[0], device)
+        store.dummy_frame = store.dummy_patch = None            # per stream: see store.streams
+        store.n_active = store.overflow = None
+        store.streams = []
+        for b, f in enumerate(dummy_frames):
+            sl = slice(b * cap, (b + 1) * cap)
+            store.ii[sl] = f
+            store.jj[sl] = f
+            store.kk[sl] = f * store.M
+            g = cls.__new__(cls)
+            g.cap, g.M, g.dummy_frame, g.dummy_patch = cap, store.M, f, f * store.M
+            g.ii, g.jj, g.kk, g.active = store.ii[sl], store.jj[sl], store.kk[sl], store.active[sl]
+            g.net = store.net[:, sl]
+            g.n_active = torch.zeros(1, dtype=torch.int32, device=store.ii.device)
+            g.overflow = torch.zeros(1, dtype=torch.int32, device=store.ii.device)
+            store.streams.append(g)
+        return store, store.streams
+
+    def _per_stream(self, what):
+        if self.dummy_frame is None:
+            raise RuntimeError("DevicePatchGraph.%s: a stacked store changes through its per-stream graphs (store.streams)" % what)
+
     # -------------------------------------------------------------------------------- dpvo.py:215-222
     def append(self, ii, jj, kk, enable=None):
         """add edges (ii = source frame, jj = target frame, kk = patch); their state rows start at zero.
         Returns the slot of every new edge (int32, -1 = store full, `overflow` is then set)."""
+        self._per_stream("append")
         return extensions()[3].pgraph_append(self.ii, self.jj, self.kk, self.active, ii, jj, kk, enable, self.net,
                                              self.n_active, self.overflow)
 
@@ -45,12 +80,14 @@ class DevicePatchGraph:
     # -------------------------------------------------------------------------------- dpvo.py:224-238, 300-306
     def remove_old(self, n_dev, window, enable=None):
         """park the edges whose patch left the removal window: ix[kk] < n - window"""
+        self._per_stream("remove_old")
         extensions()[3].pgraph_remove(self.ii, self.jj, self.kk, self.active, 0, n_dev, int(window), enable,
                                       self.dummy_frame, self.dummy_patch, self.M, self.n_active)
 
     # -------------------------------------------------------------------------------- dpvo.py:279-286
     def remove_frame(self, k_dev, enable=None):
         """keyframe removal: park the edges that touch frame k and renumber frames / patches above it"""
+        self._per_stream("remove_frame")
         extensions()[3].pgraph_remove(self.ii, self.jj, self.kk, self.active, 1, k_dev, 0, enable,
                                       self.dummy_frame, self.dummy_patch, self.M, self.n_active)
 

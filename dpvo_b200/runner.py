@@ -14,16 +14,20 @@ from . import altcorr, fastba
 from . import projective_ops as pops
 from .net import Update, EdgeGroups, DIM
 from .frontend import encoder_output_size
+from .streams import StreamBatch
 
 
 class UpdateRunner:
     def __init__(self, state, update=None, ba_iterations=2, seed=1234, graph=None, encoder=None):
-        """encoder: optional frontend.FrameEncoder, which `ingest_image` runs.
+        """state: one stream's state (synthetic.SyntheticState layout), or a streams.StreamBatch of B streams that every
+        step updates together: one launch per kernel for all of them, bundle adjustment by fastba.BA_batched.
+        encoder: optional frontend.FrameEncoder, which `ingest_image` runs.
         graph: optional DevicePatchGraph (patchgraph.py).  With it the edge lists and the recurrent state are the
         store's fixed-capacity arrays: every kernel runs over all `cap` slots, parked slots are dummy edges in groups of
         their own whose confidence weights are zeroed before bundle adjustment, and a captured CUDA graph of step()
-        stays valid while edges are appended and removed between replays."""
+        stays valid while edges are appended and removed between replays.  For a batch: DevicePatchGraph.stacked."""
         self.s = state
+        self.batch = state if isinstance(state, StreamBatch) else None
         self.pg = graph
         self.encoder = encoder
         dev = state.poses.device
@@ -35,8 +39,11 @@ class UpdateRunner:
         self.update.packed()
         self.graph = None
         self.M = state.cfg["M"]
-        self.mem = state.fmap1.shape[1]
-        self.pmem = state.imap.shape[1] // self.M
+        if self.batch is None:
+            self.mem = state.fmap1.shape[1]
+            self.pmem = state.imap.shape[1] // self.M
+        else:
+            self.mem, self.pmem = state.mem, state.pmem                # ring sizes of one stream
         self.ba_iterations = ba_iterations
         self.lmbda = torch.as_tensor([1e-4], device=dev)
         self.poses0 = state.poses.clone()
@@ -50,17 +57,21 @@ class UpdateRunner:
             n_live_frames = int((state.kk // self.M).unique().numel())
             self.max_patch_groups = n_live_frames * self.M
             self.max_pair_groups = int(torch.unique(state.ii * 100000 + state.jj).numel())
-            self.kk_ring = state.kk % (self.M * self.pmem)
-            self.jj_ring = state.jj % self.mem
+            if self.batch is None:
+                self.kk_ring = state.kk % (self.M * self.pmem)
+                self.jj_ring = state.jj % self.mem
+            else:
+                self.kk_ring, self.jj_ring = state.ring_rows(state.kk, state.jj)
         else:
             self.E = graph.cap
             self.ii, self.jj, self.kk = graph.ii, graph.jj, graph.kk
             self.net = graph.net                                      # [1, cap, 384] fp32, updated in place
             # bounds that hold for any topology the store can take: every live patch + the dummy patch; every ordered
-            # frame pair inside the removal window + the dummy pair
+            # frame pair inside the removal window + the dummy pair, per stream
             live = state.cfg["removal"] + 2
-            self.max_patch_groups = min(graph.cap, live * self.M + 1)
-            self.max_pair_groups = min(graph.cap, live * live + 1)
+            nb = 1 if self.batch is None else self.batch.B
+            self.max_patch_groups = min(graph.cap, nb * (live * self.M + 1))
+            self.max_pair_groups = min(graph.cap, nb * (live * live + 1))
             self.kk_ring = self.jj_ring = None                       # the ring indices follow the edges: computed per step
         self.corr_buf = torch.zeros(1, self.E, 896, device=dev, dtype=torch.half)   # padding columns stay zero
 
@@ -77,8 +88,12 @@ class UpdateRunner:
         patches = s.patches.view(1, -1, 3, 3, 3)
         intr = s.intrinsics.view(1, -1, 4)
         ii, jj, kk = self.ii, self.jj, self.kk
-        kk_ring = self.kk_ring if self.pg is None else kk % (self.M * self.pmem)
-        jj_ring = self.jj_ring if self.pg is None else jj % self.mem
+        if self.pg is None:
+            kk_ring, jj_ring = self.kk_ring, self.jj_ring
+        elif self.batch is None:
+            kk_ring, jj_ring = kk % (self.M * self.pmem), jj % self.mem
+        else:
+            kk_ring, jj_ring = self.batch.ring_rows(kk, jj)
         coords = pops.transform_fused(poses, patches, intr, ii, jj, kk)               # [1,E,2,3,3]
         if ev is not None:
             ev["corr0"].record()
@@ -94,8 +109,13 @@ class UpdateRunner:
             weight = weight * self.pg.active.view(1, -1, 1)          # parked edges carry no confidence into bundle adjustment
         if ev is not None:
             ev["ba0"].record()
-        fastba.BA_grouped(poses, patches, intr, target, weight, self.lmbda, ii, jj, kk, s.t0, s.n,
-                          self.ba_iterations, groups_kk, groups_ij)
+        if self.batch is None:
+            fastba.BA_grouped(poses, patches, intr, target, weight, self.lmbda, ii, jj, kk, s.t0, s.n,
+                              self.ba_iterations, groups_kk, groups_ij)
+        else:
+            t0s, t1s = self.batch.windows()
+            fastba.BA_batched(poses, patches, intr, target, weight, self.lmbda, ii, jj, kk, self.batch.F, t0s, t1s,
+                              self.ba_iterations, groups_kk, groups_ij)
         if ev is not None:
             ev["ba1"].record()
         return target, weight
@@ -124,9 +144,19 @@ class UpdateRunner:
         return self._graph_out
 
     # ----------------------------------------------------------------- end to end (host buffers)
-    def make_host_frame(self, seed=0):
+    def _stream_state(self, stream, what):
+        """the single-stream state a per-frame call writes: the state itself, or stream `stream` of a batch"""
+        if self.batch is None:
+            if stream is not None:
+                raise RuntimeError("%s: stream=%s given, but this UpdateRunner holds one stream" % (what, stream))
+            return self.s
+        if stream is None:
+            raise RuntimeError("%s: this UpdateRunner holds %d streams; say which with stream=b" % (what, self.batch.B))
+        return self.batch.stream(stream)
+
+    def make_host_frame(self, seed=0, stream=None):
         """pinned host copies of everything DPVO.__call__ writes for one new frame"""
-        s = self.s
+        s = self._stream_state(stream, "make_host_frame")
         g = torch.Generator().manual_seed(seed)
         h, w = s.fmap1.shape[3], s.fmap1.shape[4]
         f = dict(
@@ -139,9 +169,10 @@ class UpdateRunner:
         )
         return {k: v.pin_memory() for k, v in f.items()}
 
-    def ingest_frame(self, hf):
-        """H2D of one frame into ring slot n-1 (channels-last buffers take the host layout as is)."""
-        s = self.s
+    def ingest_frame(self, hf, stream=None):
+        """H2D of one frame into ring slot n-1 (channels-last buffers take the host layout as is); in a batch, into
+        stream `stream`'s slots (its own n)."""
+        s = self._stream_state(stream, "ingest_frame")
         slot = (s.n - 1) % self.mem
         pslot = (s.n - 1) % self.pmem
         s.fmap1[0, slot].permute(1, 2, 0).copy_(hf["fmap1"], non_blocking=True)
@@ -153,16 +184,16 @@ class UpdateRunner:
         return sum(v.numel() * v.element_size() for v in hf.values())
 
     @torch.no_grad()
-    def ingest_image(self, image, depth=None, coords=None):
+    def ingest_image(self, image, depth=None, coords=None, stream=None):
         """Encode a uint8 camera image [3, H, W] (CHW or HWC strides) straight into the slots `ingest_frame` writes:
         fmap1 / fmap2 slot (n-1) % mem, gmap / imap slot (n-1) % pmem, patches[(n-1) M : n M] (dpvo.py:389-438).
         Centroids are drawn as Patchifier.forward draws them, unless `coords` [M, 2] is given (CUDA-graph capture);
         the patch depths are then one torch.rand draw (dpvo.py:427), or `depth` (the median the caller computes once
-        initialised, dpvo.py:429-431).  Poses, intrinsics and the motion model stay with the caller.  Returns the
-        centroids."""
+        initialised, dpvo.py:429-431).  Poses, intrinsics and the motion model stay with the caller.  In a batch,
+        `stream` names the stream whose slots (at its own n) receive the frame.  Returns the centroids."""
         if self.encoder is None:
             raise RuntimeError("ingest_image: this UpdateRunner was built without an encoder")
-        s, M = self.s, self.M
+        s, M = self._stream_state(stream, "ingest_image"), self.M
         h, w = s.fmap1.shape[3], s.fmap1.shape[4]
         if image.dim() != 3 or encoder_output_size(image.shape[1], image.shape[2]) != (h, w):
             raise RuntimeError("ingest_image: a %s image encodes to %s features, the rings hold %dx%d"

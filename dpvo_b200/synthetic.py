@@ -135,3 +135,19 @@ def make_state(config="default", n_frames=30, device="cuda", seed=1234, features
         st.imap = (torch.randn(1, mem * M, 384, generator=gd, device=device) / 4).to(dtype)
         st.net = torch.zeros(1, st.E, 384, device=device, dtype=dtype)
     return st
+
+
+def make_batch(config="default", B=2, seeds=None, n_frames=30, device="cuda", frames_per_stream=64, mem=36):
+    """B independent steady-state streams in one streams.StreamBatch: stream b is make_state(config, n_frames[b],
+    seed=seeds[b]) (an int n_frames serves every stream), with frames_per_stream pose slots and a ring of `mem`."""
+    from .streams import StreamBatch
+    cfg = dict(CONFIGS[config]) if isinstance(config, str) else dict(config)
+    seeds = [1234 + 17 * b for b in range(B)] if seeds is None else list(seeds)
+    frames = [n_frames] * B if isinstance(n_frames, int) else list(n_frames)
+    if len(seeds) != B or len(frames) != B:
+        raise ValueError("make_batch: one seed and one frame count per stream")
+    batch = StreamBatch(B, cfg, frames_per_stream, mem, mem, device=device)
+    for b in range(B):
+        batch.load(b, make_state(cfg, frames[b], device=device, seed=seeds[b], buffer=frames_per_stream, mem=mem))
+    batch.set_edges()
+    return batch

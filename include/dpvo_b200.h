@@ -233,6 +233,28 @@ int dpvo_ba_forward_grouped(float* poses, float* patches, const float* intrinsic
                             void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * B independent sliding windows in one launch sequence (two launches per iteration for the whole batch).  Stream b owns
+ * frames [b F, (b+1) F) and patches [b F M, (b+1) F M) of poses / patches / intrinsics (F = frames_per_stream,
+ * M = patches_per_frame); its window is [t0[b], t1[b]) in global frame numbers (host arrays), and row b F of
+ * intrinsics is its camera.  The groupings are the dpvo_ba_forward_grouped ones, built over the concatenation of the
+ * streams' edges; each stream's group range is found on the device (no host synchronisation, graph-capturable).  No
+ * edge may join two streams.  A stream with t1[b] == t0[b] or without edges is left untouched.  Every t1 - t0 <= 12
+ * runs the fast path for the whole batch, otherwise the general path does; t1 - t0 > 32 is DPVO_ERR_UNSUPPORTED,
+ * B > 64 too.  Each stream's result is that of dpvo_ba_forward_grouped on the stream alone.
+ * workspace: dpvo_ba_batched_workspace_bytes(E, B, max_b (t1[b] - t0[b])) on the current device.
+ */
+int64_t dpvo_ba_batched_workspace_bytes(int64_t E, int B, int max_free_poses);
+int dpvo_ba_forward_batched(float* poses, float* patches, const float* intrinsics,
+                            const float* target, const float* weight, const float* lmbda,
+                            const int64_t* ii, const int64_t* jj, const int64_t* kk,
+                            int64_t E, int P, int B, int frames_per_stream, int patches_per_frame,
+                            const int* t0, const int* t1, int iterations,
+                            const int32_t* k_order, const int32_t* k_start, const int64_t* k_key, const int32_t* k_n,
+                            const int32_t* p_order, const int32_t* p_start, const int64_t* p_key_i,
+                            const int64_t* p_key_j, const int32_t* p_n,
+                            void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
  * Wide windows / cuda_ba.forward(..., eff_impl=True) -- replaces dpvo/fastba/block_e.cu:38-299 (EfficentE) and
  * the eff_impl branch of ba_cuda.cu:495-563.  For any number of free poses N = t1 - t0: one call assembles
  *     S = B - E diag(Q) E^T + I o (1e-4 S + 1)   fp32 [6N, 6N]  and   y = v - E diag(Q) u   fp32 [6N]
