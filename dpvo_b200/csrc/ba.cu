@@ -457,7 +457,7 @@ __device__ __forceinline__ void ba_solve_body(const BaArgs& a, const int Gk, con
       }
     };
     // work item of a thread: tile (r4 <= c4) and k-split, constant over the chunks, so the 4x4 accumulator stays
-    // in registers for the whole slice and S is touched once at the end (rounds > 1 only beyond 16 free poses;
+    // in registers for the whole slice and S is touched once at the end (rounds > 1 only beyond 20 free poses;
     // the slice is then staged once per round)
     const int ksplit = max(1, min(3, BA_SOLVE_THREADS / n_tiles4));
     const int rounds = (n_tiles4 * ksplit + BA_SOLVE_THREADS - 1) / BA_SOLVE_THREADS;

@@ -30,8 +30,9 @@ def BA_batched(poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, fr
     """BA_grouped for B streams in one reduce and one solve launch per iteration.  Stream b owns frames
     [b F, (b+1) F) and patches [b F M, (b+1) F M) (F = frames_per_stream); its window is [t0s[b], t1s[b]) in global
     frame numbers and intrinsics row b F is its camera.  The edge lists and groupings span all streams, and no edge may
-    join two streams (streams.StreamBatch builds and checks such lists).  A stream with an empty window or without edges
-    is left untouched."""
+    join two streams (streams.StreamBatch builds and checks such lists).  Each stream's result is that of BA_grouped on
+    the stream alone, with one exception: a stream with an empty window (t0s[b] == t1s[b]) is left untouched, where
+    BA_grouped runs its structure-only step and updates the depths.  A stream without edges is left untouched too."""
     gk, gp = groups_kk, groups_ij
     return extensions()[3].ba_forward_batched(poses.data, patches, intrinsics, target, weight, lmbda, ii, jj, kk,
                                               int(frames_per_stream), [int(t) for t in t0s], [int(t) for t in t1s],

@@ -240,7 +240,9 @@ int dpvo_ba_forward_grouped(float* poses, float* patches, const float* intrinsic
  * streams' edges; each stream's group range is found on the device (no host synchronisation, graph-capturable).  No
  * edge may join two streams.  A stream with t1[b] == t0[b] or without edges is left untouched.  Every t1 - t0 <= 12
  * runs the fast path for the whole batch, otherwise the general path does; t1 - t0 > 32 is DPVO_ERR_UNSUPPORTED,
- * B > 64 too.  Each stream's result is that of dpvo_ba_forward_grouped on the stream alone.
+ * B > 64 too.  Each stream's result is that of dpvo_ba_forward_grouped on the stream alone, with one exception: a
+ * stream with an empty window (t1[b] == t0[b]) keeps its depths, where dpvo_ba_forward_grouped runs its
+ * structure-only (depth-only) step.
  * workspace: dpvo_ba_batched_workspace_bytes(E, B, max_b (t1[b] - t0[b])) on the current device.
  */
 int64_t dpvo_ba_batched_workspace_bytes(int64_t E, int B, int max_free_poses);
