@@ -21,6 +21,11 @@
 // normalised layer also leaves per-CTA per-channel (count, mean, M2) of the fp16-rounded outputs in a fixed slot; the
 // last CTA to finish (integer ticket) merges the slots in tile order with Chan's formula and writes (mean, rstd) for
 // the next launch.  No float atomics: two launches give identical bits.
+// A launch covers B images x nenc encoders, blockIdx.z = nenc * image + encoder.  Image b owns block b of the workspace
+// (its activations, statistics partials, (mean, rstd) slots and tickets), so each (image, encoder) z-slice reads,
+// writes and merges exactly what a single-image launch does, and its outputs are bit-identical to encoding it alone.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace dpvo {
@@ -31,7 +36,10 @@ constexpr int EC_STEM_K = 147, EC_STEM_KC = 20;                // 3 x 7 x 7 taps
 constexpr int EC_NLAYERS = 11;
 constexpr int EC_BIAS_STRIDE = 384;
 constexpr float EC_EPS = 1e-5f;
+constexpr int EC_MAX_IMAGES = 64;                              // images per launch: gridDim.z <= 128, rows fit the params
 
+// Pointers are image 0's.  Image b's are y + row[b] y_sr and pool + row[b] pool_sr (elements), the stem's x + b x_sb
+// (elements), and every other pointer + b ws_sb (bytes: its block of the workspace).
 struct EncSide {
   const void* x;                   // stem: uint8 [3, H, W] (strides xs); otherwise fp16 NHWC [Hin, Win, CIN] dense
   int64_t xs_c, xs_y, xs_x;
@@ -44,9 +52,9 @@ struct EncSide {
   const __half* w;                 // [taps][CIN / 8][COUT][8]
   const float* bias;               // [COUT]
   __half* y;                       // [Hout, Wout, COUT] with pixel strides y_sy, y_sx, channel stride 1
-  int64_t y_sy, y_sx;
+  int64_t y_sy, y_sx, y_sr;
   __half* pool;                    // optional 4x4 average of y (fmap2): strides pool_sy, pool_sx
-  int64_t pool_sy, pool_sx;
+  int64_t pool_sy, pool_sx, pool_sr;
   float* part;                     // [tiles][3][COUT] per-CTA (count, mean, M2), with stats
   float* stats;                    // optional [2][COUT] (mean, rstd) of y
   int* ticket;
@@ -56,7 +64,25 @@ struct EncSide {
 struct EncConvParams {
   EncSide e[2];
   int Hin, Win, Hout, Wout, tiles_x;
+  int nenc;                        // encoders per image
+  int64_t x_sb, ws_sb;
+  int row[EC_MAX_IMAGES];          // destination row of each image's y / pool
 };
+
+// blockIdx.z read where it is used: volatile, so the image index is not held in registers across the MMA loop
+__device__ __forceinline__ int cta_z() {
+  int z;
+  asm volatile("mov.u32 %0, %%ctaid.z;" : "=r"(z));
+  return z;
+}
+
+// image b's copy of a workspace pointer (null stays null).  Byte-pointer arithmetic, not an integer round trip, so the
+// compiler keeps the kernel parameter's global address space (LDG / STG rather than generic loads and stores).
+template <class T>
+__device__ __forceinline__ T* img_ptr(T* q, int64_t bytes) {
+  using Byte = typename std::conditional<std::is_const<T>::value, const char, char>::type;
+  return q == nullptr ? q : reinterpret_cast<T*>(reinterpret_cast<Byte*>(q) + bytes);
+}
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -115,7 +141,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
   __shared__ float s_mrg[EC_THREADS][3];
   __shared__ int s_last;
 
-  const EncSide& E = p.e[blockIdx.z];
+  const EncSide& E = p.e[blockIdx.z % p.nenc];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int tile = blockIdx.x, n0 = blockIdx.y * NT;
   const int oy0 = (tile / p.tiles_x) * EC_TH, ox0 = (tile % p.tiles_x) * EC_TW;
@@ -128,7 +154,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
 
   // ---- input halo
   if constexpr (STEM) {
-    const uint8_t* im = static_cast<const uint8_t*>(E.x);
+    const uint8_t* im = static_cast<const uint8_t*>(E.x) + (cta_z() / p.nenc) * p.x_sb;
     const int iy0 = oy0 * 2 - 3, ix0 = ox0 * 2 - 3;
     for (int i = tid; i < 3 * C::HALO; i += EC_THREADS) {
       const int c = i / C::HALO, hp = i % C::HALO, iy = iy0 + hp / C::HWD, ix = ix0 + hp % C::HWD;
@@ -155,16 +181,20 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
       reinterpret_cast<uint4*>(As)[kc * EC_PIX + tid] = *reinterpret_cast<uint4*>(v);
     }
   } else {
+    const int64_t wo = (cta_z() / p.nenc) * p.ws_sb;
+    const float* x_stats = img_ptr(E.x_stats, wo);
+    const float* skip_stats = img_ptr(E.skip_stats, wo);
     if (tid < CIN) {
-      s_xm[tid] = E.x_stats ? E.x_stats[tid] : 0.f;
-      s_xr[tid] = E.x_stats ? E.x_stats[CIN + tid] : 1.f;
-      s_sm[tid] = E.skip_stats ? E.skip_stats[tid] : 0.f;
-      s_sr[tid] = E.skip_stats ? E.skip_stats[CIN + tid] : 1.f;
+      s_xm[tid] = x_stats ? x_stats[tid] : 0.f;
+      s_xr[tid] = x_stats ? x_stats[CIN + tid] : 1.f;
+      s_sm[tid] = skip_stats ? skip_stats[tid] : 0.f;
+      s_sr[tid] = skip_stats ? skip_stats[CIN + tid] : 1.f;
     }
     __syncthreads();
-    const __half* X = static_cast<const __half*>(E.x);
-    const bool norm_x = E.x_stats != nullptr, norm_s = E.skip_stats != nullptr, join = E.skip != nullptr;
-    __half* joined = (E.joined != nullptr && blockIdx.y == 0) ? E.joined : nullptr;
+    const __half* X = img_ptr(static_cast<const __half*>(E.x), wo);
+    const __half* skip = img_ptr(E.skip, wo);
+    const bool norm_x = x_stats != nullptr, norm_s = skip_stats != nullptr, join = skip != nullptr;
+    __half* joined = (E.joined != nullptr && blockIdx.y == 0) ? img_ptr(E.joined, wo) : nullptr;
     const int iy0 = oy0 * S - C::PAD, ix0 = ox0 * S - C::PAD;
     for (int i = tid; i < C::HALO * C::KC; i += EC_THREADS) {
       const int hp = i / C::KC, kc = i % C::KC, iy = iy0 + hp / C::HWD, ix = ix0 + hp % C::HWD;
@@ -172,7 +202,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
       if (iy >= 0 && iy < p.Hin && ix >= 0 && ix < p.Win) {
         const int64_t off = ((int64_t)iy * p.Win + ix) * CIN + kc * 8;
         uint4 raw = *reinterpret_cast<const uint4*>(X + off);
-        uint4 sraw = join ? *reinterpret_cast<const uint4*>(E.skip + off) : make_uint4(0, 0, 0, 0);
+        uint4 sraw = join ? *reinterpret_cast<const uint4*>(skip + off) : make_uint4(0, 0, 0, 0);
         const __half* xv = reinterpret_cast<const __half*>(&raw);
         const __half* sv = reinterpret_cast<const __half*>(&sraw);
         __align__(16) __half o[8];
@@ -243,6 +273,9 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
   const int g = lane >> 2, cq = 2 * (lane & 3);
   const int vh = min(EC_TH, p.Hout - oy0), vw = min(EC_TW, p.Wout - ox0);
   const bool want_stats = E.stats != nullptr, want_pool = E.pool != nullptr;
+  const int image = cta_z() / p.nenc;
+  const int64_t wo = image * p.ws_sb;
+  __half* const Y = E.y + p.row[image] * E.y_sr;
   float sum[NB][2];
 #pragma unroll
   for (int nb = 0; nb < NB; ++nb) sum[nb][0] = sum[nb][1] = 0.f;
@@ -263,7 +296,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
         acc[mt][nb][2 * hr] = f.x;                                         // keep the rounded value for the statistics
         acc[mt][nb][2 * hr + 1] = f.y;
         if (valid) {
-          *reinterpret_cast<__half2*>(E.y + oy * E.y_sy + ox * E.y_sx + n0 + n) = h;
+          *reinterpret_cast<__half2*>(Y + oy * E.y_sy + ox * E.y_sx + n0 + n) = h;
           sum[nb][0] += f.x;
           sum[nb][1] += f.y;
         }
@@ -286,6 +319,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
         }
     __syncthreads();
     const int ch = p.Hout / 4, cw = p.Wout / 4;
+    __half* const pool = E.pool + p.row[image] * E.pool_sr;
     for (int i = tid; i < (EC_TH / 4) * (EC_TW / 4) * NT; i += EC_THREADS) {
       const int cell = i / NT, c = i % NT, cy = cell / (EC_TW / 4), cx = cell % (EC_TW / 4);
       const int gy = oy0 / 4 + cy, gx = ox0 / 4 + cx;
@@ -295,7 +329,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
         for (int r = 0; r < 4; ++r)
 #pragma unroll
           for (int q = 0; q < 4; ++q) s += __half2float(ost[((cy * 4 + r) * EC_TW + cx * 4 + q) * C::OST + c]);
-        E.pool[gy * E.pool_sy + gx * E.pool_sx + n0 + c] = __float2half_rn(s / 16.f);
+        pool[gy * E.pool_sy + gx * E.pool_sx + n0 + c] = __float2half_rn(s / 16.f);
       }
     }
   }
@@ -336,15 +370,17 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
       if (g == 0) s_red[warp][nb * 8 + cq + j] = s;
     }
   __syncthreads();
+  float* const parts = img_ptr(E.part, wo);
+  int* const ticket = img_ptr(E.ticket, wo);
   if (tid < NT) {
-    float* slot = E.part + (int64_t)tile * 3 * cout;
+    float* slot = parts + (int64_t)tile * 3 * cout;
     slot[n0 + tid] = cnt;
     slot[cout + n0 + tid] = s_mean[tid];
     slot[2 * cout + n0 + tid] = ((s_red[0][tid] + s_red[1][tid]) + s_red[2][tid]) + s_red[3][tid];
   }
   __threadfence();
   __syncthreads();
-  if (tid == 0) s_last = atomicAdd(E.ticket, 1) == (int)(gridDim.x * gridDim.y) - 1;
+  if (tid == 0) s_last = atomicAdd(ticket, 1) == (int)(gridDim.x * gridDim.y) - 1;   // this (image, encoder)
   __syncthreads();
   if (!s_last) return;
   __threadfence();
@@ -355,7 +391,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
     const int t0 = tiles * part / G, t1 = tiles * (part + 1) / G;
     float n = 0.f, mean = 0.f, m2 = 0.f;
     for (int t = t0; t < t1; ++t) {
-      const float* slot = E.part + (int64_t)t * 3 * cout;
+      const float* slot = parts + (int64_t)t * 3 * cout;
       chan_merge(n, mean, m2, __ldcg(slot + c), __ldcg(slot + cout + c), __ldcg(slot + 2 * cout + c));
     }
     s_mrg[tid][0] = n; s_mrg[tid][1] = mean; s_mrg[tid][2] = m2;
@@ -364,47 +400,74 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
   if (c < cout && part == 0) {
     float n = 0.f, mean = 0.f, m2 = 0.f;
     for (int q = 0; q < G; ++q) chan_merge(n, mean, m2, s_mrg[tid + q][0], s_mrg[tid + q][1], s_mrg[tid + q][2]);
-    E.stats[c] = mean;
-    E.stats[cout + c] = 1.0f / sqrtf(m2 / n + EC_EPS);
+    float* const stats = img_ptr(E.stats, wo);
+    stats[c] = mean;
+    stats[cout + c] = 1.0f / sqrtf(m2 / n + EC_EPS);
   }
-  if (tid == 0) *E.ticket = 0;                                           // ready for the next launch
+  if (tid == 0) *ticket = 0;                                             // ready for the next launch
 }
 
-// inet's output convolution at the M centroids, the gmap windows of the written fmap1 slot and the patch grids
+// inet's output convolution at the M centroids, the gmap windows of the written fmap1 slot and the patch grids.
+// Block (m, b): centroid m of image b, whose rows are frame_row[b] (fmap1), feat_row[b] + m (gmap, imap) and
+// patch_row[b] + m (patches).
+struct EncCentroidParams {
+  const float* coords;             // [B, M, 2]
+  const float* depth;              // [B, M] or null: depth 1
+  int M, h, w, cout;
+  const __half* b3;                // image 0's level-2 block output and t9 (+ b ws_sb bytes for image b)
+  const __half* t9;
+  int64_t ws_sb;
+  const __half* W;
+  const float* bias;
+  const __half* fmap1;
+  int64_t f_sr, f_sy, f_sx;
+  __half* gmap;
+  int64_t g_sm, g_sy, g_sx;
+  __half* imap;
+  int64_t i_sm;
+  float* patches;                  // rows of 27
+  int frame_row[EC_MAX_IMAGES], feat_row[EC_MAX_IMAGES], patch_row[EC_MAX_IMAGES];
+};
+
 __global__ void __launch_bounds__(128)
-enc_centroid_kernel(const float* __restrict__ coords, int h, int w, const __half* __restrict__ b3, const __half* __restrict__ t9,
-                    const __half* __restrict__ W, const float* __restrict__ bias, int cout, const __half* __restrict__ fmap1,
-                    int64_t f_sy, int64_t f_sx, __half* __restrict__ gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx,
-                    __half* __restrict__ imap, int64_t i_sm, float* __restrict__ patches) {
+enc_centroid_kernel(const __grid_constant__ EncCentroidParams p) {
   __shared__ float xin[64];
-  const int m = blockIdx.x, tid = threadIdx.x;
-  const float fx = coords[2 * m], fy = coords[2 * m + 1];
+  const int m = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, h = p.h, w = p.w;
+  const int64_t bm = (int64_t)b * p.M + m;
+  const float fx = p.coords[2 * bm], fy = p.coords[2 * bm + 1];
   const int x = (int)floorf(fx), y = (int)floorf(fy);
   const bool inside = x >= 0 && x < w && y >= 0 && y < h;
   if (tid < 64) {
     float v = 0.f;
     if (inside) {
+      const __half* b3 = img_ptr(p.b3, b * p.ws_sb);
+      const __half* t9 = img_ptr(p.t9, b * p.ws_sb);
       const int64_t off = ((int64_t)y * w + x) * 64 + tid;                 // block 4 of inet: relu(b3 + relu(t9))
       v = __half2float(__float2half_rn(fmaxf(__fadd_rn(__half2float(b3[off]), fmaxf(__half2float(t9[off]), 0.f)), 0.f)));
     }
     xin[tid] = v;
   }
   __syncthreads();
-  for (int co = tid; co < cout; co += 128) {
+  const int64_t fr = p.feat_row[b] + (int64_t)m;
+  __half* const imap = p.imap + fr * p.i_sm;
+  for (int co = tid; co < p.cout; co += 128) {
     float a = 0.f;
 #pragma unroll 8
-    for (int ci = 0; ci < 64; ++ci) a = fmaf(xin[ci], __half2float(W[((ci >> 3) * cout + co) * 8 + (ci & 7)]), a);
-    imap[m * i_sm + co] = __float2half_rn((a + bias[co]) * 0.25f);
+    for (int ci = 0; ci < 64; ++ci) a = fmaf(xin[ci], __half2float(p.W[((ci >> 3) * p.cout + co) * 8 + (ci & 7)]), a);
+    imap[co] = __float2half_rn((a + p.bias[co]) * 0.25f);
   }
+  const __half* const fmap1 = p.fmap1 + p.frame_row[b] * p.f_sr;
+  __half* const gmap = p.gmap + fr * p.g_sm;
   for (int i = tid; i < 9 * 16; i += 128) {
     const int tap = i / 16, c8 = i % 16, dy = tap / 3, dx = tap % 3, yy = y + dy - 1, xx = x + dx - 1;
     uint4 v = make_uint4(0, 0, 0, 0);
-    if (yy >= 0 && yy < h && xx >= 0 && xx < w) v = *reinterpret_cast<const uint4*>(fmap1 + yy * f_sy + xx * f_sx + c8 * 8);
-    *reinterpret_cast<uint4*>(gmap + m * g_sm + dy * g_sy + dx * g_sx + c8 * 8) = v;
+    if (yy >= 0 && yy < h && xx >= 0 && xx < w) v = *reinterpret_cast<const uint4*>(fmap1 + yy * p.f_sy + xx * p.f_sx + c8 * 8);
+    *reinterpret_cast<uint4*>(gmap + dy * p.g_sy + dx * p.g_sx + c8 * 8) = v;
   }
   if (tid < 27) {
     const int c = tid / 9, i = (tid / 3) % 3, j = tid % 3;
-    patches[m * 27 + tid] = c == 0 ? fx + (float)(j - 1) : c == 1 ? fy + (float)(i - 1) : 1.0f;
+    const float d = p.depth ? p.depth[bm] : 1.0f;
+    p.patches[(p.patch_row[b] + (int64_t)m) * 27 + tid] = c == 0 ? fx + (float)(j - 1) : c == 1 ? fy + (float)(i - 1) : d;
   }
 }
 
@@ -434,7 +497,7 @@ static inline int64_t layer_halves(int shape) {
 static inline int64_t ntiles(int ho, int wo) { return (int64_t)((ho + EC_TH - 1) / EC_TH) * ((wo + EC_TW - 1) / EC_TW); }
 
 template <int KS, int S, int CIN, int NT, bool STEM>
-static int launch_conv(const EncConvParams& p, int nenc, int cout, const char* name, cudaStream_t st) {
+static int launch_conv(const EncConvParams& p, int nimg, int cout, const char* name, cudaStream_t st) {
   using C = EncCfg<KS, S, CIN, NT, STEM>;
   auto kern = enc_conv_kernel<KS, S, CIN, NT, STEM>;
   static bool attr = false;                                              // per instantiation
@@ -443,21 +506,22 @@ static int launch_conv(const EncConvParams& p, int nenc, int cout, const char* n
     if (e != cudaSuccess) return check_cuda(e, name);
     attr = true;
   }
-  dim3 grid((unsigned)ntiles(p.Hout, p.Wout), (unsigned)(cout / NT), (unsigned)nenc);
+  dim3 grid((unsigned)ntiles(p.Hout, p.Wout), (unsigned)(cout / NT), (unsigned)(nimg * p.nenc));
   kern<<<grid, EC_THREADS, C::SMEM, st>>>(p, cout);
   DPVO_LAUNCH_CHECK(name);
   return DPVO_OK;
 }
 
-static int launch_shape(int shape, const EncConvParams& p, int nenc, cudaStream_t st) {
+// one launch of layer `shape` over nimg images x p.nenc encoders
+static int launch_shape(int shape, const EncConvParams& p, int nimg, cudaStream_t st) {
   switch (shape) {
-    case DPVO_ENC_STEM: return launch_conv<7, 2, 8, 32, true>(p, nenc, 32, "encoder_conv stem", st);
-    case DPVO_ENC_C3_32: return launch_conv<3, 1, 32, 32, false>(p, nenc, 32, "encoder_conv 3x3/1 32", st);
-    case DPVO_ENC_C3S2_32_64: return launch_conv<3, 2, 32, 64, false>(p, nenc, 64, "encoder_conv 3x3/2 32->64", st);
-    case DPVO_ENC_C1S2_32_64: return launch_conv<1, 2, 32, 64, false>(p, nenc, 64, "encoder_conv 1x1/2 32->64", st);
-    case DPVO_ENC_C3_64: return launch_conv<3, 1, 64, 64, false>(p, nenc, 64, "encoder_conv 3x3/1 64", st);
-    case DPVO_ENC_OUT_128: return launch_conv<1, 1, 64, 64, false>(p, nenc, 128, "encoder_conv 1x1 64->128", st);
-    case DPVO_ENC_OUT_384: return launch_conv<1, 1, 64, 64, false>(p, nenc, 384, "encoder_conv 1x1 64->384", st);
+    case DPVO_ENC_STEM: return launch_conv<7, 2, 8, 32, true>(p, nimg, 32, "encoder_conv stem", st);
+    case DPVO_ENC_C3_32: return launch_conv<3, 1, 32, 32, false>(p, nimg, 32, "encoder_conv 3x3/1 32", st);
+    case DPVO_ENC_C3S2_32_64: return launch_conv<3, 2, 32, 64, false>(p, nimg, 64, "encoder_conv 3x3/2 32->64", st);
+    case DPVO_ENC_C1S2_32_64: return launch_conv<1, 2, 32, 64, false>(p, nimg, 64, "encoder_conv 1x1/2 32->64", st);
+    case DPVO_ENC_C3_64: return launch_conv<3, 1, 64, 64, false>(p, nimg, 64, "encoder_conv 3x3/1 64", st);
+    case DPVO_ENC_OUT_128: return launch_conv<1, 1, 64, 64, false>(p, nimg, 128, "encoder_conv 1x1 64->128", st);
+    case DPVO_ENC_OUT_384: return launch_conv<1, 1, 64, 64, false>(p, nimg, 384, "encoder_conv 1x1 64->384", st);
   }
   set_error("encoder_conv: unknown shape %d", shape);
   return DPVO_ERR_INVALID;
@@ -486,6 +550,7 @@ extern "C" int dpvo_encoder_conv(int shape, int H, int W, int nenc, const dpvo_e
   EncConvParams p{};
   p.Hin = H; p.Win = W; p.Hout = out_size(H, si.ks, si.s); p.Wout = out_size(W, si.ks, si.s);
   p.tiles_x = (p.Wout + EC_TW - 1) / EC_TW;
+  p.nenc = nenc;
   const int64_t tiles = ntiles(p.Hout, p.Wout);
   const int64_t part_bytes = tiles * 3 * si.cout * (int64_t)sizeof(float);
   bool any_stats = false;
@@ -519,7 +584,7 @@ extern "C" int dpvo_encoder_conv(int shape, int H, int W, int nenc, const dpvo_e
     cudaError_t ce = cudaMemsetAsync(ws + 2 * part_bytes, 0, 2 * sizeof(int), (cudaStream_t)stream);
     if (ce != cudaSuccess) return check_cuda(ce, "encoder_conv: ticket reset");
   }
-  return launch_shape(shape, p, nenc, (cudaStream_t)stream);
+  return launch_shape(shape, p, 1, (cudaStream_t)stream);
 }
 
 // ---- whole frame
@@ -550,10 +615,12 @@ FrameLayout frame_layout(int H, int W) {
 }
 }  // namespace
 
-extern "C" int64_t dpvo_encode_frame_workspace_bytes(int H, int W) {
-  if (H < 1 || W < 1) return 0;
-  return frame_layout(H, W).bytes;
+extern "C" int64_t dpvo_encode_frames_workspace_bytes(int B, int H, int W) {
+  if (B < 1 || B > EC_MAX_IMAGES || H < 1 || W < 1) return 0;
+  return B * frame_layout(H, W).bytes;
 }
+
+extern "C" int64_t dpvo_encode_frame_workspace_bytes(int H, int W) { return dpvo_encode_frames_workspace_bytes(1, H, W); }
 
 // offset (halves) of layer `layer` of encoder `encoder` (0 fnet, 1 inet) in the packed weight blob
 static int64_t weight_offset(int encoder, int layer) {
@@ -566,29 +633,58 @@ static int64_t weight_offset(int encoder, int layer) {
   return o;
 }
 
-extern "C" int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y, int64_t s_x, int H, int W,
-                                 const void* w16, const float* b32, const float* coords, int M,
-                                 void* fmap1, int64_t f1_sy, int64_t f1_sx, void* fmap2, int64_t f2_sy, int64_t f2_sx,
-                                 void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm,
-                                 float* patches, void* workspace, int64_t workspace_bytes, void* stream) {
-  DPVO_REQUIRE(image && w16 && b32 && coords && fmap1 && fmap2 && gmap && imap && patches && workspace, "encode_frame: null pointer");
-  DPVO_REQUIRE(H >= 16 && W >= 16 && (int64_t)H * W < (1ll << 26), "encode_frame: image size %dx%d outside [16, 2^26 pixels]", H, W);
-  DPVO_REQUIRE(M >= 1 && M < (1 << 20), "encode_frame: M=%d", M);
-  DPVO_REQUIRE(s_c >= 0 && s_y >= 0 && s_x >= 0, "encode_frame: negative image strides");
+// rows [a, a + n) and [b, b + n) share a row
+static bool rows_overlap(int64_t a, int64_t b, int64_t n) { return a < b + n && b < a + n; }
+
+extern "C" int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
+                                  const void* w16, const float* b32, const float* coords, int M,
+                                  void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
+                                  void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
+                                  void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm, int64_t feat_rows,
+                                  float* patches, int64_t patch_rows,
+                                  const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
+                                  const float* depth, void* workspace, int64_t workspace_bytes, void* stream) {
+  DPVO_REQUIRE(B >= 1 && B <= EC_MAX_IMAGES, "encode_frames: B=%d images, 1 to %d per call", B, EC_MAX_IMAGES);
+  DPVO_REQUIRE(images && w16 && b32 && coords && fmap1 && fmap2 && gmap && imap && patches && frame_row && feat_row && patch_row &&
+               workspace, "encode_frames: null pointer");
+  DPVO_REQUIRE(H >= 16 && W >= 16 && (int64_t)H * W < (1ll << 26), "encode_frames: image size %dx%d outside [16, 2^26 pixels]", H, W);
+  DPVO_REQUIRE(M >= 1 && M < (1 << 20), "encode_frames: M=%d", M);
+  DPVO_REQUIRE(s_b >= 0 && s_c >= 0 && s_y >= 0 && s_x >= 0, "encode_frames: negative image strides");
   DPVO_REQUIRE(al16(w16) && al16(fmap1) && al16(fmap2) && al16(gmap) && al16(workspace) && ((uintptr_t)b32 & 3) == 0 &&
-               ((uintptr_t)coords & 3) == 0 && ((uintptr_t)imap & 1) == 0 && ((uintptr_t)patches & 3) == 0,
-               "encode_frame: misaligned pointer (w16, fmap1, fmap2, gmap and workspace need 16 bytes)");
+               ((uintptr_t)coords & 3) == 0 && ((uintptr_t)imap & 1) == 0 && ((uintptr_t)patches & 3) == 0 &&
+               ((uintptr_t)depth & 3) == 0 && f1_sr % 8 == 0 && f2_sr % 8 == 0,
+               "encode_frames: misaligned pointer (w16, fmap1, fmap2, gmap, workspace and the fmap1 / fmap2 rows need 16 bytes)");
   DPVO_REQUIRE(f1_sx >= 128 && f1_sx % 8 == 0 && f1_sy % 8 == 0 && f2_sx >= 128 && f2_sx % 8 == 0 && f2_sy % 8 == 0,
-               "encode_frame: fmap1 / fmap2 must be channels-last (channel stride 1) with pixel strides that are multiples of 8");
+               "encode_frames: fmap1 / fmap2 must be channels-last (channel stride 1) with pixel strides that are multiples of 8");
   DPVO_REQUIRE(g_sx >= 128 && g_sx % 8 == 0 && g_sy % 8 == 0 && g_sm % 8 == 0 && i_sm >= 384,
-               "encode_frame: gmap must be [M, 3, 3, 128] channels-last with strides that are multiples of 8, imap [M, 384]");
+               "encode_frames: gmap must be [M, 3, 3, 128] channels-last with strides that are multiples of 8, imap [M, 384]");
+  DPVO_REQUIRE(frame_rows >= 1 && frame_rows < (1ll << 31) && feat_rows >= 1 && feat_rows < (1ll << 31) && patch_rows >= 1 &&
+               patch_rows < (1ll << 31), "encode_frames: ring sizes must be 1 to 2^31 - 1 rows");
+  for (int b = 0; b < B; ++b) {
+    DPVO_REQUIRE(frame_row[b] >= 0 && frame_row[b] < frame_rows, "encode_frames: image %d: frame row %lld outside the %lld-row fmap1 / fmap2 ring",
+                 b, (long long)frame_row[b], (long long)frame_rows);
+    DPVO_REQUIRE(feat_row[b] >= 0 && feat_row[b] + M <= feat_rows, "encode_frames: image %d: patch-feature rows [%lld, %lld) outside the "
+                 "%lld-row gmap / imap ring", b, (long long)feat_row[b], (long long)feat_row[b] + M, (long long)feat_rows);
+    DPVO_REQUIRE(patch_row[b] >= 0 && patch_row[b] + M <= patch_rows, "encode_frames: image %d: patch rows [%lld, %lld) outside the "
+                 "%lld patches", b, (long long)patch_row[b], (long long)patch_row[b] + M, (long long)patch_rows);
+    for (int a = 0; a < b; ++a) {
+      DPVO_REQUIRE(frame_row[a] != frame_row[b], "encode_frames: images %d and %d write the same destination fmap1 / fmap2 row %lld",
+                   a, b, (long long)frame_row[b]);
+      DPVO_REQUIRE(!rows_overlap(feat_row[a], feat_row[b], M), "encode_frames: images %d and %d write the same destination gmap / imap "
+                   "rows (first rows %lld and %lld, M=%d)", a, b, (long long)feat_row[a], (long long)feat_row[b], M);
+      DPVO_REQUIRE(!rows_overlap(patch_row[a], patch_row[b], M), "encode_frames: images %d and %d write the same destination patch "
+                   "rows (first rows %lld and %lld, M=%d)", a, b, (long long)patch_row[a], (long long)patch_row[b], M);
+    }
+  }
   const FrameLayout L = frame_layout(H, W);
-  DPVO_REQUIRE(workspace_bytes >= L.bytes, "encode_frame: workspace %lld B < required %lld B", (long long)workspace_bytes, (long long)L.bytes);
+  DPVO_REQUIRE(workspace_bytes >= B * L.bytes, "encode_frames: workspace %lld B < required %lld B", (long long)workspace_bytes,
+               (long long)(B * L.bytes));
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* ws = (uint8_t*)workspace;
   const __half* wh = (const __half*)w16;
-  cudaError_t ce = cudaMemsetAsync(ws + L.tickets, 0, 256, st);
-  if (ce != cudaSuccess) return check_cuda(ce, "encode_frame: ticket reset");
+  // every image's tickets (256 bytes at the same offset of each workspace block): one strided memset for the batch
+  cudaError_t ce = cudaMemset2DAsync(ws + L.tickets, (size_t)L.bytes, 0, 256, (size_t)B, st);
+  if (ce != cudaSuccess) return check_cuda(ce, "encode_frames: ticket reset");
 
   auto X = [&](int e, int i) { return (__half*)(ws + L.x[e][i]); };
   auto Y = [&](int e, int i) { return (__half*)(ws + L.y[e][i]); };
@@ -596,7 +692,7 @@ extern "C" int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y,
   auto Wt = [&](int e, int l) { return wh + weight_offset(e, l); };
   auto Bt = [&](int e, int l) { return b32 + (e * EC_NLAYERS + l) * EC_BIAS_STRIDE; };
 
-  // one launch per layer for both encoders; (input, input stats, skip, skip stats, skip relu, joined) -> output
+  // one launch per layer for both encoders of every image; (input, input stats, skip, skip stats, skip relu, joined) -> output
   struct Step { int layer; int lvl_in; int x, skip, joined; int lvl_out; int y; bool skip_norm, skip_relu; };
   // buffer index: 0..3 = level-1 buffers X, 4..7 = level-2 buffers Y, -1 = none
   const Step steps[] = {
@@ -619,14 +715,16 @@ extern "C" int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y,
     EncConvParams p{};
     p.Hin = Hin; p.Win = Win; p.Hout = out_size(Hin, si.ks, si.s); p.Wout = out_size(Win, si.ks, si.s);
     p.tiles_x = (p.Wout + EC_TW - 1) / EC_TW;
+    p.nenc = 2; p.x_sb = s_b; p.ws_sb = L.bytes;
+    for (int b = 0; b < B; ++b) p.row[b] = b;                            // y: image b's workspace block
     for (int e = 0; e < 2; ++e) {
       EncSide& d = p.e[e];
       // the producer of x (and of skip) is the layer that wrote that buffer; its stats slot is the layer index
-      d.x = s.layer == 0 ? (const void*)image : buf(e, s.lvl_in, s.x);
+      d.x = s.layer == 0 ? (const void*)images : buf(e, s.lvl_in, s.x);
       d.xs_c = s_c; d.xs_y = s_y; d.xs_x = s_x;
       d.x_relu = 1;
       d.w = Wt(e, s.layer); d.bias = Bt(e, s.layer);
-      d.y = buf(e, s.lvl_out, s.y); d.y_sy = (int64_t)p.Wout * si.cout; d.y_sx = si.cout;
+      d.y = buf(e, s.lvl_out, s.y); d.y_sy = (int64_t)p.Wout * si.cout; d.y_sx = si.cout; d.y_sr = L.bytes / 2;
       d.stats = S(e, s.layer); d.part = (float*)(ws + L.parts + e * L.part); d.ticket = (int*)(ws + L.tickets) + e * 16 + s.layer;
       d.scale = 1.0f;
     }
@@ -649,23 +747,45 @@ extern "C" int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y,
       if (!s.skip_norm) p.e[e].skip_stats = nullptr;
       p.e[e].joined = buf(e, s.lvl_in, s.joined);
     }
-    const int rc = launch_shape(shape, p, 2, st);
+    const int rc = launch_shape(shape, p, B, st);
     if (rc != DPVO_OK) return rc;
   }
   {  // fnet output: b4 = relu(b3 + act(t9)) -> (. W + b) / 4 -> fmap1 slot and its 4x4 average -> fmap2 slot
     EncConvParams p{};
     p.Hin = p.Hout = L.H2; p.Win = p.Wout = L.W2; p.tiles_x = (L.W2 + EC_TW - 1) / EC_TW;
+    p.nenc = 1; p.ws_sb = L.bytes;
+    for (int b = 0; b < B; ++b) p.row[b] = (int)frame_row[b];
     EncSide& d = p.e[0];
     d.x = Y(0, 1); d.x_stats = S(0, 9); d.x_relu = 1; d.skip = Y(0, 0);
     d.w = Wt(0, 10); d.bias = Bt(0, 10);
-    d.y = (__half*)fmap1; d.y_sy = f1_sy; d.y_sx = f1_sx;
-    d.pool = (__half*)fmap2; d.pool_sy = f2_sy; d.pool_sx = f2_sx;
+    d.y = (__half*)fmap1; d.y_sy = f1_sy; d.y_sx = f1_sx; d.y_sr = f1_sr;
+    d.pool = (__half*)fmap2; d.pool_sy = f2_sy; d.pool_sx = f2_sx; d.pool_sr = f2_sr;
     d.scale = 0.25f;
-    const int rc = launch_shape(DPVO_ENC_OUT_128, p, 1, st);
+    const int rc = launch_shape(DPVO_ENC_OUT_128, p, B, st);
     if (rc != DPVO_OK) return rc;
   }
-  enc_centroid_kernel<<<M, 128, 0, st>>>(coords, L.H2, L.W2, Y(1, 0), Y(1, 1), Wt(1, 10), Bt(1, 10), 384, (const __half*)fmap1,
-                                         f1_sy, f1_sx, (__half*)gmap, g_sm, g_sy, g_sx, (__half*)imap, i_sm, patches);
+  EncCentroidParams c{};
+  c.coords = coords; c.depth = depth; c.M = M; c.h = L.H2; c.w = L.W2; c.cout = 384;
+  c.b3 = Y(1, 0); c.t9 = Y(1, 1); c.ws_sb = L.bytes; c.W = Wt(1, 10); c.bias = Bt(1, 10);
+  c.fmap1 = (const __half*)fmap1; c.f_sr = f1_sr; c.f_sy = f1_sy; c.f_sx = f1_sx;
+  c.gmap = (__half*)gmap; c.g_sm = g_sm; c.g_sy = g_sy; c.g_sx = g_sx;
+  c.imap = (__half*)imap; c.i_sm = i_sm; c.patches = patches;
+  for (int b = 0; b < B; ++b) {
+    c.frame_row[b] = (int)frame_row[b]; c.feat_row[b] = (int)feat_row[b]; c.patch_row[b] = (int)patch_row[b];
+  }
+  enc_centroid_kernel<<<dim3(M, B), 128, 0, st>>>(c);
   DPVO_LAUNCH_CHECK("enc_centroid_kernel");
   return DPVO_OK;
+}
+
+// one image: the B = 1 case of dpvo_encode_frames, its slots the single rows of rings of one frame and M patches
+extern "C" int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y, int64_t s_x, int H, int W,
+                                 const void* w16, const float* b32, const float* coords, int M,
+                                 void* fmap1, int64_t f1_sy, int64_t f1_sx, void* fmap2, int64_t f2_sy, int64_t f2_sx,
+                                 void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm,
+                                 float* patches, void* workspace, int64_t workspace_bytes, void* stream) {
+  const int64_t row0 = 0;
+  return dpvo_encode_frames(image, 0, s_c, s_y, s_x, 1, H, W, w16, b32, coords, M, fmap1, 0, f1_sy, f1_sx, fmap2, 0, f2_sy, f2_sx, 1,
+                            gmap, g_sm, g_sy, g_sx, imap, i_sm, M, patches, M, &row0, &row0, &row0, nullptr, workspace,
+                            workspace_bytes, stream);
 }

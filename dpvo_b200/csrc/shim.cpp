@@ -921,6 +921,60 @@ void encode_frame(Tensor image, Tensor w16, Tensor b32, Tensor coords, Tensor fm
 
 int64_t encode_frame_workspace_bytes(int64_t H, int64_t W) { return dpvo_encode_frame_workspace_bytes((int)H, (int)W); }
 
+// B images [B, 3, H, W] (any strides) into rows of whole rings: fmap1 [R, h, w, 128], fmap2 [R, h/4, w/4, 128], gmap
+// [Rg, 3, 3, 128] (channels-last), imap [Rg, 384], patches [Rp, 3, 3, 3]; image b into frame row frame_rows[b], patch-feature
+// rows feat_rows[b] + [0, M) and patch rows patch_rows[b] + [0, M).  The library checks the rows.
+void encode_frames(Tensor images, Tensor w16, Tensor b32, Tensor coords, Tensor fmap1, Tensor fmap2, Tensor gmap, Tensor imap,
+                   Tensor patches, std::vector<int64_t> frame_rows, std::vector<int64_t> feat_rows, std::vector<int64_t> patch_rows,
+                   c10::optional<Tensor> depth, Tensor workspace) {
+  for (auto* t : {&images, &w16, &b32, &coords, &fmap1, &fmap2, &gmap, &imap, &patches, &workspace})
+    TORCH_CHECK(t->is_cuda(), "encode_frames: every tensor must be a CUDA tensor (this build has no CPU path)");
+  TORCH_CHECK(images.scalar_type() == at::kByte && images.dim() == 4 && images.size(1) == 3, "encode_frames: images must be uint8 [B, 3, H, W]");
+  const int64_t B = images.size(0);
+  const int H = (int)images.size(2), W = (int)images.size(3);
+  const int h = ((H - 1) / 2 + 1 - 1) / 2 + 1, w = ((W - 1) / 2 + 1 - 1) / 2 + 1;
+  TORCH_CHECK(w16.scalar_type() == at::kHalf && w16.is_contiguous(), "encode_frames: w16 must be contiguous float16");
+  TORCH_CHECK(b32.scalar_type() == at::kFloat && b32.is_contiguous() && b32.numel() == 2 * 11 * 384, "encode_frames: b32 must be float32 [2, 11, 384]");
+  TORCH_CHECK(coords.scalar_type() == at::kFloat && coords.is_contiguous() && coords.dim() == 3 && coords.size(0) == B && coords.size(2) == 2,
+              "encode_frames: coords must be contiguous float32 [B, M, 2] with B = ", B);
+  const int64_t M = coords.size(1);
+  TORCH_CHECK(fmap1.scalar_type() == at::kHalf && fmap1.dim() == 4 && fmap1.size(3) == 128 && fmap1.stride(3) == 1,
+              "encode_frames: fmap1 must be a channels-last float16 ring [R, h, w, 128]");
+  TORCH_CHECK(fmap1.size(1) == h && fmap1.size(2) == w, "encode_frames: a ", H, "x", W, " image encodes to ", h, "x", w,
+              ", the fmap1 ring holds ", fmap1.size(1), "x", fmap1.size(2));
+  TORCH_CHECK(fmap2.scalar_type() == at::kHalf && fmap2.dim() == 4 && fmap2.size(0) == fmap1.size(0) && fmap2.size(1) == h / 4 &&
+              fmap2.size(2) == w / 4 && fmap2.size(3) == 128 && fmap2.stride(3) == 1,
+              "encode_frames: fmap2 must be a channels-last float16 ring [R, h/4, w/4, 128] with fmap1's R");
+  TORCH_CHECK(gmap.scalar_type() == at::kHalf && gmap.dim() == 4 && gmap.size(1) == 3 && gmap.size(2) == 3 && gmap.size(3) == 128 &&
+              gmap.stride(3) == 1, "encode_frames: gmap must be a channels-last float16 ring [Rg, 3, 3, 128]");
+  TORCH_CHECK(imap.scalar_type() == at::kHalf && imap.dim() == 2 && imap.size(0) == gmap.size(0) && imap.size(1) == 384 && imap.stride(1) == 1,
+              "encode_frames: imap must be float16 [Rg, 384] with contiguous rows and gmap's Rg");
+  TORCH_CHECK(patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.dim() == 4 && patches.size(1) == 3 &&
+              patches.size(2) == 3 && patches.size(3) == 3, "encode_frames: patches must be contiguous float32 [Rp, 3, 3, 3]");
+  TORCH_CHECK((int64_t)frame_rows.size() == B && (int64_t)feat_rows.size() == B && (int64_t)patch_rows.size() == B,
+              "encode_frames: one frame row, one patch-feature row and one patch row per image (", B, " images)");
+  const float* dp = nullptr;
+  if (depth.has_value()) {
+    TORCH_CHECK(depth->is_cuda() && depth->scalar_type() == at::kFloat && depth->is_contiguous() && depth->dim() == 2 &&
+                depth->size(0) == B && depth->size(1) == M, "encode_frames: depth must be a contiguous float32 CUDA tensor [B, M]");
+    dp = depth->data_ptr<float>();
+  }
+  TORCH_CHECK(workspace.is_contiguous(), "encode_frames: workspace must be contiguous");
+  const c10::cuda::CUDAGuard guard(images.device());
+  check(dpvo_encode_frames(images.data_ptr<uint8_t>(), images.stride(0), images.stride(1), images.stride(2), images.stride(3), (int)B, H, W,
+                           w16.data_ptr(), b32.data_ptr<float>(), coords.data_ptr<float>(), (int)M,
+                           fmap1.data_ptr(), fmap1.stride(0), fmap1.stride(1), fmap1.stride(2),
+                           fmap2.data_ptr(), fmap2.stride(0), fmap2.stride(1), fmap2.stride(2), fmap1.size(0),
+                           gmap.data_ptr(), gmap.stride(0), gmap.stride(1), gmap.stride(2), imap.data_ptr(), imap.stride(0), gmap.size(0),
+                           patches.data_ptr<float>(), patches.size(0), frame_rows.data(), feat_rows.data(), patch_rows.data(), dp,
+                           workspace.data_ptr(), workspace.numel() * workspace.element_size(), stream()),
+        "dpvo_b200_ext.encode_frames");
+}
+
+int64_t encode_frames_workspace_bytes(int64_t B, int64_t H, int64_t W) {
+  return dpvo_encode_frames_workspace_bytes((int)B, (int)H, (int)W);
+}
+
 int64_t launch_count() { return dpvo_launch_count(); }
 std::string version() { return dpvo_version(); }
 
@@ -1011,6 +1065,11 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
         py::arg("w16"), py::arg("b32"), py::arg("coords"), py::arg("fmap1"), py::arg("fmap2"), py::arg("gmap"), py::arg("imap"),
         py::arg("patches"), py::arg("workspace"));
   m.def("encode_frame_workspace_bytes", &encode_frame_workspace_bytes, "scratch bytes of encode_frame for an H x W image");
+  m.def("encode_frames", &encode_frames, "both frame encoders over B images in one pass, into rows of the rings", py::arg("images"),
+        py::arg("w16"), py::arg("b32"), py::arg("coords"), py::arg("fmap1"), py::arg("fmap2"), py::arg("gmap"), py::arg("imap"),
+        py::arg("patches"), py::arg("frame_rows"), py::arg("feat_rows"), py::arg("patch_rows"), py::arg("depth"),
+        py::arg("workspace"));
+  m.def("encode_frames_workspace_bytes", &encode_frames_workspace_bytes, "scratch bytes of encode_frames for B H x W images");
   m.def("launch_count", &launch_count, "kernel launches issued by libdpvo_b200 so far");
   m.def("version", &version, "library version string");
 }

@@ -204,8 +204,10 @@ class FrameEncoder:
                 o += n
         return out
 
-    def workspace(self, H, W, device):
-        nb = extensions()[3].encode_frame_workspace_bytes(H, W)
+    def workspace(self, H, W, device, B=1):
+        """scratch of B H x W images; it grows and is kept, so a CUDA graph captured with a larger B or image than a
+        later call's stays valid (a graph captured before a call that grows it must be captured again)"""
+        nb = extensions()[3].encode_frames_workspace_bytes(B, H, W)
         if self._ws is None or self._ws.numel() < nb or self._ws.device != device:
             self._ws = torch.empty(nb, dtype=torch.uint8, device=device)
         return self._ws
@@ -232,4 +234,30 @@ class FrameEncoder:
         w16, b32 = self.packed()
         extensions()[3].encode_frame(image, w16, b32, coords.float().contiguous(), fmap1_slot, fmap2_slot, gmap_slot,
                                      imap_slot, patches_slot, self.workspace(image.shape[1], image.shape[2], image.device))
+        return coords
+
+    @torch.no_grad()
+    def encode_frames_into(self, images, M, strategy, fmap1_ring, fmap2_ring, gmap_ring, imap_ring, patches_ring,
+                           frame_rows, feat_rows, patch_rows, coords=None, depth=None):
+        """encode_into for B images in one pass of the encoders.  images: uint8 [B, 3, H, W] (CHW or HWC strides).
+        Image b goes to row frame_rows[b] of the rings fmap1 [R, h, w, 128] and fmap2 [R, h/4, w/4, 128], rows
+        feat_rows[b] + [0, M) of gmap [Rg, 3, 3, 128] and imap [Rg, 384], and rows patch_rows[b] + [0, M) of patches
+        [Rp, 3, 3, 3] with depth[b] (fp32 [B, M]; None: depth 1).  Each image's slots are bit-identical to encode_into
+        of that image alone with the same centroids.  Centroids are drawn once per image, in image order, unless
+        `coords` [B, M, 2] is given (then nothing is drawn and the call can be captured).  Returns the coords."""
+        if not (isinstance(images, torch.Tensor) and images.is_cuda):
+            raise RuntimeError("FrameEncoder: the images must be a CUDA tensor (there is no CPU path)")
+        if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[1] != 3:
+            raise RuntimeError("FrameEncoder: the images must be uint8 [B, 3, H, W], got %s %s" % (images.dtype, tuple(images.shape)))
+        B, H, W = images.shape[0], images.shape[2], images.shape[3]
+        if B < 1:
+            raise RuntimeError("FrameEncoder: no images (B = 0)")
+        if coords is None:
+            coords = torch.stack([self.centroids(images[b], M, strategy) for b in range(B)])
+        elif coords.shape != (B, M, 2):
+            raise RuntimeError("FrameEncoder: coords must be [B, M, 2] = [%d, %d, 2], got %s" % (B, M, tuple(coords.shape)))
+        w16, b32 = self.packed()
+        extensions()[3].encode_frames(images, w16, b32, coords.float().contiguous(), fmap1_ring, fmap2_ring, gmap_ring, imap_ring,
+                                      patches_ring, [int(r) for r in frame_rows], [int(r) for r in feat_rows],
+                                      [int(r) for r in patch_rows], depth, self.workspace(H, W, images.device, B))
         return coords

@@ -210,6 +210,57 @@ class UpdateRunner:
         patches[:, 2] = depth
         return coords
 
+    @torch.no_grad()
+    def ingest_images(self, images, depth=None, coords=None, streams=None):
+        """Encode the images of several streams of a batch in one pass of the encoders: uint8 [B', 3, H, W] (or the
+        permuted [B', H, W, 3] view), image i into stream streams[i]'s slots at that stream's own n -- the slots
+        `ingest_image(images[i], stream=streams[i])` writes, with the same bytes.  `streams` lists B' distinct streams
+        (default: all B, in order), so a rig where a camera dropped a frame passes the others.
+        Without `coords` [B', M, 2] and `depth` (fp32, broadcastable to [B', M]) the CUDA generator is drawn as those
+        ingest_image calls draw it, image by image: centroid x, centroid y, then the depths.  With both given nothing
+        is drawn and the call can be captured in a CUDA graph.  Returns the centroids [B', M, 2]."""
+        if self.batch is None:
+            raise RuntimeError("ingest_images: this UpdateRunner holds one stream; use ingest_image")
+        if self.encoder is None:
+            raise RuntimeError("ingest_images: this UpdateRunner was built without an encoder")
+        batch, M = self.batch, self.M
+        if not (isinstance(images, torch.Tensor) and images.is_cuda):
+            raise RuntimeError("ingest_images: the images must be a CUDA tensor (there is no CPU path)")
+        if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[1] != 3:
+            raise RuntimeError("ingest_images: the images must be uint8 [B', 3, H, W], got %s %s" % (images.dtype, tuple(images.shape)))
+        n = images.shape[0]
+        streams = list(range(batch.B)) if streams is None else [int(b) for b in streams]
+        if len(streams) != n:
+            raise RuntimeError("ingest_images: %d images for %d streams %s" % (n, len(streams), streams))
+        if len(set(streams)) != n:
+            raise RuntimeError("ingest_images: streams %s name a stream twice" % streams)
+        bad = [b for b in streams if not 0 <= b < batch.B]
+        if bad:
+            raise RuntimeError("ingest_images: streams %s outside the batch of %d" % (bad, batch.B))
+        h, w = batch.fmap1.shape[3], batch.fmap1.shape[4]
+        if encoder_output_size(images.shape[2], images.shape[3]) != (h, w):
+            raise RuntimeError("ingest_images: a %s image encodes to %s features, the rings hold %dx%d"
+                               % (tuple(images.shape[1:]), encoder_output_size(*images.shape[-2:]), h, w))
+        empty = [b for b in streams if batch.stream(b).n < 1]
+        if empty:
+            raise RuntimeError("ingest_images: streams %s have no frame slot yet (n = 0)" % empty)
+        dev = batch.patches.device
+        if coords is None or depth is None:
+            drawn_c, drawn_d = [], []
+            for i in range(n):                                      # ingest_image's order, image by image
+                if coords is None:
+                    drawn_c.append(self.encoder.centroids(images[i], M, self.encoder.strategy))
+                if depth is None:
+                    drawn_d.append(torch.rand(M, 1, 1, device=dev, dtype=batch.patches.dtype))
+            coords = torch.stack(drawn_c) if coords is None else coords
+            depth = torch.stack(drawn_d).view(n, M) if depth is None else depth
+        depth = torch.broadcast_to(torch.as_tensor(depth, device=dev, dtype=torch.float32), (n, M)).contiguous()
+        rows = [batch.frame_rows(b) for b in streams]
+        return self.encoder.encode_frames_into(images, M, self.encoder.strategy, batch.fmap1[0].permute(0, 2, 3, 1),
+                                               batch.fmap2[0].permute(0, 2, 3, 1), batch.gmap[0].permute(0, 2, 3, 1),
+                                               batch.imap[0], batch.patches, [r[0] for r in rows], [r[1] for r in rows],
+                                               [r[2] for r in rows], coords=coords, depth=depth)
+
     # A streaming front end has frame t+1 in pinned memory while update t runs: its H2D copy goes to a staging
     # buffer on a copy stream (overlapping the update), and only the short device-to-device move into the ring
     # slots sits on the compute stream.

@@ -120,6 +120,13 @@ class StreamBatch:
         bj = torch.div(jj, self.F, rounding_mode="floor")
         return bk * PM + torch.remainder(kk - bk * FM, PM), bj * self.mem + torch.remainder(jj - bj * self.F, self.mem)
 
+    def frame_rows(self, b):
+        """rows that stream b's newest frame (local n - 1) occupies in the stacked buffers: (fmap1 / fmap2 ring row,
+        first gmap / imap ring row, first patch row).  Its M patch features and patches are the rows that follow."""
+        s = self.stream(b)
+        f = int(s.n) - 1
+        return (int(b) * self.mem + f % self.mem, (int(b) * self.pmem + f % self.pmem) * self.M, (int(b) * self.F + f) * self.M)
+
     # ------------------------------------------------------------------------------------------------ edges, windows
     def check_edges(self, ii, jj, kk):
         """reject global edge lists with an edge outside the batch or joining two streams (one host synchronisation)"""

@@ -549,6 +549,19 @@ int dpvo_pgraph_new_edges(const int64_t* n_dev, int M, int r, int64_t* ii, int64
  *   patches fp32 [M, 3, 3, 3]   (x + dx, y + dy, 1) around each centroid, contiguous
  * coords fp32 [M, 2] (x, y) integer centroids.  h, w = the encoder output size of H, W.
  * workspace: dpvo_encode_frame_workspace_bytes(H, W) bytes (activations, statistics).
+ * It is the B = 1 case of dpvo_encode_frames.
+ *
+ * dpvo_encode_frames: B (1..64) images in one pass, the same launches as one image: image b is uint8 [3, H, W] at
+ * images + b s_b (element strides s_c, s_y, s_x: a stacked [B, 3, H, W] tensor or its permuted [B, H, W, 3] view).
+ * Each image is encoded with its own instance-norm statistics, and its slots are bit-identical to dpvo_encode_frame of
+ * that image alone.  The destinations are rows of rings (element strides between rows: f1_sr, f2_sr, g_sm, i_sm, 27):
+ *   fmap1 / fmap2  row frame_row[b] of rings of frame_rows rows
+ *   gmap / imap    rows [feat_row[b], feat_row[b] + M) of rings of feat_rows rows
+ *   patches        rows [patch_row[b], patch_row[b] + M) of a [patch_rows, 3, 3, 3] buffer
+ * The row lists are host int64 [B]; a row outside its ring, or two images writing a common row, is rejected.
+ * coords fp32 [B, M, 2].  depth fp32 [B, M] (the patches' third channel), or NULL for 1.
+ * workspace: dpvo_encode_frames_workspace_bytes(B, H, W) bytes, B blocks of dpvo_encode_frame_workspace_bytes(H, W).
+ * One strided memset and 12 launches for any B; no host synchronisation (graph-capturable).
  */
 #define DPVO_ENC_STEM        0   /* 7x7/2, 3 -> 32   */
 #define DPVO_ENC_C3_32       1   /* 3x3/1, 32 -> 32  */
@@ -586,6 +599,15 @@ int dpvo_encode_frame(const uint8_t* image, int64_t s_c, int64_t s_y, int64_t s_
                       void* fmap1, int64_t f1_sy, int64_t f1_sx, void* fmap2, int64_t f2_sy, int64_t f2_sx,
                       void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm,
                       float* patches, void* workspace, int64_t workspace_bytes, void* stream);
+int64_t dpvo_encode_frames_workspace_bytes(int B, int H, int W);
+int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
+                       const void* w16, const float* b32, const float* coords, int M,
+                       void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
+                       void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
+                       void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm, int64_t feat_rows,
+                       float* patches, int64_t patch_rows,
+                       const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
+                       const float* depth, void* workspace, int64_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
