@@ -826,6 +826,105 @@ std::vector<Tensor> pgraph_new_edges(Tensor n_dev, int64_t M, int64_t r) {
   return {ii, jj, kk};
 }
 
+// ---- proximity loop closure (include/dpvo_b200.h, csrc/loop.cu)
+static void dev_scalar(const Tensor& t, at::ScalarType ty, const char* what) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == ty && t.numel() == 1, what);
+}
+static void f32_rows(const Tensor& t, int64_t rows, int64_t cols, const char* what) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == rows * cols, what);
+}
+Tensor loop_scores(Tensor poses, Tensor patches, Tensor intrinsics, Tensor n_dev, Tensor last_ba, int64_t M, int64_t removal,
+                   int64_t max_age, int64_t freq, int64_t kf_index) {
+  need_cuda(poses, "poses");
+  c10::cuda::CUDAGuard guard(poses.device());
+  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat && intrinsics.scalar_type() == at::kFloat &&
+              poses.is_contiguous() && patches.is_contiguous() && intrinsics.is_contiguous() && patches.is_cuda() && intrinsics.is_cuda(),
+              "loop_scores: poses / patches / intrinsics are contiguous fp32 CUDA tensors");
+  TORCH_CHECK(patches.numel() % 27 == 0 && patches.size(-1) == 3, "loop_scores: patches are [K, 3, 3, 3]");
+  dev_scalar(n_dev, at::kLong, "loop_scores: n is a device int64 scalar");
+  dev_scalar(last_ba, at::kLong, "loop_scores: last_global_ba is a device int64 scalar");
+  const int64_t S = dpvo_loop_candidates((int)max_age, (int)freq, (int)kf_index);
+  Tensor scores = torch::empty({std::max<int64_t>(S, 1)}, poses.options());
+  check(dpvo_loop_scores(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(), n_dev.data_ptr<int64_t>(),
+                         last_ba.data_ptr<int64_t>(), (int)M, (int)removal, (int)max_age, (int)freq, (int)kf_index, scores.data_ptr<float>(),
+                         stream()),
+        "dpvo_b200_ext.loop_scores");
+  return scores;
+}
+void loop_select(Tensor scores, Tensor n_dev, Tensor last_ba, int64_t M, int64_t removal, int64_t max_age, int64_t freq, int64_t kf_index,
+                 double thresh, Tensor pairs, Tensor n_pairs, Tensor ii, Tensor jj, Tensor kk, Tensor active, c10::optional<Tensor> state,
+                 Tensor n_active, Tensor overflow) {
+  need_cuda(scores, "scores");
+  c10::cuda::CUDAGuard guard(scores.device());
+  const int64_t S = dpvo_loop_candidates((int)max_age, (int)freq, (int)kf_index);
+  f32_rows(scores, S, 1, "loop_select: scores are the fp32 [J * max_age] output of loop_scores");
+  dev_scalar(n_dev, at::kLong, "loop_select: n is a device int64 scalar");
+  dev_scalar(last_ba, at::kLong, "loop_select: last_global_ba is a device int64 scalar");
+  dev_scalar(n_pairs, at::kInt, "loop_select: n_pairs is a device int32 scalar");
+  dev_scalar(n_active, at::kInt, "loop_select: n_active is a device int32 scalar");
+  dev_scalar(overflow, at::kInt, "loop_select: overflow is a device int32 scalar");
+  TORCH_CHECK(pairs.is_cuda() && pairs.scalar_type() == at::kLong && pairs.is_contiguous() && pairs.dim() == 2 && pairs.size(1) == 2,
+              "loop_select: pairs is a contiguous device int64 [max_pairs, 2]");
+  pg_check(ii, jj, kk, active);
+  float* st = nullptr;
+  if (state.has_value()) {
+    f32_rows(*state, ii.numel(), 384, "loop_select: state must be the contiguous fp32 [region, 384] recurrent state of the loop region");
+    st = state->data_ptr<float>();
+  }
+  check(dpvo_loop_select(scores.data_ptr<float>(), n_dev.data_ptr<int64_t>(), last_ba.data_ptr<int64_t>(), (int)M, (int)removal, (int)max_age,
+                         (int)freq, (int)kf_index, (float)thresh, (int)pairs.size(0), pairs.data_ptr<int64_t>(), n_pairs.data_ptr<int>(),
+                         ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(), st,
+                         n_active.data_ptr<int>(), overflow.data_ptr<int>(), stream()),
+        "dpvo_b200_ext.loop_select");
+}
+void pgraph_remove_store(Tensor ii, Tensor jj, Tensor kk, Tensor active, Tensor target, Tensor weight, Tensor n_dev, int64_t removal,
+                         int64_t opt_window, c10::optional<Tensor> enable, int64_t dummy_frame, int64_t dummy_patch, int64_t M, Tensor n_active,
+                         Tensor s_ii, Tensor s_jj, Tensor s_kk, Tensor s_target, Tensor s_weight, Tensor s_count, Tensor s_overflow) {
+  need_cuda(ii, "ii");
+  c10::cuda::CUDAGuard guard(ii.device());
+  pg_check(ii, jj, kk, active);
+  const int64_t cap = ii.numel(), sc = s_ii.numel();
+  f32_rows(target, cap, 2, "pgraph_remove_store: target is the contiguous fp32 [cap, 2] of the active store");
+  f32_rows(weight, cap, 2, "pgraph_remove_store: weight is the contiguous fp32 [cap, 2] of the active store");
+  TORCH_CHECK(s_ii.is_cuda() && s_ii.scalar_type() == at::kLong && s_ii.is_contiguous() && s_jj.scalar_type() == at::kLong && s_jj.is_contiguous() &&
+              s_kk.scalar_type() == at::kLong && s_kk.is_contiguous() && s_jj.numel() == sc && s_kk.numel() == sc,
+              "pgraph_remove_store: the inactive ii / jj / kk are contiguous device int64, one entry per slot");
+  f32_rows(s_target, sc, 2, "pgraph_remove_store: the inactive target is contiguous fp32 [store, 2]");
+  f32_rows(s_weight, sc, 2, "pgraph_remove_store: the inactive weight is contiguous fp32 [store, 2]");
+  dev_scalar(n_dev, at::kLong, "pgraph_remove_store: n is a device int64 scalar");
+  dev_scalar(n_active, at::kInt, "pgraph_remove_store: n_active is a device int32 scalar");
+  dev_scalar(s_count, at::kInt, "pgraph_remove_store: the store count is a device int32 scalar");
+  dev_scalar(s_overflow, at::kInt, "pgraph_remove_store: the store overflow flag is a device int32 scalar");
+  const int32_t* en = nullptr;
+  if (enable.has_value()) { dev_scalar(*enable, at::kInt, "pgraph_remove_store: enable is a device int32 scalar"); en = enable->data_ptr<int>(); }
+  check(dpvo_pgraph_remove_store(ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(),
+                                 target.data_ptr<float>(), weight.data_ptr<float>(), cap, n_dev.data_ptr<int64_t>(), (int)removal, (int)opt_window,
+                                 en, dummy_frame, dummy_patch, (int)M, n_active.data_ptr<int>(), s_ii.data_ptr<int64_t>(), s_jj.data_ptr<int64_t>(),
+                                 s_kk.data_ptr<int64_t>(), s_target.data_ptr<float>(), s_weight.data_ptr<float>(), sc, s_count.data_ptr<int>(),
+                                 s_overflow.data_ptr<int>(), stream()),
+        "dpvo_b200_ext.pgraph_remove_store");
+}
+void loop_flags(Tensor ii, Tensor active, int64_t normal, int64_t n, int64_t removal, c10::optional<Tensor> s_count, Tensor flags) {
+  need_cuda(ii, "ii");
+  c10::cuda::CUDAGuard guard(ii.device());
+  TORCH_CHECK(ii.scalar_type() == at::kLong && ii.is_contiguous() && active.is_cuda() && active.scalar_type() == at::kByte &&
+              active.is_contiguous() && active.numel() == ii.numel(), "loop_flags: ii int64 and active uint8, one entry per slot");
+  TORCH_CHECK(flags.is_cuda() && flags.scalar_type() == at::kLong && flags.is_contiguous() && flags.numel() == 4, "loop_flags: flags is device int64 [4]");
+  const int32_t* sc = nullptr;
+  if (s_count.has_value()) { dev_scalar(*s_count, at::kInt, "loop_flags: the store count is a device int32 scalar"); sc = s_count->data_ptr<int>(); }
+  check(dpvo_loop_flags(ii.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(), normal, n, (int)removal, sc, flags.data_ptr<int64_t>(), stream()),
+        "dpvo_b200_ext.loop_flags");
+}
+void loop_normalize(Tensor poses, Tensor patches, int64_t n, int64_t M) {
+  need_cuda(poses, "poses");
+  c10::cuda::CUDAGuard guard(poses.device());
+  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat && poses.is_contiguous() && patches.is_contiguous() &&
+              patches.is_cuda() && patches.dim() >= 3 && patches.size(-3) == 3, "loop_normalize: contiguous fp32 poses [N, 7] and patches [K, 3, P, P]");
+  const int64_t P = patches.size(-1);
+  TORCH_CHECK(n >= 0 && poses.numel() >= 7 * n && patches.numel() >= n * M * 3 * P * P, "loop_normalize: n = ", n, " frames exceed the buffers");
+  check(dpvo_loop_normalize(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, stream()), "dpvo_b200_ext.loop_normalize");
+}
+
 // ------------------------------------------------------------------------------ frame encoders
 struct EncShape { int ks, s, cin, cout; };
 const EncShape kEncShapes[] = {{7, 2, 3, 32}, {3, 1, 32, 32}, {3, 2, 32, 64}, {1, 2, 32, 64}, {3, 1, 64, 64}, {1, 1, 64, 128}, {1, 1, 64, 384}};
@@ -1056,6 +1155,14 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("pgraph_append", &pgraph_append, "fill parked slots with new edges", py::arg("ii"), py::arg("jj"), py::arg("kk"), py::arg("active"), py::arg("new_ii"),
         py::arg("new_jj"), py::arg("new_kk"), py::arg("enable"), py::arg("state"), py::arg("n_active"), py::arg("overflow"));
   m.def("pgraph_new_edges", &pgraph_new_edges, "steady-state forward + backward edges of the newest frame");
+  m.def("loop_scores", &loop_scores, "loop-candidate flow scores of every (old frame, recent frame) pair");
+  m.def("loop_select", &loop_select, "greedy loop-pair selection and emission of the loop edges", py::arg("scores"), py::arg("n"),
+        py::arg("last_global_ba"), py::arg("M"), py::arg("removal"), py::arg("max_age"), py::arg("freq"), py::arg("kf_index"), py::arg("thresh"),
+        py::arg("pairs"), py::arg("n_pairs"), py::arg("ii"), py::arg("jj"), py::arg("kk"), py::arg("active"), py::arg("state"),
+        py::arg("n_active"), py::arg("overflow"));
+  m.def("pgraph_remove_store", &pgraph_remove_store, "window removal with the loop exception, removed edges kept in the inactive store");
+  m.def("loop_flags", &loop_flags, "loop-edge / long-range flags, minimum active ii and inactive count in one record");
+  m.def("loop_normalize", &loop_normalize, "PatchGraph.normalize on the device");
   m.def("neighbors_from_groups", &neighbors_from_groups, "temporal neighbours from a kk/jj grouping");
   m.def("encoder_conv", &encoder_conv, "one frame-encoder convolution (tensor cores, fused norm / join prologue)", py::arg("shape"),
         py::arg("x"), py::arg("w"), py::arg("bias"), py::arg("x_stats") = py::none(), py::arg("x_relu") = false, py::arg("skip") = py::none(),

@@ -18,17 +18,24 @@ from .streams import StreamBatch
 
 
 class UpdateRunner:
-    def __init__(self, state, update=None, ba_iterations=2, seed=1234, graph=None, encoder=None):
+    def __init__(self, state, update=None, ba_iterations=2, seed=1234, graph=None, encoder=None, loop=None):
         """state: one stream's state (synthetic.SyntheticState layout), or a streams.StreamBatch of B streams that every
         step updates together: one launch per kernel for all of them, bundle adjustment by fastba.BA_batched.
         encoder: optional frontend.FrameEncoder, which `ingest_image` runs.
         graph: optional DevicePatchGraph (patchgraph.py).  With it the edge lists and the recurrent state are the
         store's fixed-capacity arrays: every kernel runs over all `cap` slots, parked slots are dummy edges in groups of
         their own whose confidence weights are zeroed before bundle adjustment, and a captured CUDA graph of step()
-        stays valid while edges are appended and removed between replays.  For a batch: DevicePatchGraph.stacked."""
+        stays valid while edges are appended and removed between replays.  For a batch: DevicePatchGraph.stacked.
+        loop: optional loop.LoopClosure on `graph` (one stream).  While no loop edge is active a step runs over the
+        graph's normal slots only, exactly as without loop closure; while one is, over the normal slots and the used
+        part of the loop region (a captured graph: over the whole store).  Each step then
+        reads one small record from the device to decide this, and runs the global bundle adjustment in place of the
+        local one when an active edge has ii < n - removal - 1 and none ran at this n (dpvo.py:348).  The rings must
+        hold pmem = max_edge_age patch frames (dpvo.py:58-61)."""
         self.s = state
         self.batch = state if isinstance(state, StreamBatch) else None
         self.pg = graph
+        self.loop = loop
         self.encoder = encoder
         dev = state.poses.device
         if update is None:
@@ -70,8 +77,17 @@ class UpdateRunner:
             # frame pair inside the removal window + the dummy pair, per stream
             live = state.cfg["removal"] + 2
             nb = 1 if self.batch is None else self.batch.B
-            self.max_patch_groups = min(graph.cap, nb * (live * self.M + 1))
-            self.max_pair_groups = min(graph.cap, nb * (live * live + 1))
+            self.max_patch_groups = min(graph.normal_cap, nb * (live * self.M + 1))
+            self.max_pair_groups = min(graph.normal_cap, nb * (live * live + 1))
+            if loop is not None:
+                if self.batch is not None or loop.pg is not graph:
+                    raise ValueError("UpdateRunner: loop closure needs one stream and a LoopClosure on this runner's graph")
+                if self.pmem != loop.max_age:
+                    raise ValueError("UpdateRunner: the patch rings hold %d frames; loop closure needs pmem = max_edge_age = %d"
+                                     % (self.pmem, loop.max_age))
+                # with the loop region stepped: up to loop_pairs more pairs and loop_pairs * M more (old) patches
+                self.loop_groups = (min(graph.cap, self.max_patch_groups + graph.loop_pairs * self.M),
+                                    min(graph.cap, self.max_pair_groups + graph.loop_pairs))
             self.kk_ring = self.jj_ring = None                       # the ring indices follow the edges: computed per step
         self.corr_buf = torch.zeros(1, self.E, 896, device=dev, dtype=torch.half)   # padding columns stay zero
 
@@ -81,13 +97,36 @@ class UpdateRunner:
 
     # -------------------------------------------------------------------------------- one update
     @torch.no_grad()
-    def step(self):
+    def step(self, loop_edges=None, loop_record=None):
+        """One update.  With loop closure, loop_edges=None reads the device's loop record (one small D2H; or takes
+        `loop_record`, a LoopClosure.read_flags result the caller read for this frame) and picks the slots and the
+        bundle adjustment from it; True / False fixes the slots (the whole store / the normal ones) without reading
+        anything and runs the local bundle adjustment, as a captured graph does."""
         s = self.s
         ev = self.timers
         poses = s.poses.view(1, -1, 7)
         patches = s.patches.view(1, -1, 3, 3, 3)
         intr = s.intrinsics.view(1, -1, 4)
         ii, jj, kk = self.ii, self.jj, self.kk
+        net, corr_buf, gmax = self.net, self.corr_buf, (self.max_patch_groups, self.max_pair_groups)
+        global_ba = None
+        if self.loop is not None:
+            if loop_edges is None:
+                rec = self.loop.read_flags(s.n) if loop_record is None else loop_record
+                loop_edges, long_range, t0, count = rec
+                if long_range and s.n not in self.loop.ran_global_ba:
+                    global_ba = (t0, count)
+            if loop_edges is True:
+                E = self.pg.cap                                       # the captured form: the whole store
+            elif loop_edges:
+                # eager, from the record: the normal slots and the used part of the loop region only (rounded up to
+                # 128 slots); the parked remainder of the region would only add one large group of dummy edges
+                E = min(self.pg.cap, self.pg.normal_cap + (int(loop_edges) + 127) // 128 * 128)
+            else:
+                E = self.pg.normal_cap
+            ii, jj, kk, net, corr_buf = ii[:E], jj[:E], kk[:E], net[:, :E], corr_buf[:, :E]
+            if loop_edges:
+                gmax = (min(E, self.loop_groups[0]), min(E, self.loop_groups[1]))
         if self.pg is None:
             kk_ring, jj_ring = self.kk_ring, self.jj_ring
         elif self.batch is None:
@@ -97,19 +136,28 @@ class UpdateRunner:
         coords = pops.transform_fused(poses, patches, intr, ii, jj, kk)               # [1,E,2,3,3]
         if ev is not None:
             ev["corr0"].record()
-        corr = altcorr.corr_pyramid(s.gmap, (s.fmap1, s.fmap2), coords, kk_ring, jj_ring, 3, 4.0, 896, self.corr_buf)
+        corr = altcorr.corr_pyramid(s.gmap, (s.fmap1, s.fmap2), coords, kk_ring, jj_ring, 3, 4.0, 896, corr_buf)
         if ev is not None:
             ev["corr1"].record()
-        groups_kk, groups_ij = EdgeGroups.pair((kk, None, jj), (ii, jj, None), self.max_patch_groups, self.max_pair_groups)
+        groups_kk, groups_ij = EdgeGroups.pair((kk, None, jj), (ii, jj, None), gmax[0], gmax[1])
         # context gather (dpvo.py:334) and target = centre + delta (dpvo.py:341) are folded into the
         # first LayerNorm pass and the heads kernel
-        self.net, (target, weight, _) = self.update(self.net, s.imap, corr, None, ii, jj, kk, groups_kk, groups_ij,
-                                                    inp_index=kk_ring, coords=coords)
+        net, (target, weight, _) = self.update(net, s.imap, corr, None, ii, jj, kk, groups_kk, groups_ij,
+                                               inp_index=kk_ring, coords=coords)
+        if self.loop is None:
+            self.net = net
         if self.pg is not None:
-            weight = weight * self.pg.active.view(1, -1, 1)          # parked edges carry no confidence into bundle adjustment
+            weight = weight * self.pg.active[:ii.numel()].view(1, -1, 1)   # parked edges carry no confidence into bundle adjustment
+        if self.loop is not None:
+            # every slot's last target / weight: what LoopClosure.remove keeps and the global bundle adjustment reads
+            self.pg.target[:, :ii.numel()].copy_(target)
+            self.pg.weight[:, :ii.numel()].copy_(weight)
         if ev is not None:
             ev["ba0"].record()
-        if self.batch is None:
+        if global_ba is not None:
+            self.loop.global_ba(s.poses, s.patches, s.intrinsics, s.n, global_ba[0], global_ba[1], ii.numel(), self.lmbda,
+                                self.ba_iterations)
+        elif self.batch is None:
             fastba.BA_grouped(poses, patches, intr, target, weight, self.lmbda, ii, jj, kk, s.t0, s.n,
                               self.ba_iterations, groups_kk, groups_ij)
         else:
@@ -127,19 +175,38 @@ class UpdateRunner:
         private pool, and the recurrent state is updated in place, so replaying the graph IS the next update."""
         if self.timers is not None:
             raise RuntimeError("capture(): event timers cannot be recorded inside a graph")
+        if self.loop is not None:
+            # one graph over the normal slots, one over the whole store; step_graph picks by the loop record
+            self._loop_graphs = {}
+            for mode in (False, True):
+                self._loop_graphs[mode] = (self._capture(lambda: self.step(loop_edges=mode)), self._graph_out)
+            self.graph = self._loop_graphs[False][0]
+            return self.graph
+        return self._capture(self.step)
+
+    def _capture(self, fn):
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                      # warm-up off the capture: lazy inits, attribute calls
             for _ in range(2):
-                self.step()
+                fn()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self._graph_out = self.step()
+            self._graph_out = fn()
         return self.graph
 
     def step_graph(self):
+        if self.loop is not None:
+            # the global bundle adjustment is eager (dense solve); every other frame replays one of the two graphs
+            rec = self.loop.read_flags(self.s.n)
+            loop_edges, long_range, _, _ = rec
+            if long_range and self.s.n not in self.loop.ran_global_ba:
+                return self.step(loop_record=rec)            # the record already read: one D2H for the frame
+            g, out = self._loop_graphs[bool(loop_edges)]
+            g.replay()
+            return out
         self.graph.replay()
         return self._graph_out
 

@@ -151,3 +151,81 @@ def make_batch(config="default", B=2, seeds=None, n_frames=30, device="cuda", fr
         batch.load(b, make_state(cfg, frames[b], device=device, seed=seeds[b], buffer=frames_per_stream, mem=mem))
     batch.set_edges()
     return batch
+
+
+def _look(t, period, radius, dtype=torch.float64):
+    """world -> camera pose of frame t on a closed loop: the camera centre circles (radius) in the x-z plane once per
+    `period` frames while the heading swings by +-0.1 rad, so frame t and t + period see the scene from the same place"""
+    th = 2.0 * math.pi * t / period
+    c = torch.tensor([radius * (math.cos(th) - 1.0), 0.0, radius * math.sin(th)], dtype=dtype)
+    yaw = 0.1 * math.sin(th)
+    q = torch.tensor([0.0, math.sin(0.5 * yaw), 0.0, math.cos(0.5 * yaw)], dtype=dtype)   # camera -> world rotation
+    R = torch.tensor([[math.cos(yaw), 0.0, math.sin(yaw)], [0.0, 1.0, 0.0], [-math.sin(yaw), 0.0, math.cos(yaw)]], dtype=dtype)
+    # world -> camera: R^T (X - c);  as [t, q]: t = -R^T c, q = conj(q)
+    out = torch.zeros(7, dtype=dtype)
+    out[:3] = -(R.T @ c)
+    out[3:6] = -q[:3]
+    out[6] = q[3]
+    return out
+
+
+def make_loop_state(config="fast", n_frames=60, period=20, radius=2.0, noise=1e-3, max_edge_age=1000, buffer=None,
+                    mem=36, device="cuda", seed=1234, features=True, dtype=torch.half):
+    """A stream that drives a closed loop again and again (one lap per `period` frames), for loop closure: the patches
+    of every frame are M points of ONE 3-D scene (points at depth 4..8 in front of the loop) with their true pixel
+    positions and inverse depths, so frame t and frame t + period reproject onto each other and their loop score is
+    close to zero, while frames half a lap apart score tens of pixels.  `noise` jitters every pose's translation so
+    that no two candidate scores tie.  The rings hold `mem` frames of feature maps and pmem = max_edge_age frames of
+    patch features (dpvo.py:58-61); the edge lists are the steady-state window of replay_edges.  buffer (pose slots)
+    defaults to n_frames + 2, the last slot being free for DevicePatchGraph's dummy frame."""
+    cfg = dict(CONFIGS[config]) if isinstance(config, str) else dict(config)
+    cfg["max_edge_age"] = int(max_edge_age)
+    M = cfg["M"]
+    buffer = n_frames + 2 if buffer is None else int(buffer)
+    assert n_frames < buffer
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    h, w = cfg["ht"] // 4, cfg["wd"] // 4
+    fx, fy, cx, cy = [v / 4.0 for v in cfg["intrinsics"]]
+    scene = torch.empty(20000, 3, dtype=torch.float64)
+    scene[:, 0] = (torch.rand(20000, generator=g, dtype=torch.float64) - 0.5) * 16.0 - radius
+    scene[:, 1] = (torch.rand(20000, generator=g, dtype=torch.float64) - 0.5) * 8.0
+    scene[:, 2] = 4.0 + 4.0 * torch.rand(20000, generator=g, dtype=torch.float64) + radius
+    poses = torch.zeros(buffer, 7, dtype=torch.float64)
+    poses[:, 6] = 1.0
+    patches = torch.zeros(buffer * M, 3, 3, 3)
+    offs = torch.tensor([-1.0, 0.0, 1.0])
+    for t in range(n_frames):
+        P = _look(t, period, radius)
+        tq, q = P[:3], P[3:]
+        # rotate the scene into the camera: q_rot(q, X) + t
+        v = q[:3].expand_as(scene)
+        uv = 2.0 * torch.cross(v, scene, dim=1)
+        Xc = scene + q[3] * uv + torch.cross(v, uv, dim=1) + tq
+        u = fx * Xc[:, 0] / Xc[:, 2] + cx
+        vv = fy * Xc[:, 1] / Xc[:, 2] + cy
+        ok = (Xc[:, 2] > 1.0) & (u > 1) & (u < w - 2) & (vv > 1) & (vv < h - 2)
+        idx = torch.nonzero(ok).view(-1)
+        assert idx.numel() >= M, "make_loop_state: too few scene points in view"
+        pick = idx[torch.randperm(idx.numel(), generator=g)[:M]]
+        k = slice(t * M, (t + 1) * M)
+        patches[k, 0] = (u[pick].float()[:, None, None] + offs[None, None, :])
+        patches[k, 1] = (vv[pick].float()[:, None, None] + offs[None, :, None])
+        patches[k, 2] = (1.0 / Xc[pick, 2]).float()[:, None, None]
+        poses[t] = P
+    if noise > 0:
+        poses[:n_frames, :3] += noise * torch.randn(n_frames, 3, generator=g, dtype=torch.float64)
+    intr = torch.tensor([fx, fy, cx, cy]).repeat(buffer, 1)
+    ii, jj, kk = replay_edges(n_frames, M, cfg["lifetime"], cfg["removal"])
+    st = SyntheticState(cfg=cfg, n=n_frames, t0=max(n_frames - cfg["opt_window"], 1), ii=ii.to(device), jj=jj.to(device),
+                        kk=kk.to(device), poses=poses.float().to(device), patches=patches.to(device), intrinsics=intr.to(device))
+    if features:
+        pmem = int(max_edge_age)
+        gd = torch.Generator(device=device).manual_seed(seed + 1)
+        f1 = (torch.randn(1, mem, h, w, 128, generator=gd, device=device) / 4).to(dtype).permute(0, 1, 4, 2, 3)
+        f2 = torch.nn.functional.avg_pool2d(f1[0].float(), 4, 4).to(dtype)[None]
+        st.fmap1 = f1
+        st.fmap2 = f2.permute(0, 1, 3, 4, 2).contiguous().permute(0, 1, 4, 2, 3)
+        st.gmap = (torch.randn(1, pmem * M, 3, 3, 128, generator=gd, device=device) / 4).to(dtype).permute(0, 1, 4, 2, 3)
+        st.imap = (torch.randn(1, pmem * M, 384, generator=gd, device=device) / 4).to(dtype)
+        st.net = torch.zeros(1, st.E, 384, device=device, dtype=dtype)
+    return st

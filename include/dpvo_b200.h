@@ -513,6 +513,52 @@ int dpvo_pgraph_append(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* active, i
                        float* state, int32_t* slot_of_new, int32_t* n_active, int32_t* overflow, void* stream);
 int dpvo_pgraph_new_edges(const int64_t* n_dev, int M, int r, int64_t* ii, int64_t* jj, int64_t* kk, void* stream);
 
+/* ---- Proximity loop closure (dpvo_b200/csrc/loop.cu) ----------------------------------------------------------------
+ * The DPV-SLAM back end of dpvo/patchgraph.py:56-91 and dpvo/dpvo.py:223-326, 449-455 on the fixed-capacity store.
+ * Candidates: targets j in [n - freq, n - kf_index), sources i in [max(l - max_age, 0), l), l = n - removal, laid out
+ * as J = freq - kf_index rows of max_age slots: slot (j - (n - freq)) * max_age + (i - max(l - max_age, 0)).  n and
+ * last_ba are device int64 scalars; a proposal runs only when n - *last_ba >= freq (dpvo.py:449-450).
+ *   dpvo_loop_candidates  J * max_age, the length of `scores` (0 for a bad range)
+ *   dpvo_loop_scores   fp32 [J * max_age]: mean over the valid patches of frame i of the centre-pixel flow
+ *                      0.5 |full - origin| + 0.5 |translation only - origin| (valid: Z > 0.2), if more than 0.75 M are
+ *                      valid; +inf otherwise, for a slot outside the range and for every slot when no proposal is due.
+ *                      A fixed-order reduction: two launches give identical bits.
+ *   dpvo_loop_select   reduce_edges (loop_closure/optim_utils.py:23-61): slots with score < thresh in ascending
+ *                      (score, slot), skip j - i < 30 and suppressed pairs, accept and suppress (i +- 1, j), at most
+ *                      max_pairs.  pairs int64 [max_pairs, 2] = (i, j) in acceptance order, *n_pairs their count (0 when no
+ *                      proposal ran); *last_ba = n when one was accepted.  The M edges of accepted pair p go to slots
+ *                      p M + m of the loop region (ii, jj, kk, active, state: its first `region` slots), state rows zeroed;
+ *                      *n_active counts the new edges, *overflow is set if a slot still held an active edge.
+ *                      (freq - kf_index) * max_age > 16384 is DPVO_ERR_UNSUPPORTED.
+ *   dpvo_pgraph_remove_store  the third removal rule: park the active edges with
+ *                      kk / M < n - removal && !((jj - ii) > 30 && jj > n - opt_window)   (dpvo.py:300-310)
+ *                      and keep each one's (ii, jj, kk, target [2], weight [2]) in the inactive store (capacity s_cap,
+ *                      fp32 target / weight [cap, 2]).  The store fills from its end: the edges of one call are placed in
+ *                      slot order below those of the previous calls, so the used part is [s_cap - *s_count, s_cap).  Edges
+ *                      beyond the capacity are dropped and *s_overflow is set.
+ *   dpvo_loop_flags    flags int64 [4]: 1 + the offset of the last active edge in slots [normal, cap) (0 without one);
+ *                      1 if an active edge has ii < n - removal - 1
+ *                      (dpvo.py:348); the minimum active ii (INT64_MAX without one); *s_count (0 if s_count is NULL)
+ *   dpvo_loop_normalize  PatchGraph.normalize (patchgraph.py:84-91) for frames [0, n): depths / mean depth, translations
+ *                      * mean depth, every pose rebased on pose 0.  patches fp32 [>= n M, 3, P, P], poses fp32 [>= n, 7]
+ */
+int64_t dpvo_loop_candidates(int max_age, int freq, int kf_index);
+int dpvo_loop_scores(const float* poses, const float* patches, const float* intrinsics, const int64_t* n_dev,
+                     const int64_t* last_ba, int M, int removal, int max_age, int freq, int kf_index,
+                     float* scores, void* stream);
+int dpvo_loop_select(const float* scores, const int64_t* n_dev, int64_t* last_ba, int M, int removal, int max_age,
+                     int freq, int kf_index, float thresh, int max_pairs, int64_t* pairs, int32_t* n_pairs,
+                     int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* active, int64_t region, float* state,
+                     int32_t* n_active, int32_t* overflow, void* stream);
+int dpvo_pgraph_remove_store(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* active, const float* target,
+                             const float* weight, int64_t cap, const int64_t* n_dev, int removal, int opt_window,
+                             const int32_t* enable, int64_t dummy_frame, int64_t dummy_patch, int M,
+                             int32_t* n_active, int64_t* s_ii, int64_t* s_jj, int64_t* s_kk, float* s_target,
+                             float* s_weight, int64_t s_cap, int32_t* s_count, int32_t* s_overflow, void* stream);
+int dpvo_loop_flags(const int64_t* ii, const uint8_t* active, int64_t cap, int64_t normal, int64_t n, int removal,
+                    const int32_t* s_count, int64_t* flags, void* stream);
+int dpvo_loop_normalize(float* poses, float* patches, int64_t n, int M, int P, void* stream);
+
 /* ---- Frame encoders (dpvo_b200/csrc/encoder.cu) ---------------------------------------------------------------------
  * BasicEncoder4 (extractor.py:200-264) as used by Patchifier (net.py:95-157) for inference: fnet (instance norm after
  * every convolution but the last, output 128) and inet (no norm, output 384).  Activations are NHWC fp16, convolutions
