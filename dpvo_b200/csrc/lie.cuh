@@ -2,7 +2,10 @@
 // Semantics follow dpvo/lietorch/include/so3.h:31-220 and se3.h:36-217:
 //   * element layout SO3 [qx qy qz qw], SE3 [tx ty tz qx qy qz qw]
 //   * quaternions are normalised whenever a group element is constructed (so3.h:31-37)
-//   * Taylor switches at theta < EPS = 1e-6 (common.h:7)
+//   * so3_exp / so3_log switch to their series at theta < EPS = 1e-6 (common.h:7); their closed forms sin(t/2)/t and
+//     atan(n/w)/n do not cancel, so the switch only keeps 0/0 away and serves float and double alike
+//   * the Jacobian coefficients do cancel at small angles, and are evaluated differently from the reference; see
+//     "Jacobian coefficients" below
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -142,20 +145,76 @@ template <typename S> LIE_HD Quat<S> so3_exp(V3<S> phi) {
   }
   return q_normalized<S>(im * phi.x, im * phi.y, im * phi.z, re);
 }
+// ---- Jacobian coefficients ---------------------------------------------------------------------------------------
+// lietorch's closed forms, e.g. (t - sin t) / t^3, lose about ulp / t^2 relative to the coefficient as t -> 0 (ulp / t^4
+// for the Q coefficients), and switched to two-term series only below t = 1e-6 for both float and double: at t = 1e-4 the
+// float J and Q were wrong in the 4th digit, the double ones in the 10th.  Here every coefficient is within a few ulp of
+// S over the whole range:
+//   * (1 - cos t) / t^2 = 2 (sin(t/2) / t)^2 everywhere -- no cancellation; sin(t/2) / t is so3_exp's coefficient;
+//   * (t - sin t) / t^3, (t^2/2 - (1 - cos t)) / t^4 and lietorch's J^-1 coefficient (1 - t cos(t/2) / (2 sin(t/2))) / t^2
+//     by their Taylor series below t = 1, where the closed forms above lose at most ~24 ulp;
+//   * Q's third coefficient (2t - 3 sin t + t cos t) / (2 t^5) by its series below t = 2, where its closed form, written
+//     (3 c_B - c_A) / (2 t^2) over the two J coefficients, loses at most ~15 ulp.
+// The switches depend on the cancellation, not on S; the number of terms is per type (SeriesTerms), each series cut
+// where its first dropped term is below half an ulp of S at the switch.
+template <typename S> struct SeriesTerms;
+template <> struct SeriesTerms<float> { static constexpr int sin3 = 5, cos4 = 4, jinv = 5, q3 = 6; };
+template <> struct SeriesTerms<double> { static constexpr int sin3 = 8, cos4 = 8, jinv = 10, q3 = 10; };
+
+// sum_k c[k] x^k over the first n coefficients, Horner
+template <int n, typename S, int M> LIE_HD S series(const double (&c)[M], S x) {
+  static_assert(n <= M, "not enough coefficients");
+  S p = S(c[n - 1]);
+#pragma unroll
+  for (int k = n - 2; k >= 0; --k) p = p * x + S(c[k]);
+  return p;
+}
+// sin(t/2) / t, as in so3_exp
+template <typename S> LIE_HD S sinc_half(S th, S t2) {
+  return (th < S(kEps)) ? S(0.5) - S(1.0 / 48.0) * t2 + S(1.0 / 3840.0) * t2 * t2 : sin(S(0.5) * th) / th;
+}
+// (1 - cos t) / t^2
+template <typename S> LIE_HD S coef_cos2(S th, S t2) { const S h = sinc_half(th, t2); return S(2) * h * h; }
+// (t - sin t) / t^3 = sum_k (-1)^k t^2k / (2k+3)!
+template <typename S> LIE_HD S coef_sin3(S th, S t2) {
+  constexpr double c[] = {0.16666666666666666, -0.008333333333333333, 0.0001984126984126984, -2.7557319223985893e-06,
+                          2.505210838544172e-08, -1.6059043836821613e-10, 7.647163731819816e-13, -2.8114572543455206e-15};
+  return (th < S(1)) ? series<SeriesTerms<S>::sin3>(c, t2) : (th - sin(th)) / (t2 * th);
+}
+// (t^2/2 - (1 - cos t)) / t^4 = sum_k (-1)^k t^2k / (2k+4)!
+template <typename S> LIE_HD S coef_cos4(S th, S t2) {
+  constexpr double c[] = {0.041666666666666664, -0.001388888888888889, 2.48015873015873e-05, -2.755731922398589e-07,
+                          2.08767569878681e-09, -1.1470745597729725e-11, 4.779477332387385e-14, -1.5619206968586225e-16};
+  return (th < S(1)) ? series<SeriesTerms<S>::cos4>(c, t2) : (S(0.5) - coef_cos2(th, t2)) / t2;
+}
+// (1 - t cos(t/2) / (2 sin(t/2))) / t^2 = sum_{n>=1} |B_2n| t^(2n-2) / (2n)!
+template <typename S> LIE_HD S coef_jinv(S th, S t2) {
+  constexpr double c[] = {0.08333333333333333, 0.001388888888888889, 3.306878306878307e-05, 8.267195767195768e-07,
+                          2.08767569878681e-08, 5.284190138687493e-10, 1.3382536530684679e-11, 3.3896802963225827e-13,
+                          8.586062056277845e-15, 2.174868698558062e-16};
+  if (th < S(1)) return series<SeriesTerms<S>::jinv>(c, t2);
+  const S ht = S(0.5) * th;
+  return (S(1) - th * cos(ht) / (S(2) * sin(ht))) / t2;
+}
+// (2t - 3 sin t + t cos t) / (2 t^5) = sum_k (-1)^k (k+1) t^2k / (2k+5)!
+template <typename S> LIE_HD S coef_q3(S th, S t2) {
+  constexpr double c[] = {0.008333333333333333, -0.0003968253968253968, 8.267195767195768e-06, -1.0020843354176688e-07,
+                          8.029521918410807e-10, -4.58829823909189e-12, 1.9680200780418645e-14, -6.576508197299464e-17,
+                          1.7615646957052136e-19, -3.868170170630684e-22};
+  return (th < S(2)) ? series<SeriesTerms<S>::q3>(c, t2) : (S(3) * coef_sin3(th, t2) - coef_cos2(th, t2)) / (S(2) * t2);
+}
+
 // so3.h:178-197
 template <typename S> LIE_HD M3<S> so3_left_jacobian(V3<S> phi) {
   const M3<S> Phi = hat(phi), Phi2 = Phi * Phi;
   const S t2 = dot(phi, phi), th = sqrt(t2);
-  const S c1 = ((double)th < kEps) ? S(0.5) - S(1.0 / 24.0) * t2 : (S(1) - cos(th)) / t2;
-  const S c2 = ((double)th < kEps) ? S(1.0 / 6.0) - S(1.0 / 120.0) * t2 : (th - sin(th)) / (t2 * th);
-  return m3_identity<S>() + c1 * Phi + c2 * Phi2;
+  return m3_identity<S>() + coef_cos2(th, t2) * Phi + coef_sin3(th, t2) * Phi2;
 }
 // so3.h:199-215
 template <typename S> LIE_HD M3<S> so3_left_jacobian_inverse(V3<S> phi) {
   const M3<S> Phi = hat(phi), Phi2 = Phi * Phi;
-  const S t2 = dot(phi, phi), th = sqrt(t2), ht = S(0.5) * th;
-  const S c2 = ((double)th < kEps) ? S(1.0 / 12.0) : (S(1) - th * cos(ht) / (S(2) * sin(ht))) / (th * th);
-  return m3_identity<S>() + S(-0.5) * Phi + c2 * Phi2;
+  const S t2 = dot(phi, phi), th = sqrt(t2);
+  return m3_identity<S>() + S(-0.5) * Phi + coef_jinv(th, t2) * Phi2;
 }
 // so3.h:83-93: 4x4 orthogonal projector, row major
 template <typename S> LIE_HD void so3_projector(const Quat<S>& q, S (&J)[4][4]) {
@@ -208,12 +267,8 @@ template <typename S> LIE_HD Tan6<S> row_times_adj(const Tan6<S>& g, const Tan6<
 // se3.h:147-176
 template <typename S> LIE_HD M3<S> se3_calcQ(const Tan6<S>& a) {
   const M3<S> Tau = hat(a.tau), Phi = hat(a.phi);
-  const S th = sqrt(dot(a.phi, a.phi)), t2 = th * th, t4 = t2 * t2;
-  const bool small = (double)th < kEps;
-  const S c1 = small ? S(1.0 / 6.0) - S(1.0 / 120.0) * t2 : (th - sin(th)) / (t2 * th);
-  const S c2 = small ? S(1.0 / 24.0) - S(1.0 / 720.0) * t2 : (t2 + S(2) * cos(th) - S(2)) / (S(2) * t4);
-  const S c3 = small ? S(1.0 / 120.0) - S(1.0 / 2520.0) * t2
-                     : (S(2) * th - S(3) * sin(th) + th * cos(th)) / (S(2) * t4 * th);
+  const S t2 = dot(a.phi, a.phi), th = sqrt(t2);
+  const S c1 = coef_sin3(th, t2), c2 = coef_cos4(th, t2), c3 = coef_q3(th, t2);
   const M3<S> PT = Phi * Tau, TP = Tau * Phi, PTP = PT * Phi;
   return S(0.5) * Tau + c1 * (PT + TP + PTP) + c2 * (Phi * PT + TP * Phi - S(3) * PTP) +
          c3 * (PTP * Phi + Phi * PTP);

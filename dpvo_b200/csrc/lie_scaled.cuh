@@ -2,9 +2,9 @@
 // Semantics follow dpvo/lietorch/include/rxso3.h:11-324 and sim3.h:12-217:
 //   * layouts RxSO3 [qx qy qz qw s], tangent [phi, sigma]; Sim3 [tx ty tz qx qy qz qw s], tangent [tau, phi, sigma]
 //   * the quaternion is normalised on every load, the scale is taken as stored
-//   * W(phi, sigma) with its four small-angle / small-scale branches (rxso3.h:189-234); Sim3::Log uses a
-//     general inverse of W (sim3.h:151-158); Sim3's left Jacobian is the series the reference evaluates,
-//     i.e. truncated after the Xi^4/120 term (the 1/720 line is dead code behind a semicolon, sim3.h:169-180)
+//   * W(phi, sigma) as in rxso3.h:189-234, evaluated without its cancellation at small angles and scales (see
+//     rxso3_calcW); Sim3::Log uses a general inverse of W (sim3.h:151-158); Sim3's left Jacobian is the series the
+//     reference evaluates, i.e. truncated after the Xi^4/120 term (the 1/720 line is dead code behind a semicolon, sim3.h:169-180)
 // These two groups are not on the DPVO hot path (loop closure only), so the operators are written once, generically,
 // over small dense matrices: every backward operator of lietorch_gpu.cu:32-294 is a row vector times the group's
 // left Jacobian / adjoint / action Jacobian.  Everything is __host__ __device__: tests/test_lie_scaled_host_cpu.py
@@ -61,25 +61,42 @@ template <typename S> LIE_HD M3<S> m3_inverse(const M3<S>& a) {
   return r;
 }
 
-// W(phi, sigma) = A hat(phi) + B hat(phi)^2 + C I      rxso3.h:189-234
+// W(phi, sigma) = A hat(phi) + B hat(phi)^2 + C I = sum_k (hat(phi) + sigma I)^k / (k+1)!      rxso3.h:189-234
+// The reference's closed forms cancel as sigma and theta go to 0 (e.g. C = (e^sigma - 1) / sigma lost ulp / sigma, 1e-3
+// relative in float at sigma = 1e-5) and switched to their limits only below 1e-6.  Here, with z = sigma + i theta:
+//   * |z| < 1: the double series A = sum b_k / (k+1)!, B = sum c_k / (k+1)!, C = sum sigma^k / (k+1)!, where
+//     z^k = a_k + i theta b_k and c_k = (sigma^k - a_k) / theta^2 follow a_{k+1} = sigma a_k - theta^2 b_k,
+//     b_{k+1} = a_k + sigma b_k, c_{k+1} = sigma c_k + b_k -- polynomials, no division, no cancellation.  WSeriesTerms<S>
+//     terms make the first dropped one (< k^2 / (2 (k+1)!)) smaller than half an ulp of S at |z| = 1;
+//   * |z| >= 1: C = expm1(sigma) / sigma (1 at sigma = 0) and the closed forms, which have no cancellation there, except
+//     that B loses ~ulp / theta^2 as theta -> 0 at |sigma| >= 1 -- harmless for W, where B multiplies hat(phi)^2 of norm
+//     theta^2 -- and, below theta = sqrt(ulp) (WSeriesTerms<S>::theta_limit), the theta -> 0 limits, whose truncation is below an ulp.
+template <typename S> struct WSeriesTerms;
+template <> struct WSeriesTerms<float> { static constexpr int n = 13; static constexpr double theta_limit = 2.5e-4; };
+template <> struct WSeriesTerms<double> { static constexpr int n = 20; static constexpr double theta_limit = 1e-8; };
+
 template <typename S> LIE_HD M3<S> rxso3_calcW(V3<S> phi, S sigma) {
-  const S th = sqrt(dot(phi, phi));
+  const S t2 = dot(phi, phi), th = sqrt(t2);
   const M3<S> Phi = hat(phi), Phi2 = Phi * Phi;
-  const S sc = exp(sigma);
-  const bool s_small = fabs((double)sigma) < kEps, t_small = fabs((double)th) < kEps;
   S A, B, C;
-  if (s_small) {
-    C = S(1);
-    if (t_small) { A = S(0.5); B = S(1.0 / 6.0); }
-    else { const S t2 = th * th; A = (S(1) - cos(th)) / t2; B = (th - sin(th)) / (t2 * th); }
+  if (sigma * sigma + t2 < S(1)) {
+    S a = S(1), b = S(0), c = S(0), sk = S(1), f = S(1);     // k = 0; f = 1 / (k+1)!
+    A = S(0); B = S(0); C = S(0);
+#pragma unroll 1
+    for (int k = 0; k < WSeriesTerms<S>::n; ++k) {
+      C += sk * f; A += b * f; B += c * f;
+      const S an = sigma * a - t2 * b, bn = a + sigma * b, cn = sigma * c + b;
+      a = an; b = bn; c = cn; sk *= sigma; f /= S(k + 2);
+    }
   } else {
-    C = (sc - S(1)) / sigma;
-    if (t_small) {
+    const S sc = exp(sigma);
+    C = (sigma == S(0)) ? S(1) : expm1(sigma) / sigma;
+    if (th < S(WSeriesTerms<S>::theta_limit)) {                // |sigma| >= 1 here
       const S s2 = sigma * sigma;
       A = ((sigma - S(1)) * sc + S(1)) / s2;
       B = (sc * S(0.5) * s2 + sc - S(1) - sigma * sc) / (s2 * sigma);
     } else {
-      const S t2 = th * th, a = sc * sin(th), b = sc * cos(th), c = t2 + sigma * sigma;
+      const S a = sc * sin(th), b = sc * cos(th), c = t2 + sigma * sigma;
       A = (a * sigma + (S(1) - b) * th) / (th * c);
       B = (C - ((b - S(1)) * sigma + a * th) / c) / t2;
     }

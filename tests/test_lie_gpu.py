@@ -28,8 +28,10 @@ def _rand(gid, n, dtype, seed):
 def test_forward_and_backward_ops(ext, gid, dtype, tol):
     L = ext[2]
     G = OL.GROUPS[gid]
-    if gid in (2, 4):         # generic small-matrix operators, sums in another order than the oracle's
-        tol = 1e-10 if dtype == torch.float64 else 5e-4
+    if gid in (2, 4) and dtype == torch.float64:
+        # the oracle keeps lietorch's closed forms for W(phi, sigma), which lose ~ulp / |sigma| in double at small random
+        # sigma; tests/test_lie_edges_gpu.py holds these kernels to 1e-12 against the cancellation-free reference
+        tol = 1e-10
     n = 1000
     a, X, Y, p3, p4 = _rand(gid, n, dtype, 11)
     ad, Xd, Yd, p3d, p4d = [t.to(DEV) for t in (a, X, Y, p3, p4)]

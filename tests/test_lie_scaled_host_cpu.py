@@ -74,6 +74,6 @@ def test_scaled_groups_on_host_match_the_oracle(exe, tmp_path, gid, dtype):
             got = torch.from_numpy(raw[off:off + n * w].astype(np.float64)).reshape(n, w)
             off += n * w
             scale = max(1.0, r.abs().max().item())
-            tol = 1e-10 if dtype == "f64" else 2e-4
+            tol = 1e-12 if dtype == "f64" else 2e-5
             err = (got - r).abs().max().item()
             assert err <= tol * scale, (op, dtype, err)
