@@ -11,7 +11,7 @@
 // The frame counter is a device scalar in every call but normalize (the global bundle adjustment around it is eager),
 // and the grids are sized for the largest candidate range, so a frame's proposal, removal and flags can be captured.
 #include "common.cuh"
-#include "lie.cuh"
+#include "flow.cuh"
 
 namespace dpvo {
 
@@ -39,34 +39,10 @@ __device__ __forceinline__ bool loop_due(int64_t n, const int64_t* last_ba, int 
   return n - *last_ba >= freq;
 }
 
-// flow of the centre pixel of patch k from frame i to frame j: 0.5 |full - origin| + 0.5 |translation only - origin|,
-// valid when the fully transformed point has Z > 0.2 (projective_ops.py:111, 120-130, beta = 0.5)
+// flow of the centre pixel of patch k from frame i to frame j (flow.cuh)
 __device__ __forceinline__ float centre_flow(const float* __restrict__ poses, const float* __restrict__ patches,
                                              const float* __restrict__ intr, int64_t i, int64_t j, int64_t k, bool& valid) {
-  using namespace lie;
-  const float* pk = patches + k * 27;
-  const float x = pk[4], y = pk[9 + 4], d = pk[18 + 4];
-  const float fxi = intr[4 * i], fyi = intr[4 * i + 1], cxi = intr[4 * i + 2], cyi = intr[4 * i + 3];
-  const float fxj = intr[4 * j], fyj = intr[4 * j + 1], cxj = intr[4 * j + 2], cyj = intr[4 * j + 3];
-  const V3<float> p = v3<float>((x - cxi) / fxi, (y - cyi) / fyi, 1.f);
-  const SE3<float> Pi = se3_load(poses + 7 * i), Pj = se3_load(poses + 7 * j);
-  const SE3<float> Pii = se3_inv(Pi);
-  // origin: the patch reprojected into its own frame
-  const SE3<float> Gii = se3_mul(Pi, Pii);
-  const V3<float> X0 = q_rot(Gii.q, p) + d * Gii.t;
-  const float d0 = 1.f / fmaxf(X0.z, 0.1f);
-  const float u0 = fxi * (d0 * X0.x) + cxi, v0 = fyi * (d0 * X0.y) + cyi;
-  const SE3<float> Gij = se3_mul(Pj, Pii);
-  const V3<float> X1 = q_rot(Gij.q, p) + d * Gij.t;
-  const float d1 = 1.f / fmaxf(X1.z, 0.1f);
-  const float u1 = fxj * (d1 * X1.x) + cxj, v1 = fyj * (d1 * X1.y) + cyj;
-  const V3<float> X2 = p + d * Gij.t;
-  const float d2 = 1.f / fmaxf(X2.z, 0.1f);
-  const float u2 = fxj * (d2 * X2.x) + cxj, v2 = fyj * (d2 * X2.y) + cyj;
-  valid = X1.z > 0.2f;
-  const float f1 = sqrtf((u1 - u0) * (u1 - u0) + (v1 - v0) * (v1 - v0));
-  const float f2 = sqrtf((u2 - u0) * (u2 - u0) + (v2 - v0) * (v2 - v0));
-  return 0.5f * f1 + 0.5f * f2;
+  return patch_flow(poses, patches, intr, i, j, k, 4, valid);
 }
 
 // one warp per candidate slot; lane l sums patches l, l + 32, ... in order, then a fixed butterfly: two launches give
@@ -283,9 +259,10 @@ loop_flags_kernel(const int64_t* ii, const uint8_t* active, int64_t cap, int64_t
 }
 
 // PatchGraph.normalize (patchgraph.py:84-91): s = mean of every depth value of patches[:n] (fp64, a fixed order:
-// two launches give the same bits), depths /= s, translations *= s, then every pose is rebased on pose 0
+// two launches give the same bits), depths /= s, translations *= s, the translations of the n_delta relative poses of
+// a keyframe delta table (keyframe.cu) *= s, then every pose is rebased on pose 0
 __global__ void __launch_bounds__(LOOP_THREADS)
-loop_normalize_kernel(float* poses, float* patches, int64_t n, int M, int P) {
+loop_normalize_kernel(float* poses, float* patches, int64_t n, int M, int P, float* delta, int64_t n_delta) {
   __shared__ double red[LOOP_THREADS / 32];
   __shared__ float s_sh;
   __shared__ float p0[7];
@@ -311,6 +288,7 @@ loop_normalize_kernel(float* poses, float* patches, int64_t n, int M, int P) {
     const int64_t k = t / PP;
     patches[(k * 3 + 2) * PP + (t - k * PP)] /= s;
   }
+  for (int64_t t = threadIdx.x; t < 3 * n_delta; t += LOOP_THREADS) delta[7 * (t / 3) + t % 3] *= s;   // dP.scale(s)
   using namespace lie;
   const SE3<float> P0inv = se3_inv(se3_load(p0));
   for (int64_t t = threadIdx.x; t < n; t += LOOP_THREADS) {
@@ -419,11 +397,17 @@ extern "C" int dpvo_loop_flags(const int64_t* ii, const uint8_t* active, int64_t
   return DPVO_OK;
 }
 
-extern "C" int dpvo_loop_normalize(float* poses, float* patches, int64_t n, int M, int P, void* stream) {
-  DPVO_REQUIRE(n >= 0 && M > 0 && P > 0, "loop_normalize: bad sizes (n=%lld, M=%d, P=%d)", (long long)n, M, P);
+extern "C" int dpvo_loop_normalize_deltas(float* poses, float* patches, int64_t n, int M, int P, float* delta, int64_t n_delta,
+                                          void* stream) {
+  DPVO_REQUIRE(n >= 0 && M > 0 && P > 0 && n_delta >= 0, "loop_normalize: bad sizes (n=%lld, M=%d, P=%d, deltas=%lld)", (long long)n, M,
+               P, (long long)n_delta);
   if (n == 0) return DPVO_OK;
-  DPVO_REQUIRE(poses && patches, "loop_normalize: null pointer");
-  loop_normalize_kernel<<<1, LOOP_THREADS, 0, (cudaStream_t)stream>>>(poses, patches, n, M, P);
+  DPVO_REQUIRE(poses && patches && (delta || n_delta == 0), "loop_normalize: null pointer");
+  loop_normalize_kernel<<<1, LOOP_THREADS, 0, (cudaStream_t)stream>>>(poses, patches, n, M, P, delta, n_delta);
   DPVO_LAUNCH_CHECK("loop_normalize_kernel");
   return DPVO_OK;
+}
+
+extern "C" int dpvo_loop_normalize(float* poses, float* patches, int64_t n, int M, int P, void* stream) {
+  return dpvo_loop_normalize_deltas(poses, patches, n, M, P, nullptr, 0, stream);
 }

@@ -12,6 +12,7 @@
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
+#include <algorithm>
 #include <vector>
 
 #include "../../include/dpvo_b200.h"
@@ -915,14 +916,129 @@ void loop_flags(Tensor ii, Tensor active, int64_t normal, int64_t n, int64_t rem
   check(dpvo_loop_flags(ii.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(), normal, n, (int)removal, sc, flags.data_ptr<int64_t>(), stream()),
         "dpvo_b200_ext.loop_flags");
 }
-void loop_normalize(Tensor poses, Tensor patches, int64_t n, int64_t M) {
+void loop_normalize(Tensor poses, Tensor patches, int64_t n, int64_t M, c10::optional<Tensor> delta) {
   need_cuda(poses, "poses");
   c10::cuda::CUDAGuard guard(poses.device());
   TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat && poses.is_contiguous() && patches.is_contiguous() &&
               patches.is_cuda() && patches.dim() >= 3 && patches.size(-3) == 3, "loop_normalize: contiguous fp32 poses [N, 7] and patches [K, 3, P, P]");
   const int64_t P = patches.size(-1);
   TORCH_CHECK(n >= 0 && poses.numel() >= 7 * n && patches.numel() >= n * M * 3 * P * P, "loop_normalize: n = ", n, " frames exceed the buffers");
-  check(dpvo_loop_normalize(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, stream()), "dpvo_b200_ext.loop_normalize");
+  if (!delta.has_value()) {
+    check(dpvo_loop_normalize(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, stream()), "dpvo_b200_ext.loop_normalize");
+    return;
+  }
+  TORCH_CHECK(delta->is_cuda() && delta->scalar_type() == at::kFloat && delta->is_contiguous() && delta->numel() % 7 == 0,
+              "loop_normalize: delta is a contiguous fp32 [T, 7] table of relative poses");
+  check(dpvo_loop_normalize_deltas(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, delta->data_ptr<float>(),
+                                   delta->numel() / 7, stream()),
+        "dpvo_b200_ext.loop_normalize");
+}
+
+// ---- keyframe culling (include/dpvo_b200.h, csrc/keyframe.cu)
+static void i64_rows(const Tensor& t, int64_t n, const char* what) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kLong && t.is_contiguous() && t.numel() == n, what);
+}
+void keyframe_motion(Tensor poses, Tensor patches, Tensor intrinsics, int64_t F, Tensor ii, Tensor jj, Tensor kk, Tensor active,
+                     Tensor n, Tensor tstamp, Tensor delta, Tensor delta_src, int64_t ki, double thresh, Tensor flag, Tensor k, Tensor m,
+                     Tensor overflow) {
+  need_cuda(poses, "poses");
+  c10::cuda::CUDAGuard guard(poses.device());
+  const int64_t B = n.numel();
+  TORCH_CHECK(B >= 1 && F >= 2, "keyframe_motion: one frame count per stream and at least 2 frame slots");
+  f32_rows(poses, B * F, 7, "keyframe_motion: poses are contiguous fp32 [B F, 7]");
+  f32_rows(intrinsics, B * F, 4, "keyframe_motion: intrinsics are contiguous fp32 [B F, 4]");
+  TORCH_CHECK(patches.is_cuda() && patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() % (B * F * 27) == 0 &&
+              patches.size(-1) == 3, "keyframe_motion: patches are contiguous fp32 [B F M, 3, 3, 3]");
+  pg_check(ii, jj, kk, active);
+  TORCH_CHECK(ii.is_cuda() && ii.numel() % B == 0, "keyframe_motion: the edge store holds one slice of slots per stream");
+  i64_rows(n, B, "keyframe_motion: n is a device int64 [B]");
+  i64_rows(tstamp, B * F, "keyframe_motion: tstamp is a contiguous device int64 [B, F]");
+  TORCH_CHECK(delta_src.is_cuda() && delta_src.scalar_type() == at::kLong && delta_src.is_contiguous() && delta_src.numel() % B == 0,
+              "keyframe_motion: delta_src is a contiguous device int64 [B, T]");
+  const int64_t T = delta_src.numel() / B;
+  f32_rows(delta, B * T, 7, "keyframe_motion: delta is a contiguous fp32 [B, T, 7]");
+  TORCH_CHECK(flag.is_cuda() && flag.scalar_type() == at::kInt && flag.is_contiguous() && flag.numel() == B, "keyframe_motion: flag is a device int32 [B]");
+  TORCH_CHECK(overflow.is_cuda() && overflow.scalar_type() == at::kInt && overflow.is_contiguous() && overflow.numel() == B,
+              "keyframe_motion: overflow is a device int32 [B]");
+  i64_rows(k, B, "keyframe_motion: k is a device int64 [B]");
+  TORCH_CHECK(m.is_cuda() && m.scalar_type() == at::kDouble && m.is_contiguous() && m.numel() == B, "keyframe_motion: m is a device fp64 [B]");
+  const int64_t wsb = dpvo_keyframe_motion_workspace_bytes((int)B);
+  Tensor ws = torch::empty({wsb}, poses.options().dtype(at::kByte));
+  check(dpvo_keyframe_motion(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(), F, (int)B,
+                             ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel() / B,
+                             n.data_ptr<int64_t>(), tstamp.data_ptr<int64_t>(), delta.data_ptr<float>(), delta_src.data_ptr<int64_t>(), T, (int)ki,
+                             thresh, flag.data_ptr<int>(), k.data_ptr<int64_t>(), m.data_ptr<double>(), overflow.data_ptr<int>(), ws.data_ptr(),
+                             wsb, stream()),
+        "dpvo_b200_ext.keyframe_motion");
+}
+// each buffer is a dense tensor whose outermost dimension in memory holds B * rows slots of equal size, in order
+void keyframe_shift(std::vector<Tensor> bufs, std::vector<int64_t> rows, int64_t F, int64_t ki, Tensor flag, Tensor k) {
+  need_cuda(flag, "flag");
+  c10::cuda::CUDAGuard guard(flag.device());
+  const int64_t B = flag.numel();
+  TORCH_CHECK(flag.scalar_type() == at::kInt && flag.is_contiguous() && B >= 1, "keyframe_shift: flag is a device int32 [B]");
+  i64_rows(k, B, "keyframe_shift: k is a device int64 [B]");
+  TORCH_CHECK(bufs.size() == rows.size(), "keyframe_shift: one slot count per buffer");
+  std::vector<void*> bases;
+  std::vector<int64_t> rb, rw;
+  for (size_t q = 0; q < bufs.size(); ++q) {
+    const Tensor& t = bufs[q];
+    TORCH_CHECK(t.is_cuda() && t.device() == flag.device() && t.numel() > 0 && t.is_non_overlapping_and_dense(),
+                "keyframe_shift: buffer ", q, " must be a dense CUDA tensor on the flag's device");
+    // dense: the memory order is row-major over the dimensions sorted by stride, so the slots are contiguous blocks
+    // when the leading dimensions of that order hold a multiple of B * rows blocks
+    std::vector<int> dims;
+    for (int i = 0; i < t.dim(); ++i) if (t.size(i) > 1) dims.push_back(i);
+    std::stable_sort(dims.begin(), dims.end(), [&](int a, int b) { return t.stride(a) > t.stride(b); });
+    bool ok = false;
+    int64_t lead = 1;
+    for (int d : dims) { lead *= t.size(d); if (rows[q] > 0 && lead % (B * rows[q]) == 0) { ok = true; break; } }
+    TORCH_CHECK(ok, "keyframe_shift: buffer ", q, " does not hold ", B, " x ", rows[q], " slots in its leading dimensions");
+    bases.push_back(t.data_ptr());
+    rb.push_back(t.numel() * (int64_t)t.element_size() / (B * rows[q]));
+    rw.push_back(rows[q]);
+  }
+  check(dpvo_keyframe_shift(bases.data(), rb.data(), rw.data(), (int)bases.size(), F, (int)B, (int)ki, flag.data_ptr<int>(),
+                            k.data_ptr<int64_t>(), stream()),
+        "dpvo_b200_ext.keyframe_shift");
+}
+void keyframe_count(int64_t mode, Tensor n, Tensor tstamp, int64_t F, Tensor counter, Tensor delta, Tensor delta_src, Tensor overflow) {
+  need_cuda(counter, "counter");
+  c10::cuda::CUDAGuard guard(counter.device());
+  const int64_t B = counter.numel();
+  i64_rows(counter, B, "keyframe_count: counter is a device int64 [B]");
+  i64_rows(n, B, "keyframe_count: n is a device int64 [B]");
+  i64_rows(tstamp, B * F, "keyframe_count: tstamp is a contiguous device int64 [B, F]");
+  TORCH_CHECK(delta_src.is_cuda() && delta_src.scalar_type() == at::kLong && delta_src.is_contiguous() && delta_src.numel() % B == 0,
+              "keyframe_count: delta_src is a contiguous device int64 [B, T]");
+  const int64_t T = delta_src.numel() / B;
+  f32_rows(delta, B * T, 7, "keyframe_count: delta is a contiguous fp32 [B, T, 7]");
+  TORCH_CHECK(overflow.is_cuda() && overflow.scalar_type() == at::kInt && overflow.numel() == B, "keyframe_count: overflow is a device int32 [B]");
+  check(dpvo_keyframe_count((int)mode, n.data_ptr<int64_t>(), tstamp.data_ptr<int64_t>(), F, (int)B, counter.data_ptr<int64_t>(),
+                            delta.data_ptr<float>(), delta_src.data_ptr<int64_t>(), T, overflow.data_ptr<int>(), stream()),
+        "dpvo_b200_ext.keyframe_count");
+}
+Tensor keyframe_trajectory(Tensor poses, Tensor tstamp, Tensor n, int64_t F, Tensor delta, Tensor delta_src, Tensor counter, Tensor error) {
+  need_cuda(poses, "poses");
+  c10::cuda::CUDAGuard guard(poses.device());
+  const int64_t B = n.numel();
+  i64_rows(n, B, "keyframe_trajectory: n is a device int64 [B]");
+  f32_rows(poses, B * F, 7, "keyframe_trajectory: poses are contiguous fp32 [B F, 7]");
+  i64_rows(tstamp, B * F, "keyframe_trajectory: tstamp is a contiguous device int64 [B, F]");
+  i64_rows(counter, B, "keyframe_trajectory: counter is a device int64 [B]");
+  TORCH_CHECK(delta_src.is_cuda() && delta_src.scalar_type() == at::kLong && delta_src.is_contiguous() && delta_src.numel() % B == 0,
+              "keyframe_trajectory: delta_src is a contiguous device int64 [B, T]");
+  const int64_t T = delta_src.numel() / B;
+  f32_rows(delta, B * T, 7, "keyframe_trajectory: delta is a contiguous fp32 [B, T, 7]");
+  TORCH_CHECK(error.is_cuda() && error.scalar_type() == at::kInt && error.is_contiguous() && error.numel() == B,
+              "keyframe_trajectory: error is a device int32 [B]");
+  Tensor map = torch::empty({B, T}, poses.options().dtype(at::kInt));
+  Tensor out = torch::empty({B, T, 7}, poses.options());
+  check(dpvo_keyframe_trajectory(poses.data_ptr<float>(), tstamp.data_ptr<int64_t>(), n.data_ptr<int64_t>(), F, (int)B, delta.data_ptr<float>(),
+                                 delta_src.data_ptr<int64_t>(), T, counter.data_ptr<int64_t>(), map.data_ptr<int>(), out.data_ptr<float>(),
+                                 error.data_ptr<int>(), stream()),
+        "dpvo_b200_ext.keyframe_trajectory");
+  return out;
 }
 
 // ------------------------------------------------------------------------------ frame encoders
@@ -1162,7 +1278,12 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
         py::arg("n_active"), py::arg("overflow"));
   m.def("pgraph_remove_store", &pgraph_remove_store, "window removal with the loop exception, removed edges kept in the inactive store");
   m.def("loop_flags", &loop_flags, "loop-edge / long-range flags, minimum active ii and inactive count in one record");
-  m.def("loop_normalize", &loop_normalize, "PatchGraph.normalize on the device");
+  m.def("loop_normalize", &loop_normalize, "PatchGraph.normalize on the device (and the keyframe delta table's translations)",
+        py::arg("poses"), py::arg("patches"), py::arg("n"), py::arg("M"), py::arg("delta") = py::none());
+  m.def("keyframe_motion", &keyframe_motion, "keyframe motion test, delta record and frame-count decrement of B streams");
+  m.def("keyframe_shift", &keyframe_shift, "the KI - 1 slot copies of a culled keyframe over every per-frame buffer and ring");
+  m.def("keyframe_count", &keyframe_count, "add_frame (mode 0) / skip_frame (mode 1) timestamp bookkeeping of B streams");
+  m.def("keyframe_trajectory", &keyframe_trajectory, "one inverted pose per timestamp through the live keyframes and delta chains");
   m.def("neighbors_from_groups", &neighbors_from_groups, "temporal neighbours from a kk/jj grouping");
   m.def("encoder_conv", &encoder_conv, "one frame-encoder convolution (tensor cores, fused norm / join prologue)", py::arg("shape"),
         py::arg("x"), py::arg("w"), py::arg("bias"), py::arg("x_stats") = py::none(), py::arg("x_relu") = false, py::arg("skip") = py::none(),

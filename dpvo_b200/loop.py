@@ -64,6 +64,7 @@ class LoopClosure:
         self.flags = torch.zeros(4, dtype=torch.long, device=dev)
         self.ran_global_ba = set()                                                     # dpvo.py:42, host side
         self.scores = None
+        self.keyframes = None                                                          # keyframe.Keyframes, if one culls
 
     # ------------------------------------------------------------------------ dpvo.py:449-455 + patchgraph.py:56-82
     def candidates(self):
@@ -112,20 +113,23 @@ class LoopClosure:
         return (self.s_ii[a - c:], self.s_jj[a - c:], self.s_kk[a - c:], self.s_target[:, a - c:], self.s_weight[:, a - c:])
 
     # ------------------------------------------------------------------------ dpvo.py:312-326, patchgraph.py:84-91
-    def normalize(self, poses, patches, n):
-        extensions()[3].loop_normalize(poses, patches, int(n), self.M)
+    def normalize(self, poses, patches, n, delta=None):
+        """delta: a keyframe delta table (fp32 [T, 7]) whose translations are scaled with the poses', or None"""
+        extensions()[3].loop_normalize(poses, patches, int(n), self.M, delta)
 
     def global_ba(self, poses, patches, intrinsics, n, t0, count, E, lmbda, iterations=2):
         """normalize, then the wide (eff_impl) bundle adjustment of poses [t0, n) over the `count` inactive edges and the
         first E active slots (their weights already multiplied by `active`).  Eager, host-synchronised by its dense
-        solve; raises if the inactive store overflowed or a frame has more observers than the wide path holds."""
+        solve; raises if the inactive store overflowed or a frame has more observers than the wide path holds.
+        When a keyframe.Keyframes culls this stream (it registers itself as `keyframes`), normalize scales its
+        recorded relative poses with the map (patchgraph.py:89-90)."""
         if int(self.s_overflow.item()):
             raise RuntimeError("LoopClosure.global_ba: the inactive store (%d edges) overflowed; removed edges were lost"
                                % self.pg.inactive_cap)
         if int(self.region_overflow.item()):
             raise RuntimeError("LoopClosure.global_ba: a proposal overwrote loop edges that were still active")
         g = self.pg
-        self.normalize(poses, patches, n)
+        self.normalize(poses, patches, n, None if self.keyframes is None else self.keyframes.delta[0])
         lo, hi = g.inactive_cap - int(count), g.inactive_cap + int(E)
         fastba.BA(poses.view(1, -1, 7), patches.view(1, -1, 3, 3, 3), intrinsics.view(1, -1, 4), g.target_all[:, lo:hi],
                   g.weight_all[:, lo:hi], lmbda, g.ii_all[lo:hi], g.jj_all[lo:hi], g.kk_all[lo:hi], int(t0), int(n),

@@ -229,3 +229,62 @@ def make_loop_state(config="fast", n_frames=60, period=20, radius=2.0, noise=1e-
         st.imap = (torch.randn(1, pmem * M, 384, generator=gd, device=device) / 4).to(dtype)
         st.net = torch.zeros(1, st.E, 384, device=device, dtype=dtype)
     return st
+
+
+def make_stop_go_state(config="fast", n_frames=16, total=200, stop=8, go=8, speed=0.4, yaw_deg=0.5, buffer=None, mem=36,
+                       device="cuda", seed=1234, features=True, dtype=torch.half):
+    """A camera that stops and goes, for keyframe culling: over `total` timestamps it alternates `stop` frames standing
+    still (a 1e-4 jitter) with `go` frames moving `speed` units per frame sideways while turning `yaw_deg` per frame.
+    DPVO's motion test between frames two apart then gives about 0 px while stopped and tens of px while moving
+    (fx / 4 * speed * 2 * inverse depth, inverse depths 0.25..1), far from the 15 px threshold on both sides.
+    The state holds the first `n_frames` timestamps as frames (edges: replay_edges); extras["trajectory"] [total, 7]
+    and extras["patches"] [total M, 3, 3, 3] hold every timestamp's pose and patches for a tracking loop to add.
+    buffer (pose slots) defaults to total + 2, the last slot being free for DevicePatchGraph's dummy frame; the rings
+    hold `mem` frames (pmem = mem)."""
+    cfg = dict(CONFIGS[config]) if isinstance(config, str) else dict(config)
+    M = cfg["M"]
+    buffer = total + 2 if buffer is None else int(buffer)
+    assert n_frames <= total < buffer
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    h, w = cfg["ht"] // 4, cfg["wd"] // 4
+    fx, fy, cx, cy = [v / 4.0 for v in cfg["intrinsics"]]
+    traj = torch.zeros(total, 7, dtype=torch.float64)
+    x, yaw = 0.0, 0.0
+    for t in range(total):
+        if t > 0 and (t - 1) % (stop + go) >= stop:            # timestamps stop + 1 .. stop + go of each period move
+            x += speed
+            yaw += math.radians(yaw_deg)
+        traj[t, 0] = -x
+        traj[t, 4] = math.sin(0.5 * yaw)
+        traj[t, 6] = math.cos(0.5 * yaw)
+    traj[:, :3] += 1e-4 * torch.randn(total, 3, generator=g, dtype=torch.float64)
+    traj = traj.float()
+    px = torch.randint(1, w - 1, (total * M,), generator=g).float()
+    py = torch.randint(1, h - 1, (total * M,), generator=g).float()
+    offs = torch.tensor([-1.0, 0.0, 1.0])
+    allp = torch.zeros(total * M, 3, 3, 3)
+    allp[:, 0] = px[:, None, None] + offs[None, None, :]
+    allp[:, 1] = py[:, None, None] + offs[None, :, None]
+    allp[:, 2] = (0.25 + 0.75 * torch.rand(total * M, generator=g))[:, None, None]
+    poses = torch.zeros(buffer, 7)
+    poses[:, 6] = 1.0
+    poses[:n_frames] = traj[:n_frames]
+    patches = torch.zeros(buffer * M, 3, 3, 3)
+    patches[:, 2] = 1.0
+    patches[:n_frames * M] = allp[:n_frames * M]
+    intr = torch.tensor([fx, fy, cx, cy]).repeat(buffer, 1)
+    ii, jj, kk = replay_edges(n_frames, M, cfg["lifetime"], cfg["removal"])
+    st = SyntheticState(cfg=cfg, n=n_frames, t0=max(n_frames - cfg["opt_window"], 1), ii=ii.to(device), jj=jj.to(device),
+                        kk=kk.to(device), poses=poses.to(device), patches=patches.to(device), intrinsics=intr.to(device))
+    st.extras["trajectory"] = traj.to(device)
+    st.extras["patches"] = allp.to(device)
+    if features:
+        gd = torch.Generator(device=device).manual_seed(seed + 1)
+        f1 = (torch.randn(1, mem, h, w, 128, generator=gd, device=device) / 4).to(dtype).permute(0, 1, 4, 2, 3)
+        f2 = torch.nn.functional.avg_pool2d(f1[0].float(), 4, 4).to(dtype)[None]
+        st.fmap1 = f1
+        st.fmap2 = f2.permute(0, 1, 3, 4, 2).contiguous().permute(0, 1, 4, 2, 3)
+        st.gmap = (torch.randn(1, mem * M, 3, 3, 128, generator=gd, device=device) / 4).to(dtype).permute(0, 1, 4, 2, 3)
+        st.imap = (torch.randn(1, mem * M, 384, generator=gd, device=device) / 4).to(dtype)
+        st.net = torch.zeros(1, st.E, 384, device=device, dtype=dtype)
+    return st

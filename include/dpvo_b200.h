@@ -541,6 +541,9 @@ int dpvo_pgraph_new_edges(const int64_t* n_dev, int M, int r, int64_t* ii, int64
  *                      (dpvo.py:348); the minimum active ii (INT64_MAX without one); *s_count (0 if s_count is NULL)
  *   dpvo_loop_normalize  PatchGraph.normalize (patchgraph.py:84-91) for frames [0, n): depths / mean depth, translations
  *                      * mean depth, every pose rebased on pose 0.  patches fp32 [>= n M, 3, P, P], poses fp32 [>= n, 7]
+ *   dpvo_loop_normalize_deltas  the same, and the translations of the n_delta relative poses of a keyframe delta table
+ *                      (fp32 [n_delta, 7], dpvo_keyframe_*) * mean depth as well (dP.scale(s), patchgraph.py:89-90).
+ *                      dpvo_loop_normalize is this call with no table.
  */
 int64_t dpvo_loop_candidates(int max_age, int freq, int kf_index);
 int dpvo_loop_scores(const float* poses, const float* patches, const float* intrinsics, const int64_t* n_dev,
@@ -558,6 +561,49 @@ int dpvo_pgraph_remove_store(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* act
 int dpvo_loop_flags(const int64_t* ii, const uint8_t* active, int64_t cap, int64_t normal, int64_t n, int removal,
                     const int32_t* s_count, int64_t* flags, void* stream);
 int dpvo_loop_normalize(float* poses, float* patches, int64_t n, int M, int P, void* stream);
+int dpvo_loop_normalize_deltas(float* poses, float* patches, int64_t n, int M, int P, float* delta, int64_t n_delta,
+                               void* stream);
+
+/* ---- Keyframe culling (dpvo_b200/csrc/keyframe.cu) ------------------------------------------------------------------
+ * DPVO.keyframe (dpvo/dpvo.py:257-300) and get_pose / terminate (:166-198) for B >= 1 streams of F frame slots each
+ * (one stream: B = 1).  Stream b's frames are [b F, (b + 1) F) of poses fp32 [B F, 7], patches fp32 [B F M, 3, 3, 3] and
+ * intrinsics fp32 [B F, 4]; edges carry these global numbers.  Per stream, on the device: n int64 [B] (local frame
+ * counts), tstamp int64 [B, F] (the timestamp of every frame slot), counter int64 [B] (the next timestamp), and a delta
+ * table of T >= F timestamps: delta fp32 [B, T, 7] (relative poses) with delta_src int64 [B, T] (their source
+ * timestamp, < 0 where nothing is recorded).  KI = keyframe_index >= 1.
+ *   dpvo_keyframe_motion  stream b's edges are slots [b slots, (b + 1) slots) of ii / jj / kk / active.  With
+ *                      i = n - KI - 1, j = n - KI + 1, k = n - KI: m = mean(i, j) + mean(j, i), each the fp64 mean of the
+ *                      flow_mag (beta = 0.5) of all 9 pixels of every active edge of that (ii, jj), validity ignored; an
+ *                      empty set gives NaN.  flag int32 [B] = (m / 2 < thresh), k int64 [B] = b F + k (global, the
+ *                      frame for dpvo_pgraph_remove rule 1), m fp64 [B].  Under the flag: delta[tstamp[k]] =
+ *                      P_k P_{k-1}^-1 with source tstamp[k - 1] (*overflow [b] = 1 if tstamp[k] >= T), and n[b] -= 1.
+ *                      64 CTAs per stream write partial sums to workspace (dpvo_keyframe_motion_workspace_bytes(B)
+ *                      bytes), one thread per stream adds them in order: two launches give identical bits.
+ *   dpvo_keyframe_shift  under flag[b]: for t = k .. n - 2 (KI - 1 launches, one per step, in that order), slot t + 1 ->
+ *                      slot t of each of the nbuf (<= 8) buffers.  Buffer q's slot t of stream b is the row_bytes[q]
+ *                      bytes at bases[q] + (b rows[q] + t mod rows[q]) row_bytes[q]: rows = F for per-frame buffers,
+ *                      mem / pmem for the rings.  rows[q] < KI and row_bytes not a positive multiple of 4 are rejected.
+ *   dpvo_keyframe_count  mode 0 (add_frame, dpvo.py:400, 440): tstamp[n - 1] = counter, counter += 1.  mode 1
+ *                      (skip_frame, :441-444): delta[counter] = identity with source counter - 1, counter += 1.  A
+ *                      timestamp outside the table sets overflow[b].
+ *   dpvo_keyframe_trajectory  out fp32 [B, T, 7]: for t < counter, pose(t)^-1 where pose(t) is the pose of the live
+ *                      frame with tstamp t, else dP_t pose(src_t) (terminate()'s poses.inv()).  map int32 [B, T] is
+ *                      scratch.  A chain of stream b that meets an unrecorded timestamp writes NaN and sets error[b]
+ *                      (int32 [B]).
+ */
+int dpvo_keyframe_motion(const float* poses, const float* patches, const float* intrinsics, int64_t F, int B,
+                         const int64_t* ii, const int64_t* jj, const int64_t* kk, const uint8_t* active, int64_t slots,
+                         int64_t* n, const int64_t* tstamp, float* delta, int64_t* delta_src, int64_t T, int ki,
+                         double thresh, int32_t* flag, int64_t* k, double* m, int32_t* overflow, void* workspace,
+                         int64_t workspace_bytes, void* stream);
+int64_t dpvo_keyframe_motion_workspace_bytes(int B);
+int dpvo_keyframe_shift(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F, int B,
+                        int ki, const int32_t* flag, const int64_t* k, void* stream);
+int dpvo_keyframe_count(int mode, const int64_t* n, int64_t* tstamp, int64_t F, int B, int64_t* counter, float* delta,
+                        int64_t* delta_src, int64_t T, int32_t* overflow, void* stream);
+int dpvo_keyframe_trajectory(const float* poses, const int64_t* tstamp, const int64_t* n, int64_t F, int B,
+                             const float* delta, const int64_t* delta_src, int64_t T, const int64_t* counter,
+                             int32_t* map, float* out, int32_t* error, void* stream);
 
 /* ---- Frame encoders (dpvo_b200/csrc/encoder.cu) ---------------------------------------------------------------------
  * BasicEncoder4 (extractor.py:200-264) as used by Patchifier (net.py:95-157) for inference: fnet (instance norm after
