@@ -333,7 +333,12 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
       for (int i = 0; i < 96; ++i) acc[i] = fmaxf(acc[i], 0.f);
     };
     // LayerNorm over the 384 columns of each of this thread's two rows: 48 columns here, the rest in the 3 other lanes of
-    // the quad and in the paired warp of the other column half
+    // the quad and in the paired warp of the other column half.  One pass gives the row's sum S and sum of squares S2;
+    // S2/n - mean^2 is accurate to 34 u of the variance (u = 2^-24) while 17 mean^2 <= S2/n.  Past that it cancels (by up to
+    // all of its digits where |mean| >> spread), and the row takes a second pass, M2 = sum (x - mean)^2 about the mean of
+    // the first, through a second exchange round; nn.LayerNorm does not cancel either.  Both halves of a row combine
+    // their parts in the same order and so compute the same mean and rstd bits, and the two warps of a pair cover the
+    // same rows, so both take the second round or neither (its barriers are theirs).
     auto layer_norm = [&](const float* g, const float* b) {
       float s[2] = {0.f, 0.f}, q[2] = {0.f, 0.f};
 #pragma unroll
@@ -350,14 +355,41 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
         for (int o = 1; o <= 2; o <<= 1) { s[rr] += __shfl_xor_sync(0xffffffffu, s[rr], o); q[rr] += __shfl_xor_sync(0xffffffffu, q[rr], o); }
       if ((lane & 3) == 0) { xch2[h * CH_M + rl] = make_float2(s[0], q[0]); xch2[h * CH_M + rl + 8] = make_float2(s[1], q[1]); }
       pair_sync();
-      float mean[2], rstd[2];
+      float mean[2], var[2];
+      bool again = false;
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const float2 o = xch2[(h ^ 1) * CH_M + rl + 8 * rr];
         const float S = h ? o.x + s[rr] : s[rr] + o.x, S2 = h ? o.y + q[rr] : q[rr] + o.y;     // same order in both halves
         mean[rr] = S * (1.0f / CH_DIM);
-        rstd[rr] = rsqrtf(fmaxf(S2 * (1.0f / CH_DIM) - mean[rr] * mean[rr], 0.f) + CH_EPS);
+        const float ms = S2 * (1.0f / CH_DIM);
+        var[rr] = ms - mean[rr] * mean[rr];
+        again |= 17.0f * (mean[rr] * mean[rr]) > ms;
       }
+      if (__any_sync(0xffffffffu, again)) {
+        pair_sync();                                                 // both warps have read the first exchange
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          q[rr] = 0.f;
+#pragma unroll
+          for (int j = 0; j < 24; ++j) {
+            const float d0 = acc[4 * j + 2 * rr] - mean[rr], d1 = acc[4 * j + 2 * rr + 1] - mean[rr];
+            q[rr] += d0 * d0 + d1 * d1;
+          }
+#pragma unroll
+          for (int o = 1; o <= 2; o <<= 1) q[rr] += __shfl_xor_sync(0xffffffffu, q[rr], o);
+        }
+        if ((lane & 3) == 0) { xch2[h * CH_M + rl].x = q[0]; xch2[h * CH_M + rl + 8].x = q[1]; }
+        pair_sync();
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const float o = xch2[(h ^ 1) * CH_M + rl + 8 * rr].x;
+          var[rr] = (h ? o + q[rr] : q[rr] + o) * (1.0f / CH_DIM);
+        }
+      }
+      float rstd[2];
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) rstd[rr] = rsqrtf(fmaxf(var[rr], 0.f) + CH_EPS);
       pair_sync();                                                   // exchange slots free for the next use
 #pragma unroll
       for (int j = 0; j < 24; ++j) {

@@ -738,7 +738,8 @@ Tensor update_neighbor_mlp(Tensor net16_in, Tensor index, Tensor Wab, Tensor par
 }
 
 std::vector<Tensor> update_gru_heads(Tensor net32, c10::optional<Tensor> hij16, c10::optional<Tensor> group_of, Tensor W6, Tensor params,
-                                     c10::optional<Tensor> coords, c10::optional<Tensor> workspace, c10::optional<Tensor> hkk16, c10::optional<Tensor> group_kk) {
+                                     c10::optional<Tensor> coords, c10::optional<Tensor> workspace, c10::optional<Tensor> hkk16, c10::optional<Tensor> group_kk,
+                                     c10::optional<Tensor> delta_out, c10::optional<Tensor> weight_out) {
   need_cuda(net32, "net");
   c10::cuda::CUDAGuard guard(net32.device());
   chain_check(net32, at::kFloat, "net32"); chain_check(W6, at::kHalf, "W6"); chain_check(params, at::kFloat, "params");
@@ -763,7 +764,10 @@ std::vector<Tensor> update_gru_heads(Tensor net32, c10::optional<Tensor> hij16, 
   const int64_t wsb = dpvo_update_gru_workspace_bytes();
   Tensor ws = workspace.has_value() ? *workspace : byte_ws(wsb, net32);
   TORCH_CHECK(ws.is_cuda() && ws.is_contiguous() && (int64_t)(ws.numel() * ws.element_size()) >= wsb, "update_gru_heads: workspace too small");
-  Tensor delta = torch::empty({1, E, 2}, net32.options()), weight = torch::empty({1, E, 2}, net32.options());
+  Tensor delta = delta_out.has_value() ? *delta_out : torch::empty({1, E, 2}, net32.options());
+  Tensor weight = weight_out.has_value() ? *weight_out : torch::empty({1, E, 2}, net32.options());
+  chain_check(delta, at::kFloat, "delta_out"); chain_check(weight, at::kFloat, "weight_out");
+  TORCH_CHECK(delta.numel() == E * 2 && weight.numel() == E * 2, "update_gru_heads: delta_out / weight_out must hold [E, 2]");
   check(dpvo_update_gru_heads(net32.data_ptr<float>(), hij.defined() ? hij.data_ptr() : nullptr, gof.defined() ? gof.data_ptr<int>() : nullptr,
                               hkk.defined() ? hkk.data_ptr() : nullptr, gkk.defined() ? gkk.data_ptr<int>() : nullptr, W6.data_ptr(), params.data_ptr<float>(), cd.defined() ? cd.data_ptr<float>() : nullptr, P,
                               delta.data_ptr<float>(), weight.data_ptr<float>(), ws.data_ptr(), E, stream()),
@@ -1264,7 +1268,8 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("update_neighbor_mlp", &update_neighbor_mlp, "fused masked neighbour gather + 2-layer MLP + residual (net.py:83-85)", py::arg("net16_in"), py::arg("index"),
         py::arg("Wab"), py::arg("params"), py::arg("net32"), py::arg("net16_out") = py::none());
   m.def("update_gru_heads", &update_gru_heads, "fused group add + GRU + heads (net.py:88-92)", py::arg("net32"), py::arg("hij16"), py::arg("group_of"),
-        py::arg("W6"), py::arg("params"), py::arg("coords") = py::none(), py::arg("workspace") = py::none(), py::arg("hkk16") = py::none(), py::arg("group_kk") = py::none());
+        py::arg("W6"), py::arg("params"), py::arg("coords") = py::none(), py::arg("workspace") = py::none(), py::arg("hkk16") = py::none(), py::arg("group_kk") = py::none(),
+        py::arg("delta_out") = py::none(), py::arg("weight_out") = py::none());
   m.def("update_gru_workspace_bytes", &update_gru_workspace_bytes, "scratch bytes of update_gru_heads");
   m.def("pgraph_remove", &pgraph_remove, "park edges by rule on the fixed-capacity edge store", py::arg("ii"), py::arg("jj"), py::arg("kk"), py::arg("active"),
         py::arg("rule"), py::arg("frame"), py::arg("param"), py::arg("enable"), py::arg("dummy_frame"), py::arg("dummy_patch"), py::arg("M"), py::arg("n_active"));
