@@ -793,7 +793,8 @@ extern "C" int dpvo_corr_forward_pyramid2(const void* fmap1, const int64_t* fmap
   a.coords = coords; a.ii = ii; a.jj = jj; a.out = out; a.out_stride = 2;
   a.out_offset[0] = 0; a.out_offset[1] = 1; a.nlev = 2; a.B = B; a.M = M; a.C = C; a.P = P; a.R = radius;
   a.out_row = out_row_stride;
-  // wgmma + TMA path: fp16 channels-last rings, batch 1, caller-provided scratch for the edge list
+  // binned path (level 1 from shared-memory regions, level 0 on wgmma + TMA): fp16 channels-last rings, batch 1,
+  // caller-provided scratch for the bins and edge lists
   if (workspace && workspace_bytes >= dpvo_corr_pyramid2_workspace_bytes(M) && B == 1 && S1 > 0 && S2 > 0 &&
       mma_eligible(a, dtype)) {
     const int rc = corr_tc_forward(fmap1, a.s1, S1, fmap2_l0, a.s2[0], H0, W0, fmap2_l1, a.s2[1], H1, W1, S2, lvl1_div, coords, ii, jj,
@@ -803,7 +804,8 @@ extern "C" int dpvo_corr_forward_pyramid2(const void* fmap1, const int64_t* fmap
   return corr_dispatch(a, dtype, true, (cudaStream_t)stream);
 }
 
-extern "C" int64_t dpvo_corr_pyramid2_workspace_bytes(int64_t M) { return (M + 1) * (int64_t)sizeof(int) + 16; }
+namespace dpvo { int64_t corr_bin_workspace_bytes(int64_t M); }
+extern "C" int64_t dpvo_corr_pyramid2_workspace_bytes(int64_t M) { return corr_bin_workspace_bytes(M); }
 
 extern "C" int dpvo_corr_backward(const void* fmap1, const int64_t* fmap1_strides,
                                   const void* fmap2, const int64_t* fmap2_strides,

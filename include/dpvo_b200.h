@@ -96,10 +96,10 @@ int dpvo_corr_forward_pyramid2(const void* fmap1, const int64_t* fmap1_strides,
                                int dtype, int B, int M, int C, int P,
                                int S1, int S2, int radius,
                                void* workspace, int64_t workspace_bytes, void* stream);
-/* Scratch for the wgmma/TMA kernel of dpvo_corr_forward_pyramid2 (list of edges whose nine tap windows do
- * not fit one 10x10 box, finished by the mma.sync kernel).  workspace may be NULL: the call then runs the
- * mma.sync kernel for every edge.  S1 / S2 are the slot counts of the patch-feature and frame-feature rings
- * (extents of the TMA tensor maps). */
+/* Scratch for the binned path of dpvo_corr_forward_pyramid2 (per-bin counters and edge lists of the level-1
+ * regions and the level-0 wgmma/TMA kernel, and the list of edges whose nine tap windows fit no box, finished by the
+ * mma.sync kernel).  workspace may be NULL: the call then runs the mma.sync kernel for every edge.  S1 / S2 are the
+ * slot counts of the patch-feature and frame-feature rings (extents of the TMA tensor maps and of the bins). */
 int64_t dpvo_corr_pyramid2_workspace_bytes(int64_t M);
 
 /*
