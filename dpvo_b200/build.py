@@ -23,7 +23,7 @@ EXTDIR = os.path.join(ROOT, "_ext")
 OBJDIR = os.path.join(os.path.dirname(ROOT), "build", "obj")
 INCLUDE = os.path.join(os.path.dirname(ROOT), "include")
 
-CU_SOURCES = ["common.cu", "chain.cu", "corr.cu", "corr_bin.cu", "corr_tc.cu", "patchify.cu", "lie.cu", "graph.cu", "pgraph.cu", "loop.cu", "keyframe.cu", "ba.cu", "ba_wide.cu", "update_ops.cu", "gemm.cu", "softagg.cu", "encoder.cu"]
+CU_SOURCES = ["common.cu", "chain.cu", "corr.cu", "corr_bin.cu", "corr_tc.cu", "patchify.cu", "lie.cu", "graph.cu", "pgraph.cu", "loop.cu", "keyframe.cu", "ba.cu", "ba_wide.cu", "update_ops.cu", "gemm.cu", "softagg.cu", "encoder.cu", "map.cu"]
 SHIM_MODULES = ["cuda_corr", "cuda_ba", "lietorch_backends", "dpvo_b200_ext"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",

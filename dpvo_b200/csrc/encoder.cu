@@ -407,9 +407,9 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
   if (tid == 0) *ticket = 0;                                             // ready for the next launch
 }
 
-// inet's output convolution at the M centroids, the gmap windows of the written fmap1 slot and the patch grids.
-// Block (m, b): centroid m of image b, whose rows are frame_row[b] (fmap1), feat_row[b] + m (gmap, imap) and
-// patch_row[b] + m (patches).
+// inet's output convolution at the M centroids, the gmap windows of the written fmap1 slot, the patch grids and
+// (optional) the viewer colours.  Block (m, b): centroid m of image b, whose rows are frame_row[b] (fmap1),
+// feat_row[b] + m (gmap, imap) and patch_row[b] + m (patches, colours).
 struct EncCentroidParams {
   const float* coords;             // [B, M, 2]
   const float* depth;              // [B, M] or null: depth 1
@@ -426,8 +426,45 @@ struct EncCentroidParams {
   __half* imap;
   int64_t i_sm;
   float* patches;                  // rows of 27
+  uint8_t* colors;                 // rows of 3, or null: no colours
+  const uint8_t* image;            // image 0 (+ b x_sb for image b), element strides xs_c, xs_y, xs_x
+  int64_t x_sb, xs_c, xs_y, xs_x;
+  int img_h, img_w;
   int frame_row[EC_MAX_IMAGES], feat_row[EC_MAX_IMAGES], patch_row[EC_MAX_IMAGES];
 };
+
+// The viewer colour of dpvo.py:392-404, channel c (BGR -> RGB: image channel 2 - c) of the centroid (fx, fy):
+//   clr = patchify(2 (img / 255.0) - 0.5, 4 (coords + 0.5), 0)     the bilinear form of altcorr.patchify
+//   byte = uint8((clr + 0.5) * 127.5)                               truncating, through int64 as torch converts
+// Every step is one fp32 operation rounded to nearest, in torch's order, so that nothing is contracted into an FMA.
+// img / 255.0 is the product with the fp32 reciprocal of 255: that is how PyTorch's CUDA kernel divides a tensor by a
+// scalar (the CPU kernel divides, and differs for the bytes 24..31).  Pixels outside the image read 0 (the normalised
+// value, not the byte), as patchify zero-fills its window.
+__device__ __forceinline__ uint8_t centroid_color(const uint8_t* im, int64_t sc, int64_t sy, int64_t sx, int H, int W, float fx,
+                                                  float fy, int c) {
+  constexpr float kInv255 = 1.0f / 255.0f;
+  const float px = __fmul_rn(4.0f, __fadd_rn(fx, 0.5f)), py = __fmul_rn(4.0f, __fadd_rn(fy, 0.5f));
+  const float flx = floorf(px), fly = floorf(py);
+  const float dx = __fsub_rn(px, flx), dy = __fsub_rn(py, fly);
+  const int x0 = (int)flx, y0 = (int)fly;
+  const uint8_t* plane = im + (int64_t)(2 - c) * sc;
+  float v[2][2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int y = y0 + i, x = x0 + j;
+      v[i][j] = (y >= 0 && y < H && x >= 0 && x < W)
+                    ? __fsub_rn(__fmul_rn(2.0f, __fmul_rn((float)plane[y * sy + x * sx], kInv255)), 0.5f) : 0.0f;
+    }
+  const float omx = __fsub_rn(1.0f, dx), omy = __fsub_rn(1.0f, dy);
+  const float x00 = __fmul_rn(__fmul_rn(omy, omx), v[0][0]);
+  const float x01 = __fmul_rn(__fmul_rn(omy, dx), v[0][1]);
+  const float x10 = __fmul_rn(__fmul_rn(dy, omx), v[1][0]);
+  const float x11 = __fmul_rn(__fmul_rn(dy, dx), v[1][1]);
+  const float clr = __fadd_rn(__fadd_rn(__fadd_rn(x00, x01), x10), x11);
+  return (uint8_t)__float2ll_rz(__fmul_rn(__fadd_rn(clr, 0.5f), 127.5f));
+}
 
 __global__ void __launch_bounds__(128)
 enc_centroid_kernel(const __grid_constant__ EncCentroidParams p) {
@@ -468,6 +505,10 @@ enc_centroid_kernel(const __grid_constant__ EncCentroidParams p) {
     const int c = tid / 9, i = (tid / 3) % 3, j = tid % 3;
     const float d = p.depth ? p.depth[bm] : 1.0f;
     p.patches[(p.patch_row[b] + (int64_t)m) * 27 + tid] = c == 0 ? fx + (float)(j - 1) : c == 1 ? fy + (float)(i - 1) : d;
+  } else if (tid >= 32 && tid < 35 && p.colors != nullptr) {
+    const int c = tid - 32;
+    p.colors[(p.patch_row[b] + (int64_t)m) * 3 + c] =
+        centroid_color(p.image + b * p.x_sb, p.xs_c, p.xs_y, p.xs_x, p.img_h, p.img_w, fx, fy, c);
   }
 }
 
@@ -636,14 +677,14 @@ static int64_t weight_offset(int encoder, int layer) {
 // rows [a, a + n) and [b, b + n) share a row
 static bool rows_overlap(int64_t a, int64_t b, int64_t n) { return a < b + n && b < a + n; }
 
-extern "C" int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
-                                  const void* w16, const float* b32, const float* coords, int M,
-                                  void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
-                                  void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
-                                  void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm, int64_t feat_rows,
-                                  float* patches, int64_t patch_rows,
-                                  const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
-                                  const float* depth, void* workspace, int64_t workspace_bytes, void* stream) {
+static int encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
+                         const void* w16, const float* b32, const float* coords, int M,
+                         void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
+                         void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
+                         void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm, int64_t feat_rows,
+                         float* patches, int64_t patch_rows,
+                         const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
+                         const float* depth, uint8_t* colors, void* workspace, int64_t workspace_bytes, void* stream) {
   DPVO_REQUIRE(B >= 1 && B <= EC_MAX_IMAGES, "encode_frames: B=%d images, 1 to %d per call", B, EC_MAX_IMAGES);
   DPVO_REQUIRE(images && w16 && b32 && coords && fmap1 && fmap2 && gmap && imap && patches && frame_row && feat_row && patch_row &&
                workspace, "encode_frames: null pointer");
@@ -770,12 +811,43 @@ extern "C" int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_
   c.fmap1 = (const __half*)fmap1; c.f_sr = f1_sr; c.f_sy = f1_sy; c.f_sx = f1_sx;
   c.gmap = (__half*)gmap; c.g_sm = g_sm; c.g_sy = g_sy; c.g_sx = g_sx;
   c.imap = (__half*)imap; c.i_sm = i_sm; c.patches = patches;
+  c.colors = colors; c.image = images; c.x_sb = s_b; c.xs_c = s_c; c.xs_y = s_y; c.xs_x = s_x; c.img_h = H; c.img_w = W;
   for (int b = 0; b < B; ++b) {
     c.frame_row[b] = (int)frame_row[b]; c.feat_row[b] = (int)feat_row[b]; c.patch_row[b] = (int)patch_row[b];
   }
   enc_centroid_kernel<<<dim3(M, B), 128, 0, st>>>(c);
   DPVO_LAUNCH_CHECK("enc_centroid_kernel");
   return DPVO_OK;
+}
+
+extern "C" int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
+                                  const void* w16, const float* b32, const float* coords, int M,
+                                  void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
+                                  void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
+                                  void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm, int64_t feat_rows,
+                                  float* patches, int64_t patch_rows,
+                                  const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
+                                  const float* depth, void* workspace, int64_t workspace_bytes, void* stream) {
+  return encode_frames(images, s_b, s_c, s_y, s_x, B, H, W, w16, b32, coords, M, fmap1, f1_sr, f1_sy, f1_sx, fmap2, f2_sr, f2_sy,
+                       f2_sx, frame_rows, gmap, g_sm, g_sy, g_sx, imap, i_sm, feat_rows, patches, patch_rows, frame_row, feat_row,
+                       patch_row, depth, nullptr, workspace, workspace_bytes, stream);
+}
+
+// dpvo_encode_frames that also writes the viewer colours: uint8 rows [patch_row[b], patch_row[b] + M) of colors
+// [patch_rows, 3], the rows of the patches
+extern "C" int dpvo_encode_frames_colors(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H,
+                                         int W, const void* w16, const float* b32, const float* coords, int M,
+                                         void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
+                                         void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
+                                         void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm,
+                                         int64_t feat_rows, float* patches, int64_t patch_rows,
+                                         const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
+                                         const float* depth, uint8_t* colors, void* workspace, int64_t workspace_bytes,
+                                         void* stream) {
+  DPVO_REQUIRE(colors, "encode_frames_colors: null colour destination (dpvo_encode_frames writes none)");
+  return encode_frames(images, s_b, s_c, s_y, s_x, B, H, W, w16, b32, coords, M, fmap1, f1_sr, f1_sy, f1_sx, fmap2, f2_sr, f2_sy,
+                       f2_sx, frame_rows, gmap, g_sm, g_sy, g_sx, imap, i_sm, feat_rows, patches, patch_rows, frame_row, feat_row,
+                       patch_row, depth, colors, workspace, workspace_bytes, stream);
 }
 
 // one image: the B = 1 case of dpvo_encode_frames, its slots the single rows of rings of one frame and M patches

@@ -4,6 +4,7 @@
 //                            j = n - KI + 1; under the decision it records frame k's relative pose in the delta table and
 //                            decrements the device frame counter
 //   * dpvo_keyframe_shift    the KI - 1 slot copies t + 1 -> t, t = k .. n - 2, of every per-frame buffer and ring
+//                            (dpvo_keyframe_shift_bytes: also slots of any byte count, e.g. the 3 M-byte colour rows)
 //   * dpvo_keyframe_count    add_frame (tstamp[n - 1] = counter++) and skip_frame (delta[c] = (c - 1, identity))
 //   * dpvo_keyframe_trajectory  one pose per timestamp t < counter, through the live keyframes and the delta chains
 // Every call reads the frame counters from device memory, so a frame's add_frame + cull can be captured in a CUDA graph.
@@ -14,14 +15,14 @@
 namespace dpvo {
 
 constexpr int KF_THREADS = 256;
-constexpr int KF_MAX_BUFS = 8;
+constexpr int KF_MAX_BUFS = 9;
 constexpr int KF_PARTS = 64;                 // CTAs per stream of the motion test's partial sums
 
 struct KfBufs {
   char* base[KF_MAX_BUFS];
   int64_t row_bytes[KF_MAX_BUFS];
   int64_t rows[KF_MAX_BUFS];
-  int vec[KF_MAX_BUFS];                         // bytes per copy: 16, 8 or 4
+  int vec[KF_MAX_BUFS];                         // bytes per copy: 16, 8, 4 or 1
   int nbuf;
 };
 
@@ -135,8 +136,10 @@ keyframe_shift_kernel(KfBufs bufs, int64_t F, int step, const int32_t* __restric
       for (int64_t x = tid; x < rb / 16; x += stride) reinterpret_cast<uint4*>(dst)[x] = reinterpret_cast<const uint4*>(src)[x];
     } else if (bufs.vec[q] == 8) {
       for (int64_t x = tid; x < rb / 8; x += stride) reinterpret_cast<uint2*>(dst)[x] = reinterpret_cast<const uint2*>(src)[x];
-    } else {
+    } else if (bufs.vec[q] == 4) {
       for (int64_t x = tid; x < rb / 4; x += stride) reinterpret_cast<uint32_t*>(dst)[x] = reinterpret_cast<const uint32_t*>(src)[x];
+    } else {
+      for (int64_t x = tid; x < rb; x += stride) dst[x] = src[x];
     }
   }
 }
@@ -238,8 +241,9 @@ extern "C" int dpvo_keyframe_motion(const float* poses, const float* patches, co
   return DPVO_OK;
 }
 
-extern "C" int dpvo_keyframe_shift(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F, int B,
-                                   int ki, const int32_t* flag, const int64_t* k, void* stream) {
+// any_bytes: rows of any positive byte count at any alignment, copied 1 byte at a time where 4 does not divide them
+static int keyframe_shift(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F, int B, int ki,
+                          const int32_t* flag, const int64_t* k, bool any_bytes, void* stream) {
   DPVO_REQUIRE(ki >= 1, "keyframe_shift: keyframe_index=%d must be at least 1", ki);
   DPVO_REQUIRE(nbuf >= 0 && nbuf <= KF_MAX_BUFS && B >= 1 && F >= 2, "keyframe_shift: bad sizes (buffers=%d, B=%d, frames=%lld)",
                nbuf, B, (long long)F);
@@ -248,16 +252,21 @@ extern "C" int dpvo_keyframe_shift(void* const* bases, const int64_t* row_bytes,
   int64_t most = 0;
   for (int q = 0; q < nbuf; ++q) {
     DPVO_REQUIRE(bases[q], "keyframe_shift: null pointer (buffer %d)", q);
-    DPVO_REQUIRE(row_bytes[q] > 0 && row_bytes[q] % 4 == 0, "keyframe_shift: buffer %d has %lld-byte slots, a positive multiple of 4 is needed",
-                 q, (long long)row_bytes[q]);
+    if (any_bytes)
+      DPVO_REQUIRE(row_bytes[q] > 0, "keyframe_shift: buffer %d has %lld-byte slots, a positive count is needed", q,
+                   (long long)row_bytes[q]);
+    else
+      DPVO_REQUIRE(row_bytes[q] > 0 && row_bytes[q] % 4 == 0, "keyframe_shift: buffer %d has %lld-byte slots, a positive multiple of 4 is needed",
+                   q, (long long)row_bytes[q]);
     DPVO_REQUIRE(rows[q] >= ki, "keyframe_shift: buffer %d holds %lld slots per stream, fewer than keyframe_index=%d", q,
                  (long long)rows[q], ki);
     const uintptr_t a = (uintptr_t)bases[q];
     bufs.base[q] = (char*)bases[q];
     bufs.row_bytes[q] = row_bytes[q];
     bufs.rows[q] = rows[q];
-    bufs.vec[q] = (a % 16 == 0 && row_bytes[q] % 16 == 0) ? 16 : (a % 8 == 0 && row_bytes[q] % 8 == 0) ? 8 : 4;
-    DPVO_REQUIRE(a % 4 == 0, "keyframe_shift: buffer %d is not 4-byte aligned", q);
+    bufs.vec[q] = (a % 16 == 0 && row_bytes[q] % 16 == 0) ? 16 : (a % 8 == 0 && row_bytes[q] % 8 == 0) ? 8
+                : (a % 4 == 0 && row_bytes[q] % 4 == 0) ? 4 : 1;
+    DPVO_REQUIRE(any_bytes || a % 4 == 0, "keyframe_shift: buffer %d is not 4-byte aligned", q);
     most = std::max(most, row_bytes[q] / bufs.vec[q]);
   }
   bufs.nbuf = nbuf;
@@ -267,6 +276,16 @@ extern "C" int dpvo_keyframe_shift(void* const* bases, const int64_t* row_bytes,
     DPVO_LAUNCH_CHECK("keyframe_shift_kernel");
   }
   return DPVO_OK;
+}
+
+extern "C" int dpvo_keyframe_shift(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F, int B,
+                                   int ki, const int32_t* flag, const int64_t* k, void* stream) {
+  return keyframe_shift(bases, row_bytes, rows, nbuf, F, B, ki, flag, k, false, stream);
+}
+
+extern "C" int dpvo_keyframe_shift_bytes(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F,
+                                         int B, int ki, const int32_t* flag, const int64_t* k, void* stream) {
+  return keyframe_shift(bases, row_bytes, rows, nbuf, F, B, ki, flag, k, true, stream);
 }
 
 extern "C" int dpvo_keyframe_count(int mode, const int64_t* n, int64_t* tstamp, int64_t F, int B, int64_t* counter, float* delta,

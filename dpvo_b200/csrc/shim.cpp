@@ -1002,8 +1002,8 @@ void keyframe_shift(std::vector<Tensor> bufs, std::vector<int64_t> rows, int64_t
     rb.push_back(t.numel() * (int64_t)t.element_size() / (B * rows[q]));
     rw.push_back(rows[q]);
   }
-  check(dpvo_keyframe_shift(bases.data(), rb.data(), rw.data(), (int)bases.size(), F, (int)B, (int)ki, flag.data_ptr<int>(),
-                            k.data_ptr<int64_t>(), stream()),
+  check(dpvo_keyframe_shift_bytes(bases.data(), rb.data(), rw.data(), (int)bases.size(), F, (int)B, (int)ki, flag.data_ptr<int>(),
+                                  k.data_ptr<int64_t>(), stream()),
         "dpvo_b200_ext.keyframe_shift");
 }
 void keyframe_count(int64_t mode, Tensor n, Tensor tstamp, int64_t F, Tensor counter, Tensor delta, Tensor delta_src, Tensor overflow) {
@@ -1107,8 +1107,18 @@ std::vector<c10::optional<Tensor>> encoder_conv(int64_t shape, Tensor x, Tensor 
   return {y, st, jn, pl};
 }
 
+// the viewer colours of M patch rows: a contiguous CUDA uint8 tensor of M x 3 bytes ([M, 3], or [F, M, 3] rows)
+static uint8_t* color_rows(const c10::optional<Tensor>& colors, int64_t rows, const Tensor& like, const char* what) {
+  if (!colors.has_value()) return nullptr;
+  const Tensor& c = *colors;
+  TORCH_CHECK(c.is_cuda() && c.device() == like.device() && c.scalar_type() == at::kByte && c.is_contiguous() && c.dim() >= 2 &&
+              c.size(-1) == 3 && c.numel() == rows * 3, what, ": colors must be a contiguous uint8 CUDA tensor of ", rows,
+              " rows of 3 bytes on the image's device");
+  return c.data_ptr<uint8_t>();
+}
+
 void encode_frame(Tensor image, Tensor w16, Tensor b32, Tensor coords, Tensor fmap1, Tensor fmap2, Tensor gmap, Tensor imap,
-                  Tensor patches, Tensor workspace) {
+                  Tensor patches, Tensor workspace, c10::optional<Tensor> colors) {
   for (auto* t : {&image, &w16, &b32, &coords, &fmap1, &fmap2, &gmap, &imap, &patches, &workspace})
     TORCH_CHECK(t->is_cuda(), "encode_frame: every tensor must be a CUDA tensor (this build has no CPU path)");
   TORCH_CHECK(image.scalar_type() == at::kByte && image.dim() == 3 && image.size(0) == 3, "encode_frame: image must be uint8 [3, H, W]");
@@ -1131,6 +1141,18 @@ void encode_frame(Tensor image, Tensor w16, Tensor b32, Tensor coords, Tensor fm
   TORCH_CHECK(patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() == M * 27, "encode_frame: patches must be contiguous float32 [M, 3, 3, 3]");
   TORCH_CHECK(workspace.is_contiguous(), "encode_frame: workspace must be contiguous");
   const c10::cuda::CUDAGuard guard(image.device());
+  if (colors.has_value()) {
+    uint8_t* cp = color_rows(colors, M, image, "encode_frame");
+    const int64_t row0 = 0;
+    check(dpvo_encode_frames_colors(image.data_ptr<uint8_t>(), 0, image.stride(0), image.stride(1), image.stride(2), 1, H, W,
+                                    w16.data_ptr(), b32.data_ptr<float>(), coords.data_ptr<float>(), (int)M,
+                                    fmap1.data_ptr(), 0, fmap1.stride(0), fmap1.stride(1), fmap2.data_ptr(), 0, fmap2.stride(0),
+                                    fmap2.stride(1), 1, gmap.data_ptr(), gmap.stride(0), gmap.stride(1), gmap.stride(2), imap.data_ptr(),
+                                    imap.stride(0), M, patches.data_ptr<float>(), M, &row0, &row0, &row0, nullptr, cp,
+                                    workspace.data_ptr(), workspace.numel() * workspace.element_size(), stream()),
+          "dpvo_b200_ext.encode_frame");
+    return;
+  }
   check(dpvo_encode_frame(image.data_ptr<uint8_t>(), image.stride(0), image.stride(1), image.stride(2), H, W, w16.data_ptr(), b32.data_ptr<float>(),
                           coords.data_ptr<float>(), (int)M, fmap1.data_ptr(), fmap1.stride(0), fmap1.stride(1), fmap2.data_ptr(), fmap2.stride(0),
                           fmap2.stride(1), gmap.data_ptr(), gmap.stride(0), gmap.stride(1), gmap.stride(2), imap.data_ptr(), imap.stride(0),
@@ -1145,7 +1167,7 @@ int64_t encode_frame_workspace_bytes(int64_t H, int64_t W) { return dpvo_encode_
 // rows feat_rows[b] + [0, M) and patch rows patch_rows[b] + [0, M).  The library checks the rows.
 void encode_frames(Tensor images, Tensor w16, Tensor b32, Tensor coords, Tensor fmap1, Tensor fmap2, Tensor gmap, Tensor imap,
                    Tensor patches, std::vector<int64_t> frame_rows, std::vector<int64_t> feat_rows, std::vector<int64_t> patch_rows,
-                   c10::optional<Tensor> depth, Tensor workspace) {
+                   c10::optional<Tensor> depth, Tensor workspace, c10::optional<Tensor> colors) {
   for (auto* t : {&images, &w16, &b32, &coords, &fmap1, &fmap2, &gmap, &imap, &patches, &workspace})
     TORCH_CHECK(t->is_cuda(), "encode_frames: every tensor must be a CUDA tensor (this build has no CPU path)");
   TORCH_CHECK(images.scalar_type() == at::kByte && images.dim() == 4 && images.size(1) == 3, "encode_frames: images must be uint8 [B, 3, H, W]");
@@ -1180,6 +1202,18 @@ void encode_frames(Tensor images, Tensor w16, Tensor b32, Tensor coords, Tensor 
   }
   TORCH_CHECK(workspace.is_contiguous(), "encode_frames: workspace must be contiguous");
   const c10::cuda::CUDAGuard guard(images.device());
+  if (colors.has_value()) {
+    uint8_t* cp = color_rows(colors, patches.size(0), images, "encode_frames");
+    check(dpvo_encode_frames_colors(images.data_ptr<uint8_t>(), images.stride(0), images.stride(1), images.stride(2), images.stride(3),
+                                    (int)B, H, W, w16.data_ptr(), b32.data_ptr<float>(), coords.data_ptr<float>(), (int)M,
+                                    fmap1.data_ptr(), fmap1.stride(0), fmap1.stride(1), fmap1.stride(2),
+                                    fmap2.data_ptr(), fmap2.stride(0), fmap2.stride(1), fmap2.stride(2), fmap1.size(0),
+                                    gmap.data_ptr(), gmap.stride(0), gmap.stride(1), gmap.stride(2), imap.data_ptr(), imap.stride(0),
+                                    gmap.size(0), patches.data_ptr<float>(), patches.size(0), frame_rows.data(), feat_rows.data(),
+                                    patch_rows.data(), dp, cp, workspace.data_ptr(), workspace.numel() * workspace.element_size(), stream()),
+          "dpvo_b200_ext.encode_frames");
+    return;
+  }
   check(dpvo_encode_frames(images.data_ptr<uint8_t>(), images.stride(0), images.stride(1), images.stride(2), images.stride(3), (int)B, H, W,
                            w16.data_ptr(), b32.data_ptr<float>(), coords.data_ptr<float>(), (int)M,
                            fmap1.data_ptr(), fmap1.stride(0), fmap1.stride(1), fmap1.stride(2),
@@ -1192,6 +1226,27 @@ void encode_frames(Tensor images, Tensor w16, Tensor b32, Tensor coords, Tensor 
 
 int64_t encode_frames_workspace_bytes(int64_t B, int64_t H, int64_t W) {
   return dpvo_encode_frames_workspace_bytes((int)B, (int)H, (int)W);
+}
+
+// ------------------------------------------------------------------------------ map
+// points [B F M, 3] rows [b F M, b F M + n[b] M) of every stream b = 0 .. len(n) - 1, from poses [B F, 7], patches
+// [B F M, 3, 3, 3] and intrinsics [B F, 4]
+void point_cloud(Tensor poses, Tensor patches, Tensor intrinsics, int64_t F, std::vector<int64_t> n, Tensor points) {
+  need_cuda(poses, "poses");
+  c10::cuda::CUDAGuard guard(poses.device());
+  const int64_t B = (int64_t)n.size();
+  TORCH_CHECK(B >= 1 && F >= 1, "point_cloud: one frame count per stream and F >= 1 needed");
+  f32_rows(poses, B * F, 7, "point_cloud: poses are contiguous fp32 [B F, 7]");
+  f32_rows(intrinsics, B * F, 4, "point_cloud: intrinsics are contiguous fp32 [B F, 4]");
+  TORCH_CHECK(patches.is_cuda() && patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() % (B * F * 27) == 0 &&
+              patches.numel() > 0, "point_cloud: patches are contiguous fp32 [B F M, 3, 3, 3]");
+  const int64_t M = patches.numel() / (B * F * 27);
+  f32_rows(points, B * F * M, 3, "point_cloud: points are contiguous fp32 [B F M, 3]");
+  for (const Tensor* t : {&patches, &intrinsics, &points})
+    TORCH_CHECK(t->device() == poses.device(), "point_cloud: every tensor must be on the poses' device");
+  check(dpvo_point_cloud(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(), F, (int)M, (int)B, n.data(),
+                         points.data_ptr<float>(), stream()),
+        "dpvo_b200_ext.point_cloud");
 }
 
 int64_t launch_count() { return dpvo_launch_count(); }
@@ -1296,12 +1351,14 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
         py::arg("want_pool") = false, py::arg("scale") = 1.0);
   m.def("encode_frame", &encode_frame, "both frame encoders: uint8 image -> fmap1, fmap2, gmap, imap, patches slots", py::arg("image"),
         py::arg("w16"), py::arg("b32"), py::arg("coords"), py::arg("fmap1"), py::arg("fmap2"), py::arg("gmap"), py::arg("imap"),
-        py::arg("patches"), py::arg("workspace"));
+        py::arg("patches"), py::arg("workspace"), py::arg("colors") = py::none());
   m.def("encode_frame_workspace_bytes", &encode_frame_workspace_bytes, "scratch bytes of encode_frame for an H x W image");
   m.def("encode_frames", &encode_frames, "both frame encoders over B images in one pass, into rows of the rings", py::arg("images"),
         py::arg("w16"), py::arg("b32"), py::arg("coords"), py::arg("fmap1"), py::arg("fmap2"), py::arg("gmap"), py::arg("imap"),
         py::arg("patches"), py::arg("frame_rows"), py::arg("feat_rows"), py::arg("patch_rows"), py::arg("depth"),
-        py::arg("workspace"));
+        py::arg("workspace"), py::arg("colors") = py::none());
+  m.def("point_cloud", &point_cloud, "the world points of every patch centre of frames [0, n) of each stream (dpvo.py:358-360)",
+        py::arg("poses"), py::arg("patches"), py::arg("intrinsics"), py::arg("F"), py::arg("n"), py::arg("points"));
   m.def("encode_frames_workspace_bytes", &encode_frames_workspace_bytes, "scratch bytes of encode_frames for B H x W images");
   m.def("launch_count", &launch_count, "kernel launches issued by libdpvo_b200 so far");
   m.def("version", &version, "library version string");

@@ -220,9 +220,11 @@ class FrameEncoder:
         return torch.stack([x, y], dim=-1).float()[0]
 
     @torch.no_grad()
-    def encode_into(self, image, M, strategy, fmap1_slot, fmap2_slot, gmap_slot, imap_slot, patches_slot, coords=None):
+    def encode_into(self, image, M, strategy, fmap1_slot, fmap2_slot, gmap_slot, imap_slot, patches_slot, coords=None,
+                    colors_slot=None):
         """Encode `image` into the slots: fmap1 [h, w, 128], fmap2 [h/4, w/4, 128], gmap [M, 3, 3, 128] (all fp16,
-        channels-last), imap fp16 [M, 384], patches fp32 [M, 3, 3, 3] with depth 1.  Returns the centroids [M, 2]."""
+        channels-last), imap fp16 [M, 384], patches fp32 [M, 3, 3, 3] with depth 1, and, when `colors_slot` (contiguous
+        uint8 [M, 3]) is given, the viewer colours of dpvo.py:392-404 there.  Returns the centroids [M, 2]."""
         if not (isinstance(image, torch.Tensor) and image.is_cuda):
             raise RuntimeError("FrameEncoder: the image must be a CUDA tensor (there is no CPU path)")
         if image.dtype != torch.uint8 or image.dim() != 3 or image.shape[0] != 3:
@@ -233,18 +235,21 @@ class FrameEncoder:
             raise RuntimeError("FrameEncoder: coords must be [M, 2] = [%d, 2], got %s" % (M, tuple(coords.shape)))
         w16, b32 = self.packed()
         extensions()[3].encode_frame(image, w16, b32, coords.float().contiguous(), fmap1_slot, fmap2_slot, gmap_slot,
-                                     imap_slot, patches_slot, self.workspace(image.shape[1], image.shape[2], image.device))
+                                     imap_slot, patches_slot, self.workspace(image.shape[1], image.shape[2], image.device),
+                                     colors=colors_slot)
         return coords
 
     @torch.no_grad()
     def encode_frames_into(self, images, M, strategy, fmap1_ring, fmap2_ring, gmap_ring, imap_ring, patches_ring,
-                           frame_rows, feat_rows, patch_rows, coords=None, depth=None):
+                           frame_rows, feat_rows, patch_rows, coords=None, depth=None, colors_ring=None):
         """encode_into for B images in one pass of the encoders.  images: uint8 [B, 3, H, W] (CHW or HWC strides).
         Image b goes to row frame_rows[b] of the rings fmap1 [R, h, w, 128] and fmap2 [R, h/4, w/4, 128], rows
         feat_rows[b] + [0, M) of gmap [Rg, 3, 3, 128] and imap [Rg, 384], and rows patch_rows[b] + [0, M) of patches
         [Rp, 3, 3, 3] with depth[b] (fp32 [B, M]; None: depth 1).  Each image's slots are bit-identical to encode_into
         of that image alone with the same centroids.  Centroids are drawn once per image, in image order, unless
-        `coords` [B, M, 2] is given (then nothing is drawn and the call can be captured).  Returns the coords."""
+        `coords` [B, M, 2] is given (then nothing is drawn and the call can be captured).  colors_ring (contiguous uint8
+        with Rp rows of 3 bytes, e.g. [Rp / M, M, 3]) receives image b's viewer colours in rows patch_rows[b] + [0, M),
+        the rows of its patches.  Returns the coords."""
         if not (isinstance(images, torch.Tensor) and images.is_cuda):
             raise RuntimeError("FrameEncoder: the images must be a CUDA tensor (there is no CPU path)")
         if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[1] != 3:
@@ -259,5 +264,6 @@ class FrameEncoder:
         w16, b32 = self.packed()
         extensions()[3].encode_frames(images, w16, b32, coords.float().contiguous(), fmap1_ring, fmap2_ring, gmap_ring, imap_ring,
                                       patches_ring, [int(r) for r in frame_rows], [int(r) for r in feat_rows],
-                                      [int(r) for r in patch_rows], depth, self.workspace(H, W, images.device, B))
+                                      [int(r) for r in patch_rows], depth, self.workspace(H, W, images.device, B),
+                                      colors=colors_ring)
         return coords

@@ -12,6 +12,7 @@ and `read` is the frame's one device-to-host copy.  For a streams.StreamBatch ev
 import torch
 
 from . import extensions
+from .synthetic import check_map
 
 # the reference's defaults (dpvo/config.py: KEYFRAME_INDEX, KEYFRAME_THRESH)
 KEYFRAME_DEFAULTS = dict(keyframe_index=4, keyframe_thresh=15.0)
@@ -30,6 +31,7 @@ class Keyframes:
         def param(name, given):
             return given if given is not None else cfg.get(name, KEYFRAME_DEFAULTS[name])
 
+        check_map(state, "Keyframes")
         self.ki = int(param("keyframe_index", keyframe_index))
         self.thresh = float(param("keyframe_thresh", keyframe_thresh))
         if self.ki < 1:
@@ -61,9 +63,10 @@ class Keyframes:
         if self.T < self.F:
             raise ValueError("Keyframes: max_timestamps=%d is smaller than the %d frame slots" % (self.T, self.F))
         self.bufs, self.rows = [], []
-        for name in ("poses", "patches", "intrinsics", "fmap1", "fmap2", "gmap", "imap"):
-            t = getattr(state, name)
-            if t is None:                                       # states built with features=False
+        # colors: the viewer colours of a state with map buffers (dpvo.py:289); points are recomputed by the next update
+        for name in ("poses", "patches", "intrinsics", "fmap1", "fmap2", "gmap", "imap", "colors"):
+            t = getattr(state, name, None)
+            if t is None:                                       # features=False, or no map
                 continue
             rows = self.F
             if name in ("fmap1", "fmap2"):

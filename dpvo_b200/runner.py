@@ -15,6 +15,7 @@ from . import projective_ops as pops
 from .net import Update, EdgeGroups, DIM
 from .frontend import encoder_output_size
 from .streams import StreamBatch
+from .synthetic import check_map
 
 
 class UpdateRunner:
@@ -31,7 +32,11 @@ class UpdateRunner:
         part of the loop region (a captured graph: over the whole store).  Each step then
         reads one small record from the device to decide this, and runs the global bundle adjustment in place of the
         local one when an active edge has ii < n - removal - 1 and none ran at this n (dpvo.py:348).  The rings must
-        hold pmem = max_edge_age patch frames (dpvo.py:58-61)."""
+        hold pmem = max_edge_age patch frames (dpvo.py:58-61).
+        A state with map buffers (synthetic.make_state(map=True), StreamBatch(map=True)) also gets the map: every step
+        ends with the points of frames [0, n) (dpvo.py:358-360), and ingest_image(s) write the new frame's colours
+        (dpvo.py:404).  `map()` returns them."""
+        check_map(state, "UpdateRunner")
         self.s = state
         self.batch = state if isinstance(state, StreamBatch) else None
         self.pg = graph
@@ -166,7 +171,23 @@ class UpdateRunner:
                               self.ba_iterations, groups_kk, groups_ij)
         if ev is not None:
             ev["ba1"].record()
+        if getattr(s, "points", None) is not None:
+            # dpvo.py:358-360, after whichever bundle adjustment ran; n is a launch parameter, as the BA window is
+            if self.batch is None:
+                F, ns = s.poses.shape[0], [s.n]
+            else:
+                F, ns = self.batch.F, [self.batch.stream(b).n for b in range(self.batch.B)]
+            extensions()[3].point_cloud(s.poses, s.patches, s.intrinsics, F, ns, s.points)
         return target, weight
+
+    def map(self, stream=None):
+        """demo.py:53-54's arrays of one stream, read-only views: (points [n M, 3] fp32, colors [n M, 3] uint8), the
+        points of the last step and the colours of the ingested frames.  In a batch, `stream` names the stream."""
+        s = self._stream_state(stream, "map")
+        if getattr(s, "points", None) is None or getattr(s, "colors", None) is None:
+            raise RuntimeError("map: this state has no map buffers (make_state(map=True) / StreamBatch(map=True))")
+        m = s.n * self.M
+        return s.points[:m], s.colors.view(-1, 3)[:m]
 
     # ----------------------------------------------------------------------------- CUDA graph
     def capture(self):
@@ -253,7 +274,8 @@ class UpdateRunner:
     @torch.no_grad()
     def ingest_image(self, image, depth=None, coords=None, stream=None):
         """Encode a uint8 camera image [3, H, W] (CHW or HWC strides) straight into the slots `ingest_frame` writes:
-        fmap1 / fmap2 slot (n-1) % mem, gmap / imap slot (n-1) % pmem, patches[(n-1) M : n M] (dpvo.py:389-438).
+        fmap1 / fmap2 slot (n-1) % mem, gmap / imap slot (n-1) % pmem, patches[(n-1) M : n M] (dpvo.py:389-438), and
+        colors[n-1] (dpvo.py:404) when the state has map buffers.
         Centroids are drawn as Patchifier.forward draws them, unless `coords` [M, 2] is given (CUDA-graph capture);
         the patch depths are then one torch.rand draw (dpvo.py:427), or `depth` (the median the caller computes once
         initialised, dpvo.py:429-431).  Poses, intrinsics and the motion model stay with the caller.  In a batch,
@@ -271,7 +293,8 @@ class UpdateRunner:
         coords = self.encoder.encode_into(image, M, self.encoder.strategy, s.fmap1[0, slot].permute(1, 2, 0),
                                           s.fmap2[0, slot].permute(1, 2, 0),
                                           s.gmap[0, pslot * M:(pslot + 1) * M].permute(0, 2, 3, 1),
-                                          s.imap[0, pslot * M:(pslot + 1) * M], patches, coords=coords)
+                                          s.imap[0, pslot * M:(pslot + 1) * M], patches, coords=coords,
+                                          colors_slot=None if getattr(s, "colors", None) is None else s.colors[s.n - 1])
         if depth is None:
             depth = torch.rand(M, 1, 1, device=patches.device, dtype=patches.dtype)
         patches[:, 2] = depth
@@ -326,7 +349,7 @@ class UpdateRunner:
         return self.encoder.encode_frames_into(images, M, self.encoder.strategy, batch.fmap1[0].permute(0, 2, 3, 1),
                                                batch.fmap2[0].permute(0, 2, 3, 1), batch.gmap[0].permute(0, 2, 3, 1),
                                                batch.imap[0], batch.patches, [r[0] for r in rows], [r[1] for r in rows],
-                                               [r[2] for r in rows], coords=coords, depth=depth)
+                                               [r[2] for r in rows], coords=coords, depth=depth, colors_ring=getattr(batch, "colors", None))
 
     # A streaming front end has frame t+1 in pinned memory while update t runs: its H2D copy goes to a staging
     # buffer on a copy stream (overlapping the update), and only the short device-to-device move into the ring

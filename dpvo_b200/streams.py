@@ -8,6 +8,9 @@ intrinsics, patches, feature rings and edges.  Stream b owns
     patches  [b F M, (b+1) F M)             of patches [B F M, 3, 3, 3]
     ring rows [b mem, (b+1) mem)            of fmap1 [1, B mem, 128, h, w] and fmap2 [1, B mem, 128, h/4, w/4]
     ring rows [b pmem M, (b+1) pmem M)      of gmap [1, B pmem M, 128, 3, 3] and imap [1, B pmem M, 384]
+    with map=True also
+    patches  [b F M, (b+1) F M)             of points [B F M, 3]   (fp32 world points, pg.points_'s layout)
+    frames   [b F, (b+1) F)                 of colors [B F, M, 3]  (uint8 viewer colours, pg.colors_'s layout)
 
 Every tensor has the single-stream layout (feature maps channels-last).  Edges carry global frame / patch numbers, so
 every per-edge and per-group kernel of the update sees one graph; no edge may join two streams.  `stream(b)` is a
@@ -23,7 +26,7 @@ MAX_STREAMS = 64
 
 
 class StreamBatch:
-    def __init__(self, B, cfg, frames_per_stream, mem, pmem=None, device="cuda", dtype=torch.half):
+    def __init__(self, B, cfg, frames_per_stream, mem, pmem=None, device="cuda", dtype=torch.half, map=False):
         B, F, mem = int(B), int(frames_per_stream), int(mem)
         pmem = mem if pmem is None else int(pmem)
         if not 1 <= B <= MAX_STREAMS:
@@ -45,6 +48,8 @@ class StreamBatch:
         self.fmap2 = torch.zeros(1, B * mem, h // 4, w // 4, 128, device=dev, dtype=dtype).permute(0, 1, 4, 2, 3)
         self.gmap = torch.zeros(1, B * pmem * M, 3, 3, 128, device=dev, dtype=dtype).permute(0, 1, 4, 2, 3)
         self.imap = torch.zeros(1, B * pmem * M, 384, device=dev, dtype=dtype)
+        self.points = torch.zeros(B * F * M, 3, device=dev) if map else None
+        self.colors = torch.zeros(B * F, M, 3, dtype=torch.uint8, device=dev) if map else None
         z = torch.zeros(0, dtype=torch.long, device=dev)
         self._streams = []
         for b in range(B):
@@ -53,7 +58,9 @@ class StreamBatch:
             self._streams.append(SyntheticState(cfg=self.cfg, n=0, t0=0, ii=z, jj=z, kk=z, poses=self.poses[fs],
                                                 patches=self.patches[ps], intrinsics=self.intrinsics[fs],
                                                 fmap1=self.fmap1[:, rs], fmap2=self.fmap2[:, rs], gmap=self.gmap[:, gs],
-                                                imap=self.imap[:, gs]))
+                                                imap=self.imap[:, gs],
+                                                points=self.points[ps] if map else None,
+                                                colors=self.colors[fs] if map else None))
         self.ii, self.jj, self.kk = z, z, z
 
     # ------------------------------------------------------------------------------------------------ streams
@@ -64,8 +71,12 @@ class StreamBatch:
         return self._streams[int(b)]
 
     def load(self, b, state):
-        """copy a single-stream state (its poses, patches, intrinsics, feature rings, edges, n and t0) into stream b"""
+        """copy a single-stream state (its poses, patches, intrinsics, feature rings, edges, n and t0) into stream b; in a
+        batch with map buffers also its points and colours (zeros where the state has none)"""
         s = self.stream(b)
+        if self.points is not None:
+            from .synthetic import check_map
+            check_map(state, "StreamBatch.load")
         if int(state.cfg["M"]) != self.M or (int(state.cfg["ht"]), int(state.cfg["wd"])) != (self.ht, self.wd):
             raise ValueError("StreamBatch.load: stream %d has M=%s and a %sx%s image, the batch M=%d and %dx%d: one "
                              "configuration and one image size per batch" % (b, state.cfg["M"], state.cfg["ht"],
@@ -87,6 +98,12 @@ class StreamBatch:
         s.poses[:nf].copy_(state.poses)
         s.patches[:nf * self.M].copy_(state.patches)
         s.intrinsics[:nf].copy_(state.intrinsics)
+        if self.points is not None:
+            for name, rows in (("points", nf * self.M), ("colors", nf)):
+                src, dst = getattr(state, name), getattr(s, name)
+                dst.zero_()
+                if src is not None:
+                    dst[:rows].copy_(src)
         s.ii, s.jj, s.kk = (t.to(self.poses.device) for t in (state.ii, state.jj, state.kk))
         s.n, s.t0 = int(state.n), int(state.t0)
 
@@ -95,7 +112,9 @@ class StreamBatch:
         s = self.stream(b)
         return SyntheticState(cfg=dict(self.cfg), n=s.n, t0=s.t0, ii=s.ii.clone(), jj=s.jj.clone(), kk=s.kk.clone(),
                               poses=s.poses.clone(), patches=s.patches.clone(), intrinsics=s.intrinsics.clone(),
-                              fmap1=s.fmap1.clone(), fmap2=s.fmap2.clone(), gmap=s.gmap.clone(), imap=s.imap.clone())
+                              fmap1=s.fmap1.clone(), fmap2=s.fmap2.clone(), gmap=s.gmap.clone(), imap=s.imap.clone(),
+                              points=None if s.points is None else s.points.clone(),
+                              colors=None if s.colors is None else s.colors.clone())
 
     # ------------------------------------------------------------------------------------------------ index maps
     def to_global(self, b, ii=None, jj=None, kk=None):

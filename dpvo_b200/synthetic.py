@@ -70,6 +70,8 @@ class SyntheticState:
     imap: torch.Tensor = None   # [1,mem*M,384]
     net: torch.Tensor = None    # [1,E,384]
     extras: dict = field(default_factory=dict)
+    points: torch.Tensor = None  # [N*M,3] fp32 world points of the patch centres (pg.points_), or None: no map
+    colors: torch.Tensor = None  # [N,M,3] uint8 viewer colours of the patches (pg.colors_), or None
 
     @property
     def E(self):
@@ -88,10 +90,34 @@ def _trajectory(n, device, dtype=torch.float32):
     return out.to(device=device, dtype=dtype)
 
 
+def add_map(state):
+    """give `state` the map buffers of dpvo.py:68-72, in the reference's layouts: points fp32 [N M, 3] (pg.points_) and
+    colors uint8 [N, M, 3] (pg.colors_), N = its pose slots; zero-filled.  Returns the state."""
+    N, M = state.poses.shape[0], int(state.cfg["M"])
+    state.points = torch.zeros(N * M, 3, device=state.poses.device)
+    state.colors = torch.zeros(N, M, 3, dtype=torch.uint8, device=state.poses.device)
+    return state
+
+
+def check_map(state, what):
+    """reject map buffers that are not in the layouts add_map gives (state: one stream, or a StreamBatch whose pose
+    rows are all its streams' frames)"""
+    N, M, dev = state.poses.shape[0], int(state.cfg["M"]), state.poses.device
+    for name, shape, dtype in (("points", (N * M, 3), torch.float32), ("colors", (N, M, 3), torch.uint8)):
+        t = getattr(state, name, None)
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != shape or t.dtype != dtype or not t.is_contiguous() or t.device != dev:
+            got = (tuple(t.shape), t.dtype, str(t.device)) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError("%s: %s must be a contiguous %s tensor %s on %s (the state's %d pose slots x M=%d), got %s"
+                             % (what, name, dtype, list(shape), dev, N, M, got))
+
+
 def make_state(config="default", n_frames=30, device="cuda", seed=1234, features=True, dtype=torch.half,
-               channels_last=True, buffer=64, mem=36, noise=0.0):
+               channels_last=True, buffer=64, mem=36, noise=0.0, map=False):
     """Build a steady-state synthetic DPVO state.  `buffer` is the number of pose slots allocated
-    (the reference allocates 4096); `mem` the feature ring size (dpvo.py:58)."""
+    (the reference allocates 4096); `mem` the feature ring size (dpvo.py:58).  map=True adds the map buffers
+    (`add_map`): UpdateRunner then writes the patch points every step and the encoders the patch colours."""
     cfg = dict(CONFIGS[config]) if isinstance(config, str) else dict(config)
     M = cfg["M"]
     g = torch.Generator(device="cpu").manual_seed(seed)
@@ -134,19 +160,22 @@ def make_state(config="default", n_frames=30, device="cuda", seed=1234, features
         st.fmap1, st.fmap2, st.gmap = f1, f2, gm
         st.imap = (torch.randn(1, mem * M, 384, generator=gd, device=device) / 4).to(dtype)
         st.net = torch.zeros(1, st.E, 384, device=device, dtype=dtype)
+    if map:
+        add_map(st)
     return st
 
 
-def make_batch(config="default", B=2, seeds=None, n_frames=30, device="cuda", frames_per_stream=64, mem=36):
+def make_batch(config="default", B=2, seeds=None, n_frames=30, device="cuda", frames_per_stream=64, mem=36, map=False):
     """B independent steady-state streams in one streams.StreamBatch: stream b is make_state(config, n_frames[b],
-    seed=seeds[b]) (an int n_frames serves every stream), with frames_per_stream pose slots and a ring of `mem`."""
+    seed=seeds[b]) (an int n_frames serves every stream), with frames_per_stream pose slots and a ring of `mem`.
+    map=True gives the batch (and every stream) the map buffers."""
     from .streams import StreamBatch
     cfg = dict(CONFIGS[config]) if isinstance(config, str) else dict(config)
     seeds = [1234 + 17 * b for b in range(B)] if seeds is None else list(seeds)
     frames = [n_frames] * B if isinstance(n_frames, int) else list(n_frames)
     if len(seeds) != B or len(frames) != B:
         raise ValueError("make_batch: one seed and one frame count per stream")
-    batch = StreamBatch(B, cfg, frames_per_stream, mem, mem, device=device)
+    batch = StreamBatch(B, cfg, frames_per_stream, mem, mem, device=device, map=map)
     for b in range(B):
         batch.load(b, make_state(cfg, frames[b], device=device, seed=seeds[b], buffer=frames_per_stream, mem=mem))
     batch.set_edges()

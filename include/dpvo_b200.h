@@ -580,9 +580,11 @@ int dpvo_loop_normalize_deltas(float* poses, float* patches, int64_t n, int M, i
  *                      64 CTAs per stream write partial sums to workspace (dpvo_keyframe_motion_workspace_bytes(B)
  *                      bytes), one thread per stream adds them in order: two launches give identical bits.
  *   dpvo_keyframe_shift  under flag[b]: for t = k .. n - 2 (KI - 1 launches, one per step, in that order), slot t + 1 ->
- *                      slot t of each of the nbuf (<= 8) buffers.  Buffer q's slot t of stream b is the row_bytes[q]
+ *                      slot t of each of the nbuf (<= 9) buffers.  Buffer q's slot t of stream b is the row_bytes[q]
  *                      bytes at bases[q] + (b rows[q] + t mod rows[q]) row_bytes[q]: rows = F for per-frame buffers,
  *                      mem / pmem for the rings.  rows[q] < KI and row_bytes not a positive multiple of 4 are rejected.
+ *   dpvo_keyframe_shift_bytes  dpvo_keyframe_shift for slots of any positive byte count at any alignment (a buffer whose
+ *                      slots 4 does not divide is copied one byte per thread), e.g. the colours uint8 [F, M, 3].
  *   dpvo_keyframe_count  mode 0 (add_frame, dpvo.py:400, 440): tstamp[n - 1] = counter, counter += 1.  mode 1
  *                      (skip_frame, :441-444): delta[counter] = identity with source counter - 1, counter += 1.  A
  *                      timestamp outside the table sets overflow[b].
@@ -599,6 +601,8 @@ int dpvo_keyframe_motion(const float* poses, const float* patches, const float* 
 int64_t dpvo_keyframe_motion_workspace_bytes(int B);
 int dpvo_keyframe_shift(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F, int B,
                         int ki, const int32_t* flag, const int64_t* k, void* stream);
+int dpvo_keyframe_shift_bytes(void* const* bases, const int64_t* row_bytes, const int64_t* rows, int nbuf, int64_t F,
+                              int B, int ki, const int32_t* flag, const int64_t* k, void* stream);
 int dpvo_keyframe_count(int mode, const int64_t* n, int64_t* tstamp, int64_t F, int B, int64_t* counter, float* delta,
                         int64_t* delta_src, int64_t T, int32_t* overflow, void* stream);
 int dpvo_keyframe_trajectory(const float* poses, const int64_t* tstamp, const int64_t* n, int64_t F, int B,
@@ -654,6 +658,12 @@ int dpvo_keyframe_trajectory(const float* poses, const int64_t* tstamp, const in
  * coords fp32 [B, M, 2].  depth fp32 [B, M] (the patches' third channel), or NULL for 1.
  * workspace: dpvo_encode_frames_workspace_bytes(B, H, W) bytes, B blocks of dpvo_encode_frame_workspace_bytes(H, W).
  * One strided memset and 12 launches for any B; no host synchronisation (graph-capturable).
+ *
+ * dpvo_encode_frames_colors: dpvo_encode_frames that also writes the viewer colours (dpvo.py:392-404), uint8 rows
+ * [patch_row[b], patch_row[b] + M) of colors [patch_rows, 3] (the patches' rows; pg.colors_'s [F, M, 3] layout):
+ *   colors[m][c] = uint8((clr[2 - c] + 0.5) * 127.5),  clr = the bilinear patchify (altcorr/correlation.py:51-66) of
+ *   2 (image * fp32(1 / 255)) - 0.5 at 4 (coords[m] + 0.5), pixels outside the image 0, each step one fp32 operation
+ *   rounded to nearest, the cast truncating.  Same launches as dpvo_encode_frames; colors must not be NULL.
  */
 #define DPVO_ENC_STEM        0   /* 7x7/2, 3 -> 32   */
 #define DPVO_ENC_C3_32       1   /* 3x3/1, 32 -> 32  */
@@ -700,6 +710,28 @@ int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t 
                        float* patches, int64_t patch_rows,
                        const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
                        const float* depth, void* workspace, int64_t workspace_bytes, void* stream);
+
+int dpvo_encode_frames_colors(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
+                              const void* w16, const float* b32, const float* coords, int M,
+                              void* fmap1, int64_t f1_sr, int64_t f1_sy, int64_t f1_sx,
+                              void* fmap2, int64_t f2_sr, int64_t f2_sy, int64_t f2_sx, int64_t frame_rows,
+                              void* gmap, int64_t g_sm, int64_t g_sy, int64_t g_sx, void* imap, int64_t i_sm, int64_t feat_rows,
+                              float* patches, int64_t patch_rows,
+                              const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
+                              const float* depth, uint8_t* colors, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- Map (dpvo_b200/csrc/map.cu) --------------------------------------------------------------------------------------
+ * dpvo_point_cloud: the points of DPVO.update (dpvo.py:358-360) for B (1..64) streams of F frame slots and M patches per
+ * frame.  Stream b's frames are [b F, (b + 1) F) of poses fp32 [B F, 7] and intrinsics fp32 [B F, 4], its patches
+ * [b F M, (b + 1) F M) of patches fp32 [B F M, 3, 3, 3] and its points the same rows of points fp32 [B F M, 3].  n is a
+ * host int64 [B] (each stream's frame count, passed by value: a captured graph keeps it).  Rows [0, n[b] M) of stream b
+ * get pops.point_cloud's centre point of each patch,
+ *   X = ((x - cx) / fx, (y - cy) / fy, 1, d),  P = act4(pose^-1, X),  point = P.xyz / P.w
+ * with the lietorch SE3 operators (pose^-1 rounded to fp32 and loaded again, as SE3.inv() then act4 do); the rows above
+ * are not written.  One launch, one thread per patch.
+ */
+int dpvo_point_cloud(const float* poses, const float* patches, const float* intrinsics, int64_t F, int M, int B,
+                     const int64_t* n, float* points, void* stream);
 
 #ifdef __cplusplus
 }
