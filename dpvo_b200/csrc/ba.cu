@@ -886,8 +886,6 @@ __global__ void reproject_kernel(const float* __restrict__ poses, const float* _
   }
 }
 
-static inline int64_t al256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 }  // namespace dpvo
 
 using namespace dpvo;
@@ -902,7 +900,7 @@ struct BaWs {
 };
 int64_t ba_ws_layout(int64_t E, int N, char* base, BaWs* w) {
   char* p = base;
-  auto take = [&](int64_t bytes) { char* r = p; p += al256(bytes); return r; };
+  auto take = [&](int64_t bytes) { char* r = p; p += align256(bytes); return r; };
   const int64_t gb = dpvo_group_workspace_bytes(E);
   char* k_order = take(E * 4); char* k_of = take(E * 4); char* k_start = take((E + 1) * 4);
   char* k_key = take(E * 8); char* k_n = take(4);
@@ -984,8 +982,8 @@ static int ba_run(BaArgs& a, int iterations, cudaStream_t st) {
 
 extern "C" int64_t dpvo_ba_grouped_workspace_bytes(int64_t E, int n_free_poses) {
   if (E < 0) E = 0;
-  return al256(E * 6 * (int64_t)std::max(n_free_poses, 1) * 4) + 2 * al256(E * 4) + al256(E * (int64_t)BA_REC * 4) +
-         al256(6 * BA_MAX_N * 4) + 512;
+  return align256(E * 6 * (int64_t)std::max(n_free_poses, 1) * 4) + 2 * align256(E * 4) + align256(E * (int64_t)BA_REC * 4) +
+         align256(6 * BA_MAX_N * 4) + 512;
 }
 
 extern "C" int dpvo_ba_forward_grouped(float* poses, float* patches, const float* intrinsics,
@@ -1004,16 +1002,16 @@ extern "C" int dpvo_ba_forward_grouped(float* poses, float* patches, const float
   DPVO_REQUIRE(N == 0 || (p_order && p_start && p_key_i && p_key_j && p_n), "ba_forward_grouped: pair grouping missing");
   if (N > BA_MAX_N) { set_error("ba_forward_grouped: %d free poses > %d", N, BA_MAX_N); return DPVO_ERR_UNSUPPORTED; }
   if (workspace_bytes < dpvo_ba_grouped_workspace_bytes(E, N)) { set_error("ba_forward_grouped: workspace too small"); return DPVO_ERR_WORKSPACE; }
-  char* p = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* p = align256(workspace);
   BaArgs a;
   a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
   a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = t0; a.N = N;
   a.k_order = k_order; a.k_start = k_start; a.k_key = k_key; a.k_n = k_n;
   a.p_order = p_order; a.p_start = p_start; a.p_key_i = p_key_i; a.p_key_j = p_key_j; a.p_n = p_n;
-  a.Ed = (float*)p; p += al256(E * 6 * (int64_t)std::max(N, 1) * 4);
-  a.Qk = (float*)p; p += al256(E * 4);
-  a.uk = (float*)p; p += al256(E * 4);
-  a.rec = (float*)p; p += al256(E * (int64_t)BA_REC * 4);
+  a.Ed = (float*)p; p += align256(E * 6 * (int64_t)std::max(N, 1) * 4);
+  a.Qk = (float*)p; p += align256(E * 4);
+  a.uk = (float*)p; p += align256(E * 4);
+  a.rec = (float*)p; p += align256(E * (int64_t)BA_REC * 4);
   a.dX = (float*)p;
   return ba_run(a, iterations, (cudaStream_t)stream);
 }
@@ -1027,9 +1025,9 @@ static int64_t ba_batched_part_floats(int max_free_poses) {
 extern "C" int64_t dpvo_ba_batched_workspace_bytes(int64_t E, int B, int max_free_poses) {
   if (E < 0) E = 0;
   if (B < 1) B = 1;
-  return al256(2 * (int64_t)(B + 1) * 4) + al256(E * 6 * (int64_t)std::max(max_free_poses, 1) * 4) + 2 * al256(E * 4) +
-         al256(E * (int64_t)BA_REC * 4) + al256((int64_t)B * 6 * BA_MAX_N * 4) +
-         al256((int64_t)B * ba_batched_part_floats(max_free_poses) * 4) + 256;
+  return align256(2 * (int64_t)(B + 1) * 4) + align256(E * 6 * (int64_t)std::max(max_free_poses, 1) * 4) + 2 * align256(E * 4) +
+         align256(E * (int64_t)BA_REC * 4) + align256((int64_t)B * 6 * BA_MAX_N * 4) +
+         align256((int64_t)B * ba_batched_part_floats(max_free_poses) * 4) + 256;
 }
 
 extern "C" int dpvo_ba_forward_batched(float* poses, float* patches, const float* intrinsics,
@@ -1062,18 +1060,18 @@ extern "C" int dpvo_ba_forward_batched(float* poses, float* patches, const float
                k_start && k_key && k_n && p_order && p_start && p_key_i && p_key_j && p_n, "ba_forward_batched: null pointer");
   if (workspace_bytes < dpvo_ba_batched_workspace_bytes(E, B, max_n)) { set_error("ba_forward_batched: workspace too small"); return DPVO_ERR_WORKSPACE; }
   cudaStream_t st = (cudaStream_t)stream;
-  char* p = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  int32_t* bounds = (int32_t*)p; p += al256(2 * (int64_t)(B + 1) * 4);
+  char* p = align256(workspace);
+  int32_t* bounds = (int32_t*)p; p += align256(2 * (int64_t)(B + 1) * 4);
   BaArgs a;
   a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
   a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = 0; a.N = max_n;
   a.k_order = k_order; a.k_start = k_start; a.k_key = k_key; a.k_n = k_n;
   a.p_order = p_order; a.p_start = p_start; a.p_key_i = p_key_i; a.p_key_j = p_key_j; a.p_n = p_n;
-  a.Ed = (float*)p; p += al256(E * 6 * (int64_t)max_n * 4);
-  a.Qk = (float*)p; p += al256(E * 4);
-  a.uk = (float*)p; p += al256(E * 4);
-  a.rec = (float*)p; p += al256(E * (int64_t)BA_REC * 4);
-  a.dX = (float*)p; p += al256((int64_t)B * 6 * BA_MAX_N * 4);
+  a.Ed = (float*)p; p += align256(E * 6 * (int64_t)max_n * 4);
+  a.Qk = (float*)p; p += align256(E * 4);
+  a.uk = (float*)p; p += align256(E * 4);
+  a.rec = (float*)p; p += align256(E * (int64_t)BA_REC * 4);
+  a.dX = (float*)p; p += align256((int64_t)B * 6 * BA_MAX_N * 4);
   a.dbg = nullptr;
   // the fast path applies to the whole batch when every window fits it, the general path otherwise
   const bool fast = max_n <= BA_FAST_MAX_N;
@@ -1128,7 +1126,7 @@ extern "C" int dpvo_ba_forward(float* poses, float* patches, const float* intrin
     return DPVO_ERR_WORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  char* base = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* base = align256(workspace);
   BaWs w;
   ba_ws_layout(E, N, base, &w);
 

@@ -39,7 +39,6 @@
 // and stays in L2.
 #include "common.cuh"
 #include "tc.cuh"
-#include <cuda.h>
 #include <algorithm>
 #include <atomic>
 #include <cooperative_groups.h>
@@ -146,7 +145,7 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
     for (int s = 0; s < CH_WST; ++s) { mbar_init(&bars->w_full[s], 1); mbar_init(&bars->w_empty[s], 4 * CH_CL); }
     for (int s = 0; s < CH_KB; ++s) { mbar_init(&bars->a_full[s], CHAIN == CHAIN_C ? CH_GATHER_THREADS : 1); mbar_init(&bars->a_empty[s], CH_CONS_WARPS); }
     mbar_init(&bars->slots_free, CH_CONS_WARPS);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    mbar_init_fence();
   }
   for (int i = threadIdx.x; i < Cfg::NPARAM; i += blockDim.x) sparam[i] = i < a.n_params ? a.p[i] : 0.f;
   cluster.sync();                                                    // no peer multicasts or arrives before the barriers exist
@@ -590,33 +589,6 @@ chain_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CU
 
 using namespace dpvo;
 
-typedef CUresult (*ChEncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static int ch_tmap(CUtensorMap* m, const void* ptr, CUtensorMapDataType dt, int elt, int64_t rows, int64_t cols, int64_t ld,
-                   int box_cols, int box_rows, CUtensorMapSwizzle sw) {
-  // the encoder is a driver symbol, the same for every device of the process: looked up once (thread-safe static init)
-  static void* const p = []() -> void* {
-    void* f = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return nullptr;
-    return f;
-  }();
-  if (!p) {
-    set_error("update chain: cuTensorMapEncodeTiled is not available from the driver");
-    return DPVO_ERR_CUDA;
-  }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * elt};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = ((ChEncodeTiledFn)p)(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("update chain: cuTensorMapEncodeTiled failed (%d)", (int)r); return DPVO_ERR_CUDA; }
-  return DPVO_OK;
-}
-
 struct ChainMaps { CUtensorMap X, W0, W; };
 
 // how many CH_CL-CTA clusters of chain_kernel<CHAIN> the current device runs at once; queried once per device, after the
@@ -669,9 +641,9 @@ extern "C" int dpvo_update_corr_norm(const void* corr16, int64_t ld_corr, const 
   DPVO_REQUIRE(al16(corr16) && al16(W0) && al16(W25) && al16(params) && al16(net32) && al16(inp16) && al16(net16), "update_corr_norm: pointers must be 16-byte aligned");
   ChainMaps m;
   memset(&m, 0, sizeof(m));
-  int rc = ch_tmap(&m.X, corr16, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, E, CH_K0, ld_corr, 64, CH_M, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.W0, W0, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, CH_DIM, CH_K0, CH_K0, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
-  if (!rc) rc = ch_tmap(&m.W, W25, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
+  int rc = encode_tmap_2d(&m.X, "update chain", corr16, E, CH_K0, ld_corr, CH_M);
+  if (!rc) rc = encode_tmap_2d(&m.W0, "update chain", W0, CH_DIM, CH_K0, CH_K0, CH_WBOX);
+  if (!rc) rc = encode_tmap_2d(&m.W, "update chain", W25, 2 * CH_DIM, CH_DIM, CH_DIM, CH_WBOX);
   if (rc) return rc;
   ChainArgs a;
   memset(&a, 0, sizeof(a));
@@ -688,7 +660,7 @@ extern "C" int dpvo_update_neighbor_mlp(const void* net16_in, const int64_t* ind
   DPVO_REQUIRE(al16(net16_in) && al16(Wab) && al16(params) && al16(net32) && al16(net16_out), "update_neighbor_mlp: pointers must be 16-byte aligned");
   ChainMaps m;
   memset(&m, 0, sizeof(m));
-  int rc = ch_tmap(&m.W, Wab, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 2 * CH_DIM, CH_DIM, CH_DIM, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
+  int rc = encode_tmap_2d(&m.W, "update chain", Wab, 2 * CH_DIM, CH_DIM, CH_DIM, CH_WBOX);
   if (rc) return rc;
   m.X = m.W; m.W0 = m.W;
   ChainArgs a;
@@ -712,7 +684,7 @@ extern "C" int dpvo_update_gru_heads(float* net32, const void* hij16, const int3
   DPVO_REQUIRE(!coords || P >= 1, "update_gru_heads: patch size");
   ChainMaps m;
   memset(&m, 0, sizeof(m));
-  int rc = ch_tmap(&m.W, W6, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, 6 * CH_DIM, CH_DIM, CH_DIM, 64, CH_WBOX, CU_TENSOR_MAP_SWIZZLE_128B);
+  int rc = encode_tmap_2d(&m.W, "update chain", W6, 6 * CH_DIM, CH_DIM, CH_DIM, CH_WBOX);
   if (rc) return rc;
   m.X = m.W; m.W0 = m.W;
   ChainArgs a;

@@ -62,6 +62,10 @@ inline size_t dtype_size(int dtype) {
   return 0;
 }
 
+// every array of a workspace starts on a 256-byte boundary: round-up of sizes and of the workspace pointer
+inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
+inline char* align256(void* p) { return (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255); }
+
 // ---- scalar conversion ------------------------------------------------------------------
 template <typename T> struct acc_of { using type = float; };
 template <> struct acc_of<double> { using type = double; };

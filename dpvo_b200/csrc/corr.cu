@@ -18,6 +18,7 @@
 // Both fall back, per edge, to nine separate 8x8 boxes when the reprojected patch is stretched so
 // much that the union box would not fit -- results are exact in every case.
 #include "common.cuh"
+#include "tc.cuh"
 #include <algorithm>
 #include <cstdlib>
 
@@ -218,15 +219,6 @@ corr_fwd_generic(const CorrArgs a, int Cpad) {
 // ==========================================================================================
 // fp16 tensor-core path (mma.sync m16n8k16, fp32 accumulate)
 // ==========================================================================================
-__device__ __forceinline__ void mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2,
-                                         uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
-      "{%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
 __device__ __forceinline__ uint4 ldg128(const void* p) {
   uint4 r;
   asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];\n"
@@ -366,8 +358,8 @@ corr_fwd_mma(const CorrArgs a) {
           float acc0[4] = {0.f, 0.f, 0.f, 0.f}, acc1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
           for (int kb = 0; kb < 4; ++kb) {
-            mma16816(acc0, PA[kb].x, PB[kb].x, PA[kb].y, PB[kb].y, Q[kb].x, Q[kb].y);
-            mma16816(acc1, PA[kb].z, PB[kb].z, PA[kb].w, PB[kb].w, Q[kb].z, Q[kb].w);
+            mma_m16n8k16(acc0, PA[kb].x, PB[kb].x, PA[kb].y, PB[kb].y, Q[kb].x, Q[kb].y);
+            mma_m16n8k16(acc1, PA[kb].z, PB[kb].z, PA[kb].w, PB[kb].w, Q[kb].z, Q[kb].w);
           }
           // rows of the accumulator tile = patch pixels g (c0,c1) and 8 (c2,c3; g==0 lanes);
           // columns = box pixels nt*8 + 2t, +1: stored densely, no per-tap logic

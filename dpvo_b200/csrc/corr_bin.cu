@@ -20,6 +20,7 @@
 // 82 + 121 KB, and per SM sub-partition 3 x 64 + 3 x 104 registers per lane).
 // The bin order within a bin depends on atomic arrival order; every output depends on its own edge only.
 #include "common.cuh"
+#include "tc.cuh"
 
 namespace dpvo {
 
@@ -145,10 +146,6 @@ struct CbArgs {
   const int* order; const int4* items; const int* item_count;
 };
 
-__device__ __forceinline__ uint32_t cb_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void cb_cp_async16(uint32_t dst, const void* src, int bytes) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ uint4 cb_lds128(uint32_t a) {
   uint4 r;
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(a));
@@ -158,12 +155,6 @@ __device__ __forceinline__ uint4 cb_ldg128(const void* p) {
   uint4 r;
   asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];\n" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
   return r;
-}
-__device__ __forceinline__ void cb_mma16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
 // Region pixel q (row-major 16 x 16) holds its 16 channel chunks of 16 B with chunk c stored at position c ^ 4 (q & 1):
@@ -176,7 +167,7 @@ corr_fwd_l1_tiles(const CbArgs a) {
   const int4 item = a.items[blockIdx.x];
   const int tiles = a.nty * a.ntx, t_in = item.x % tiles, slot = item.x / tiles;
   const int ry0 = (t_in / a.ntx) * CB_T1 - CB_APRON, rx0 = (t_in % a.ntx) * CB_T1 - CB_APRON;
-  const uint32_t region = cb_smem_u32(cb_smem), zero = region + CB_REGION_BYTES;
+  const uint32_t region = smem_u32(cb_smem), zero = region + CB_REGION_BYTES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   CbWarpSmem& sm = reinterpret_cast<CbWarpSmem*>(cb_smem + CB_REGION_BYTES + 256)[warp];
 
@@ -187,9 +178,9 @@ corr_fwd_l1_tiles(const CbArgs a) {
       const int y = ry0 + (q >> 4), x = rx0 + (q & 15);
       const bool in = (unsigned)y < (unsigned)a.H1 && (unsigned)x < (unsigned)a.W1;
       const __half* src = in ? f2 + (int64_t)y * a.sy + (int64_t)x * a.sx + c * 8 : f2;
-      cb_cp_async16(region + q * 256 + ((c ^ ((q & 1) << 2)) << 4), src, in ? 16 : 0);
+      cp_async16(region + q * 256 + ((c ^ ((q & 1) << 2)) << 4), src, in ? 16 : 0);
     }
-    asm volatile("cp.async.commit_group;\n" ::: "memory");
+    cp_async_commit();
     if (threadIdx.x < 16) asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};\n" ::"r"(zero + threadIdx.x * 16), "r"(0u) : "memory");
   }
 
@@ -216,7 +207,7 @@ corr_fwd_l1_tiles(const CbArgs a) {
     if (lane < 9) { cx = a.coords[(int64_t)e * 18 + lane]; cy = a.coords[(int64_t)e * 18 + 9 + lane]; }
   };
   if (warp < item.z) fetch(0);
-  asm volatile("cp.async.wait_group 0;\n" ::: "memory");
+  cp_async_wait<0>();
   __syncthreads();
 
   for (int j = warp, k = 0; j < item.z; j += CB_WARPS, ++k) {
@@ -252,8 +243,8 @@ corr_fwd_l1_tiles(const CbArgs a) {
       float acc0[4] = {0.f, 0.f, 0.f, 0.f}, acc1[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
       for (int kb = 0; kb < 4; ++kb) {
-        cb_mma16816(acc0, PA[kb].x, PB[kb].x, PA[kb].y, PB[kb].y, Q[kb].x, Q[kb].y);
-        cb_mma16816(acc1, PA[kb].z, PB[kb].z, PA[kb].w, PB[kb].w, Q[kb].z, Q[kb].w);
+        mma_m16n8k16(acc0, PA[kb].x, PB[kb].x, PA[kb].y, PB[kb].y, Q[kb].x, Q[kb].y);
+        mma_m16n8k16(acc1, PA[kb].z, PB[kb].z, PA[kb].w, PB[kb].w, Q[kb].z, Q[kb].w);
       }
       const int col = nt * 8 + 2 * t;
       *reinterpret_cast<float2*>(&sm.raw[g * CB_RAWP + col + (g & 1)]) = make_float2(acc0[0] + acc1[0], acc0[1] + acc1[1]);

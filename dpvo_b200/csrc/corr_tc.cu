@@ -21,7 +21,6 @@
 // stage per warpgroup, refilled as soon as its MMAs have retired, keeps TMA, tensor pipe and the blends overlapped.
 #include "common.cuh"
 #include "tc.cuh"
-#include <cuda.h>
 #include <cstring>
 
 namespace dpvo {
@@ -65,38 +64,12 @@ struct TcBars {
   uint64_t full[TC_STAGES], empty[TC_STAGES];
 };
 
-__device__ __forceinline__ uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void tc_mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(tc_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void tc_mbar_arrive(uint64_t* bar) {
-  asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.shared::cta.b64 st, [%0];\n}\n" ::"r"(tc_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}\n" ::"r"(tc_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n.reg .pred p;\nWAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}\n" ::"r"(tc_smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tc_tma_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];\n" ::"r"(dst),
-               "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(tc_smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_tma_2d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
-               "l"(tmap), "r"(c0), "r"(c1), "r"(tc_smem_u32(bar))
-               : "memory");
-}
 // 64 registers: with those, one CTA of corr_fwd_l1_tiles (corr_bin.cu) fits beside this one on every SM
 __global__ void __maxnreg__(64)
 corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
   extern __shared__ unsigned char tc_smem_raw[];
   // 1024-byte alignment by pointer arithmetic on the shared array (keeps LDS/STS; an integer round trip gives generic LD/ST)
-  unsigned char* base = tc_smem_raw + ((1024u - (tc_smem_u32(tc_smem_raw) & 1023u)) & 1023u);
+  unsigned char* base = tc_smem_raw + ((1024u - (smem_u32(tc_smem_raw) & 1023u)) & 1023u);
   unsigned char* stages = base;                                        // [TC_STAGES][TC_STAGE_BYTES]
   float* raw = reinterpret_cast<float*>(base + TC_STAGES * TC_STAGE_BYTES);      // [TC_NG][9][TC_RAWP]
   TcMeta* meta = reinterpret_cast<TcMeta*>(raw + TC_RAW_FLOATS);
@@ -105,8 +78,8 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     // a stage is handed back by lane 0 of each of the four warps of the consuming warpgroup
-    for (int s = 0; s < TC_STAGES; ++s) { tc_mbar_init(&bars->full[s], 1); tc_mbar_init(&bars->empty[s], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&bars->full[s], 1); mbar_init(&bars->empty[s], 4); }
+    mbar_init_fence();
   }
   __syncthreads();
   const int n = *a.count;
@@ -153,17 +126,17 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
       const int bh = min(__reduce_max_sync(0xffffffffu, px ? ay : -(1 << 28)) - by, 64) + 8;
       if (lane == 0) *reinterpret_cast<int4*>(&mt) = make_int4(bx, by, bw, e);
       __syncwarp();
-      tc_mbar_wait(&bars->empty[s], ph ^ 1);
+      mbar_wait(&bars->empty[s], ph ^ 1);
       if (lane == 0) {
-        const uint32_t w0a = tc_smem_u32(stages + (size_t)s * TC_STAGE_BYTES), pa = w0a + 2 * TC_WIN0_BYTES;
-        tc_mbar_expect_tx(&bars->full[s], 2 * 128 * bw * bh + 2 * TC_PAT_TX);
+        const uint32_t w0a = smem_u32(stages + (size_t)s * TC_STAGE_BYTES), pa = w0a + 2 * TC_WIN0_BYTES;
+        mbar_arrive_expect_tx(&bars->full[s], 2 * 128 * bw * bh + 2 * TC_PAT_TX);
         // clamp wild origins so the coordinates stay in int32 range; such boxes are entirely out of bounds
         const int x0 = max(min(bx, 1 << 20), -(1 << 20)), y0 = max(min(by, 1 << 20), -(1 << 20));
         const CUtensorMap* m0 = &maps.l0[(bw - 8) * TC_L0_SHAPES + (bh - 8)];
-        tc_tma_4d(w0a, m0, 0, x0, y0, slot, &bars->full[s]);
-        tc_tma_4d(w0a + TC_WIN0_BYTES, m0, 64, x0, y0, slot, &bars->full[s]);
-        tc_tma_2d(pa, &maps.pat, 0, prow, &bars->full[s]);
-        tc_tma_2d(pa + TC_PAT_BYTES, &maps.pat, 64, prow, &bars->full[s]);
+        tma_load_4d(w0a, m0, 0, x0, y0, slot, &bars->full[s]);
+        tma_load_4d(w0a + TC_WIN0_BYTES, m0, 64, x0, y0, slot, &bars->full[s]);
+        tma_load_2d(pa, &maps.pat, 0, prow, &bars->full[s]);
+        tma_load_2d(pa + TC_PAT_BYTES, &maps.pat, 64, prow, &bars->full[s]);
       }
       __syncwarp();
       c0 = c1; i0 = i1; c1 = c2; i1 = i2;
@@ -194,11 +167,11 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
       const int ax = safe_floor_int(x) - 3, ay = safe_floor_int(y) - 3;
       const float fx = x - floorf(x), fy = y - floorf(y);
       const float4 w = make_float4((1.f - fx) * (1.f - fy), fx * (1.f - fy), (1.f - fx) * fy, fx * fy);
-      tc_mbar_wait(&bars->full[s], ph);
+      mbar_wait(&bars->full[s], ph);
       const int4 box = *reinterpret_cast<const int4*>(&mt);             // bx by pitch edge
       float acc[2][8];                                // [rows 0-63 | 64-127][fragment]
       {
-        const uint32_t wa = tc_smem_u32(stages + (size_t)s * TC_STAGE_BYTES);
+        const uint32_t wa = smem_u32(stages + (size_t)s * TC_STAGE_BYTES);
         const uint32_t pa = wa + 2 * TC_WIN0_BYTES;
         wgmma_fence();
 #pragma unroll
@@ -216,7 +189,7 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
 #pragma unroll
         for (int rh = 0; rh < 2; ++rh) wgmma_fence_regs(acc[rh]);
         __syncwarp();
-        if (lane == 0) tc_mbar_arrive(&bars->empty[s]);
+        if (lane == 0) mbar_arrive(&bars->empty[s]);
       }
       // transpose: raw[p][r]   (rows past the box are padding); fragment i of row half rh: box pixel
       // r = 64 rh + 16 wq + lane / 4 + 8 ((i / 2) % 2), patch pixel 8 (i / 4) + 2 (lane % 4) + i % 2
@@ -228,7 +201,7 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
           const int pp = 8 * (k >> 2) + 2 * (lane & 3) + (k & 1);
           if (pp < 9) rw[pp * TC_RAWP + r] = acc[rh][k];
         }
-      asm volatile("bar.sync %0, 128;\n" ::"r"(1 + eg) : "memory");
+      named_bar_sync(1 + eg, 128);
       if (et < 126) {
         __half* orow = a.out + (int64_t)box.w * a.out_row;       // even halves: level 0 of each pair
         const int p0 = box.z;
@@ -247,24 +220,10 @@ corr_fwd_tc(const __grid_constant__ TcMaps maps, const TcArgs a) {
           }
         }
       }
-      asm volatile("bar.sync %0, 128;\n" ::"r"(1 + eg) : "memory");   // tile free for this group's next edge
+      named_bar_sync(1 + eg, 128);   // tile free for this group's next edge
     }
   }
 
-}
-
-typedef CUresult (*TcEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static TcEncodeFn tc_encode() {
-  static TcEncodeFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (TcEncodeFn)p;
-  }
-  return fn;
 }
 
 // corr.cu: the mma.sync kernel run over a device-side list of edges
@@ -321,8 +280,7 @@ struct TcMapCache {
   TcMaps maps;
 };
 
-static bool tc_build_maps(TcEncodeFn enc, TcMaps& m, const void* fmap1, int S1, const void* l0, const int64_t* s20, int H0, int W0,
-                          int S2) {
+static int tc_build_maps(TcMaps& m, const void* fmap1, int S1, const void* l0, const int64_t* s20, int H0, int W0, int S2) {
   memset(&m, 0, sizeof(m));
   for (int i = 0; i < TC_L0_SHAPES; ++i)
     for (int j = 0; j < TC_L0_SHAPES; ++j) {
@@ -330,18 +288,9 @@ static bool tc_build_maps(TcEncodeFn enc, TcMaps& m, const void* fmap1, int S1, 
       cuuint64_t dims[4] = {128, (cuuint64_t)W0, (cuuint64_t)H0, (cuuint64_t)S2};
       cuuint64_t strides[3] = {(cuuint64_t)s20[4] * 2, (cuuint64_t)s20[3] * 2, (cuuint64_t)s20[1] * 2};
       cuuint32_t box[4] = {64, (cuuint32_t)(8 + i), (cuuint32_t)(8 + j), 1};
-      cuuint32_t es[4] = {1, 1, 1, 1};
-      if (enc(&m.l0[i * TC_L0_SHAPES + j], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(l0), dims, strides, box, es,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return false;
+      if (int rc = encode_tmap(&m.l0[i * TC_L0_SHAPES + j], "corr_tc", 4, l0, dims, strides, box)) return rc;
     }
-  cuuint64_t dims[2] = {128, (cuuint64_t)S1 * 9};
-  cuuint64_t strides[1] = {256};
-  cuuint32_t box[2] = {64, 9};
-  cuuint32_t es[2] = {1, 1};
-  return enc(&m.pat, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(fmap1), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  return encode_tmap_2d(&m.pat, "corr_tc", fmap1, (int64_t)S1 * 9, 128, 128, 9);
 }
 
 // Both levels of the correlation: binning and level 1 (corr_bin.cu), level 0 here, stretched edges on the mma.sync
@@ -355,8 +304,6 @@ int corr_tc_forward(const void* fmap1, const int64_t* s1, int S1, const void* l0
   if (s20[2] != 1 || s21[2] != 1 || s1[2] != 1 || s1[4] != 128 || s1[3] != 384 || s1[1] != 1152) return DPVO_ERR_UNSUPPORTED;
   if (((uintptr_t)fmap1 & 15) || ((uintptr_t)l0 & 15) || ((uintptr_t)l1 & 15) || ((uintptr_t)out & 3)) return DPVO_ERR_UNSUPPORTED;
   for (int d = 1; d < 5; ++d) if (d != 2 && ((s20[d] % 8) || (s21[d] % 8))) return DPVO_ERR_UNSUPPORTED;
-  TcEncodeFn enc = tc_encode();
-  if (!enc) return DPVO_ERR_UNSUPPORTED;
   static thread_local TcMapCache cache;
   TcMapKey key;
   memset(&key, 0, sizeof(key));
@@ -365,7 +312,7 @@ int corr_tc_forward(const void* fmap1, const int64_t* s1, int S1, const void* l0
   key.dims[0] = S1; key.dims[1] = S2; key.dims[2] = H0; key.dims[3] = W0;
   if (!cache.valid || memcmp(&cache.key, &key, sizeof(key)) != 0) {
     cache.valid = false;
-    if (!tc_build_maps(enc, cache.maps, fmap1, S1, l0, s20, H0, W0, S2)) return DPVO_ERR_UNSUPPORTED;
+    if (tc_build_maps(cache.maps, fmap1, S1, l0, s20, H0, W0, S2)) return DPVO_ERR_UNSUPPORTED;
     cache.key = key;
     cache.valid = true;
   }

@@ -27,6 +27,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "tc.cuh"
 
 namespace dpvo {
 
@@ -84,17 +85,9 @@ __device__ __forceinline__ T* img_ptr(T* q, int64_t bytes) {
   return q == nullptr ? q : reinterpret_cast<T*>(reinterpret_cast<Byte*>(q) + bytes);
 }
 
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
                : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-
-__device__ __forceinline__ void mma16816(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 // the normalised image value of dpvo.py:389 as the fp16 operand of the stem
@@ -239,7 +232,7 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) acc[mt][nb][j] = 0.f;
 
-  const uint32_t a_base = smem_addr(As), w_base = smem_addr(Ws);
+  const uint32_t a_base = smem_u32(As), w_base = smem_u32(Ws);
   const int lr = lane & 15, lk = lane >> 4;                              // A: row of the fragment, chunk half
   const int bn = (lane & 7) + ((lane >> 4) << 3), bk = (lane >> 3) & 1;  // B: channel within 16, chunk half
 #pragma unroll 1
@@ -262,8 +255,8 @@ enc_conv_kernel(const __grid_constant__ EncConvParams p, const int cout) {
         ldsm_x4(w_base + ((tap * C::KC + kc + bk) * NT + np * 16 + bn) * 16, b0, b1, b2, b3);
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
-          mma16816(acc[mt][2 * np], a[mt], b0, b1);
-          mma16816(acc[mt][2 * np + 1], a[mt], b2, b3);
+          mma_m16n8k16(acc[mt][2 * np], a[mt][0], a[mt][1], a[mt][2], a[mt][3], b0, b1);
+          mma_m16n8k16(acc[mt][2 * np + 1], a[mt][0], a[mt][1], a[mt][2], a[mt][3], b2, b3);
         }
       }
     }
@@ -639,17 +632,16 @@ FrameLayout frame_layout(int H, int W) {
   FrameLayout L{};
   L.H1 = out_size(H, 7, 2); L.W1 = out_size(W, 7, 2);
   L.H2 = out_size(L.H1, 3, 2); L.W2 = out_size(L.W1, 3, 2);
-  auto up = [](int64_t v) { return (v + 255) / 256 * 256; };
-  L.l1 = up((int64_t)L.H1 * L.W1 * 32 * 2);
-  L.l2 = up((int64_t)L.H2 * L.W2 * 64 * 2);
-  L.part = up(std::max(ntiles(L.H1, L.W1) * 3 * 32, ntiles(L.H2, L.W2) * 3 * 64) * (int64_t)sizeof(float));
+  L.l1 = align256((int64_t)L.H1 * L.W1 * 32 * 2);
+  L.l2 = align256((int64_t)L.H2 * L.W2 * 64 * 2);
+  L.part = align256(std::max(ntiles(L.H1, L.W1) * 3 * 32, ntiles(L.H2, L.W2) * 3 * 64) * (int64_t)sizeof(float));
   int64_t o = 0;
   for (int e = 0; e < 2; ++e) {
     for (int i = 0; i < 4; ++i) { L.x[e][i] = o; o += L.l1; }
     for (int i = 0; i < 4; ++i) { L.y[e][i] = o; o += L.l2; }
   }
   L.parts = o; o += 2 * L.part;
-  L.stats = o; o += up(2 * EC_NLAYERS * 2 * 64 * sizeof(float));
+  L.stats = o; o += align256(2 * EC_NLAYERS * 2 * 64 * sizeof(float));
   L.tickets = o; o += 256;
   L.bytes = o;
   return L;

@@ -13,7 +13,6 @@
 // The weights (<= 0.7 MB per layer) stay L2 resident; X is read once per 192-column slice.
 #include "common.cuh"
 #include "tc.cuh"
-#include <cuda.h>          // CUtensorMap types only; the encoder is fetched from the driver at run time
 
 namespace dpvo {
 
@@ -76,7 +75,7 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     for (int s = 0; s < GM_STAGES; ++s) { mbar_init(&bars->full[s], GATHER ? GM_PROD_THREADS : 1); mbar_init(&bars->empty[s], GM_CONS_WARPS); }
     mbar_init(&bars->wfull, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    mbar_init_fence();
   }
   __syncthreads();
 
@@ -246,36 +245,6 @@ linear_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
 using namespace dpvo;
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn encode_tiled() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
-  }
-  return fn;
-}
-
-// row-major fp16 [rows, cols] with row stride ld (elements) -> tiles of box_rows x 64 columns, 128-byte swizzle
-static int make_tmap(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
-  EncodeTiledFn fn = encode_tiled();
-  if (!fn) { set_error("linear_f16: cuTensorMapEncodeTiled is not available from the driver"); return DPVO_ERR_CUDA; }
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)GM_K, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("linear_f16: cuTensorMapEncodeTiled failed (%d)", (int)r); return DPVO_ERR_CUDA; }
-  return DPVO_OK;
-}
-
 struct GemmMaps { CUtensorMap A, B; };
 
 template <bool GATHER, bool WS, int EPI, int OUT>
@@ -319,10 +288,10 @@ static int linear_launch(GemmArgs& a, cudaStream_t st) {
   if (ws) grid = std::max<int64_t>(n_tiles_n, grid / n_tiles_n * n_tiles_n);
   GemmMaps m;
   memset(&m, 0, sizeof(m));
-  int rc = make_tmap(&m.B, a.W, a.N, a.K, a.ldw, GM_N);
+  int rc = encode_tmap_2d(&m.B, "linear_f16", a.W, a.N, a.K, a.ldw, GM_N);
   if (rc) return rc;
   if (a.gather) return ws ? launch_variant<true, true>(m, a, (unsigned)grid, st) : launch_variant<true, false>(m, a, (unsigned)grid, st);
-  rc = make_tmap(&m.A, a.X, a.rows, a.K, a.ldx, GM_M);
+  rc = encode_tmap_2d(&m.A, "linear_f16", a.X, a.rows, a.K, a.ldx, GM_M);
   if (rc) return rc;
   return ws ? launch_variant<false, true>(m, a, (unsigned)grid, st) : launch_variant<false, false>(m, a, (unsigned)grid, st);
 }

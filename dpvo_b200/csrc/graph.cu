@@ -316,8 +316,6 @@ __global__ void neighbors_kernel(const int32_t* __restrict__ order, const int32_
   }
 }
 
-static inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 static int64_t group_ws_bytes(int64_t E) {
   const int64_t ntiles = (E + G_TILE - 1) / G_TILE;
   return align256(sizeof(GroupHeader)) + 2 * align256(E * 4) + align256(ntiles * (int64_t)G_BINS * 4) + align256((ntiles + 1) * 4);

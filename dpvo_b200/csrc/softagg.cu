@@ -78,7 +78,7 @@ softagg_fused_kernel(const __half* __restrict__ X, int64_t ldx, const int32_t* _
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < SF_STAGES; ++s) { mbar_init(&full[s], SF_PROD_THREADS); mbar_init(&full[SF_STAGES + s], SF_PROD_THREADS); mbar_init(&empty[s], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    mbar_init_fence();
   }
   __syncthreads();
 

@@ -1,6 +1,9 @@
-// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (gemm.cu, chain.cu, corr_tc.cu).
+// The one home of the inline-PTX wrappers of the kernels: shared-memory addresses, mbarriers, TMA and 1-D bulk copies,
+// cp.async, named barriers, mma.sync and wgmma, used by chain.cu, gemm.cu, softagg.cu, corr.cu, corr_bin.cu,
+// corr_tc.cu, encoder.cu and update_ops.cu.  Also declares the host-side tensor-map encoder (common.cu).
 #pragma once
 #include "common.cuh"
+#include <cuda.h>          // CUtensorMap types only; the encoder is fetched from the driver at run time
 
 namespace dpvo {
 
@@ -9,18 +12,22 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)_
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count));
 }
+// makes the initialised mbarriers visible to the async proxy (TMA, bulk copies) and to the other CTAs of the cluster
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.shared::cta.b64 st, [%0];\n}\n" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}\n" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+// also takes the barrier's shared-memory address (smem_u32), for callers that keep it in a register
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
       "{\n.reg .pred p;\nWAIT_%=:\n"
       "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
+      "@p bra DONE_%=;\nbra WAIT_%=;\nDONE_%=:\n}\n" ::"r"(bar), "r"(parity) : "memory");
 }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 // bounded wait: a broken hand-shake traps (launch failure) instead of hanging the device.  try_wait suspends the
 // thread for a hardware-defined interval per attempt, so the bound is tens of milliseconds at the very least.  No
 // printf here: a function call between wgmma instructions would serialise the MMA pipeline of the caller.
@@ -46,6 +53,19 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
                "l"(tmap), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+               : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, int c0, int c1, int c2, int c3, uint64_t* bar) {
+  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];\n" ::"r"(dst),
+               "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(smem_u32(bar))
+               : "memory");
+}
+// 1-D bulk copy of `bytes` (a multiple of 16) global -> shared, completion signalled on the mbarrier at shared-memory
+// address bar: a caller that issues several copies per barrier, from several lanes, then keeps one 32-bit register
+// live rather than a 64-bit generic pointer
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(dst), "l"(src),
+               "r"(bytes), "r"(bar)
                : "memory");
 }
 // 2-D TMA tile load multicast to the CTAs of the cluster in cta_mask: the tile lands at the same shared-memory offset in
@@ -75,6 +95,12 @@ __device__ __forceinline__ void tma_store_2d(const void* tmap, int c0, int c1, u
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;\n" ::"n"(N) : "memory"); }
+// ---- warp MMA (mma.sync): D[16x8] += A[16x16] B[16x8], fp16 operands, fp32 accumulate -----------------------
+__device__ __forceinline__ void mma_m16n8k16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
 // ---- warpgroup MMA (wgmma, sm_90a) ------------------------------------------------------------
 // A warpgroup (four consecutive warps, the first a multiple of four) issues the MMA collectively; the fp32
 // accumulator of an m64nN tile lives in its registers: thread (warp w of the group, lane l) holds rows
@@ -110,5 +136,19 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory"); }
+
+// ---- host: tensor maps ---------------------------------------------------------------------------------------
+// Encodes a TMA descriptor of an fp16 tensor of `rank` dimensions, innermost first (byte strides of dimensions 1 ..
+// rank - 1), loaded in boxes of box[] elements with the 128-byte swizzle; unit element strides, 256-byte L2
+// promotion, out-of-bounds elements read as zero.  Returns DPVO_OK, or DPVO_ERR_CUDA with the error text prefixed by op.
+int encode_tmap(CUtensorMap* m, const char* op, int rank, const void* ptr, const cuuint64_t* dims, const cuuint64_t* strides,
+                const cuuint32_t* box);
+// row-major fp16 [rows, cols] with a row stride of ld elements, in boxes of box_rows rows x 64 columns (128 bytes)
+inline int encode_tmap_2d(CUtensorMap* m, const char* op, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  return encode_tmap(m, op, 2, ptr, dims, strides, box);
+}
 
 }  // namespace dpvo

@@ -13,6 +13,7 @@
 //   gated_residual       x + sigmoid(g) * r                              blocks.py:28-29
 //   heads                delta = Wd relu(net), weight = sigmoid(Ww relu(net))   net.py:62-71, 92
 #include "common.cuh"
+#include "tc.cuh"
 #include <cstdlib>
 #include <algorithm>
 
@@ -148,8 +149,6 @@ constexpr int LNB_STAGES = 4;
 constexpr int LNB_DIM = 384;
 constexpr size_t LNB_SMEM_CAP = 200 * 1024;
 
-__device__ __forceinline__ uint32_t lnb_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 // Block = ROW_WARPS consumer warps + one producer warp (its lane 0 issues the copies of the tile three iterations
 // ahead while the consumers normalise the current one).
 template <int DA, bool HAS_C>
@@ -170,9 +169,8 @@ add_layernorm_bulk_kernel(const void* a, const void* b, const __half* c, int db,
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t n_tiles = (rows + LNB_ROWS - 1) / LNB_ROWS;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < LNB_STAGES; ++i)
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(lnb_smem_u32(&full[i])), "r"(1));
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for (int i = 0; i < LNB_STAGES; ++i) mbar_init(&full[i], 1);
+    mbar_init_fence();
   }
   __syncthreads();
   // producer warp: lane 0 arms the barrier and copies the dense tiles of a and c with one bulk copy each; the rows
@@ -180,31 +178,21 @@ add_layernorm_bulk_kernel(const void* a, const void* b, const __half* c, int db,
   auto issue = [&](int64_t tile, int stage) {
     const int64_t r0 = tile * LNB_ROWS;
     const uint32_t nrow = (uint32_t)min((int64_t)LNB_ROWS, rows - r0);
-    const uint32_t bar = lnb_smem_u32(&full[stage]);
+    const uint32_t bar = smem_u32(&full[stage]);
     const uint32_t ba = nrow * LNB_DIM * ES, bc = HAS_C ? nrow * LNB_DIM * 2 : 0;
     const uint32_t brow = LNB_DIM * 2, bb = b ? nrow * brow : 0, bs = cs ? nrow * brow : 0;
     if (lane == 0) {
-      asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}\n" ::"r"(bar), "r"(ba + bc + bb + bs) : "memory");
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(lnb_smem_u32(sA + stage * A_BYTES)),
-                   "l"(reinterpret_cast<const unsigned char*>(a) + r0 * LNB_DIM * ES), "r"(ba), "r"(bar)
-                   : "memory");
-      if constexpr (HAS_C)
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(lnb_smem_u32(sC + stage * C_BYTES)),
-                     "l"(reinterpret_cast<const unsigned char*>(c) + r0 * LNB_DIM * 2), "r"(bc), "r"(bar)
-                     : "memory");
+      mbar_arrive_expect_tx(&full[stage], ba + bc + bb + bs);
+      bulk_load(smem_u32(sA + stage * A_BYTES), reinterpret_cast<const unsigned char*>(a) + r0 * LNB_DIM * ES, ba, bar);
+      if constexpr (HAS_C) bulk_load(smem_u32(sC + stage * C_BYTES), reinterpret_cast<const unsigned char*>(c) + r0 * LNB_DIM * 2, bc, bar);
     }
     if ((uint32_t)lane < nrow) {
       const uint32_t q = (uint32_t)lane;
       if (b) {
         const int64_t src = b_index ? b_index[r0 + q] : r0 + q;
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(lnb_smem_u32(sB + stage * R_BYTES + q * brow)),
-                     "l"(reinterpret_cast<const unsigned char*>(b) + src * brow), "r"(brow), "r"(bar)
-                     : "memory");
+        bulk_load(smem_u32(sB + stage * R_BYTES + q * brow), reinterpret_cast<const unsigned char*>(b) + src * brow, brow, bar);
       }
-      if (cs)
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(lnb_smem_u32(sS + stage * R_BYTES + q * brow)),
-                     "l"(reinterpret_cast<const unsigned char*>(cs) + (r0 + q) * ld_cs * 2), "r"(brow), "r"(bar)
-                     : "memory");
+      if (cs) bulk_load(smem_u32(sS + stage * R_BYTES + q * brow), reinterpret_cast<const unsigned char*>(cs) + (r0 + q) * ld_cs * 2, brow, bar);
     }
   };
   // gamma / beta of this lane's columns stay in registers
@@ -229,13 +217,7 @@ add_layernorm_bulk_kernel(const void* a, const void* b, const __half* c, int db,
       __syncthreads();
       continue;
     }
-    {
-      const uint32_t bar = lnb_smem_u32(&full[stage]), parity = (uint32_t)((it / LNB_STAGES) & 1);
-      asm volatile(
-          "{\n.reg .pred p;\nLNB_WAIT_%=:\n"
-          "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-          "@p bra LNB_DONE_%=;\nbra LNB_WAIT_%=;\nLNB_DONE_%=:\n}\n" ::"r"(bar), "r"(parity) : "memory");
-    }
+    mbar_wait(smem_u32(&full[stage]), (uint32_t)((it / LNB_STAGES) & 1));
     const unsigned char* ta = sA + stage * A_BYTES;
     const unsigned char* tc = sC + stage * C_BYTES;
     const unsigned char* tb = sB + stage * R_BYTES;
