@@ -38,14 +38,56 @@ int dt(const Tensor& t) {
   return -1;
 }
 
-void need_cuda(const Tensor& t, const char* name) {
-  TORCH_CHECK(t.is_cuda(), "dpvo_b200: ", name, " must be a CUDA tensor (this build has no CPU path)");
+const char* dtype_name(at::ScalarType st) {
+  switch (st) {
+    case at::kHalf: return "float16";
+    case at::kFloat: return "float32";
+    case at::kDouble: return "float64";
+    case at::kByte: return "uint8";
+    case at::kInt: return "int32";
+    case at::kLong: return "int64";
+    default: return c10::toString(st);
+  }
 }
 
-void* stream() { return (void*)at::cuda::getCurrentCUDAStream().stream(); }
+// The tensor contract of every entry point.  Each tensor argument, outputs and workspaces the caller passes included,
+// goes through one of these before the op allocates on the device or calls the library: it must be a CUDA tensor on
+// the device of the op's anchor tensor, the one its CUDAGuard selects.  A host tensor or one on another GPU is an error
+// here and never reaches a kernel.  Messages start with the op's name.
+constexpr at::ScalarType kAny = at::ScalarType::Undefined;
+struct Args {
+  const char* op;
+  c10::Device dev;
+  Args(const char* op, const Tensor& anchor, const char* what) : op(op), dev(anchor.device()) {
+    TORCH_CHECK(anchor.is_cuda(), op, ": ", what, " must be a CUDA tensor (this build has no CPU path)");
+  }
+  // any layout, of dtype st unless st is kAny
+  Tensor on(const Tensor& t, const char* what, at::ScalarType st = kAny) const {
+    TORCH_CHECK(t.is_cuda() && t.device() == dev, op, ": ", what, " must be a CUDA tensor on ", dev, " (this build has no CPU path)");
+    TORCH_CHECK(st == kAny || t.scalar_type() == st, op, ": ", what, " must be ", dtype_name(st), ", not ", dtype_name(t.scalar_type()));
+    return t;
+  }
+  // on(), contiguous, and of n elements unless n < 0
+  Tensor need(const Tensor& t, const char* what, at::ScalarType st = kAny, int64_t n = -1) const {
+    on(t, what, st);
+    TORCH_CHECK(t.is_contiguous(), op, ": ", what, " must be contiguous");
+    TORCH_CHECK(n < 0 || t.numel() == n, op, ": ", what, " must have ", n, " elements, not ", t.numel());
+    return t;
+  }
+  // on(), then converted to st (unless kAny) and made contiguous
+  Tensor as(const Tensor& t, const char* what, at::ScalarType st = kAny) const {
+    on(t, what);
+    return (st == kAny ? t : t.to(st)).contiguous();
+  }
+  // optional arguments: an undefined tensor when absent
+  Tensor on(const c10::optional<Tensor>& t, const char* what, at::ScalarType st = kAny) const { return t ? on(*t, what, st) : Tensor(); }
+  Tensor need(const c10::optional<Tensor>& t, const char* what, at::ScalarType st = kAny, int64_t n = -1) const {
+    return t ? need(*t, what, st, n) : Tensor();
+  }
+  Tensor as(const c10::optional<Tensor>& t, const char* what, at::ScalarType st = kAny) const { return t ? as(*t, what, st) : Tensor(); }
+};
 
-Tensor i64c(const Tensor& t) { return t.to(at::kLong).contiguous(); }
-Tensor f32c(const Tensor& t) { return t.to(at::kFloat).contiguous(); }
+void* stream() { return (void*)at::cuda::getCurrentCUDAStream().stream(); }
 
 std::vector<int64_t> strides5(const Tensor& t) {
   TORCH_CHECK(t.dim() == 5, "dpvo_b200: expected a 5-d tensor");
@@ -58,11 +100,11 @@ Tensor byte_ws(int64_t bytes, const Tensor& like) {
 
 // ------------------------------------------------------------------------------ cuda_corr
 std::vector<Tensor> corr_forward(Tensor fmap1, Tensor fmap2, Tensor coords, Tensor ii, Tensor jj, int radius) {
-  need_cuda(fmap1, "fmap1"); need_cuda(fmap2, "fmap2"); need_cuda(coords, "coords");
-  c10::cuda::CUDAGuard guard(fmap1.device());
-  TORCH_CHECK(fmap1.scalar_type() == fmap2.scalar_type(), "corr: fmap1/fmap2 dtype mismatch");
+  const Args arg("cuda_corr.forward", fmap1, "fmap1");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(fmap2, "fmap2", fmap1.scalar_type());
+  coords = arg.as(coords, "coords", at::kFloat); ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong);
   TORCH_CHECK(fmap1.dim() == 5 && fmap2.dim() == 5 && coords.dim() == 5, "corr: expected 5-d inputs");
-  coords = f32c(coords); ii = i64c(ii); jj = i64c(jj);
   const int B = coords.size(0), M = coords.size(1), P = coords.size(3);
   const int C = fmap1.size(2), O = 2 * radius + 1;
   TORCH_CHECK(coords.size(2) == 2 && coords.size(4) == P, "corr: coords must be [B,M,2,P,P]");
@@ -78,10 +120,11 @@ std::vector<Tensor> corr_forward(Tensor fmap1, Tensor fmap2, Tensor coords, Tens
 }
 
 std::vector<Tensor> corr_backward(Tensor fmap1, Tensor fmap2, Tensor coords, Tensor ii, Tensor jj, Tensor grad, int radius) {
-  need_cuda(fmap1, "fmap1"); need_cuda(fmap2, "fmap2"); need_cuda(grad, "corr_grad");
-  c10::cuda::CUDAGuard guard(fmap1.device());
-  coords = f32c(coords); ii = i64c(ii); jj = i64c(jj);
-  grad = grad.contiguous();
+  const Args arg("cuda_corr.backward", fmap1, "fmap1");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(fmap2, "fmap2");
+  coords = arg.as(coords, "coords", at::kFloat); ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong);
+  grad = arg.as(grad, "grad");
   const int B = coords.size(0), M = coords.size(1), P = coords.size(3), C = fmap1.size(2);
   Tensor g1 = torch::zeros_like(fmap1);
   Tensor g2 = torch::zeros_like(fmap2);
@@ -95,10 +138,10 @@ std::vector<Tensor> corr_backward(Tensor fmap1, Tensor fmap2, Tensor coords, Ten
 }
 
 std::vector<Tensor> patchify_forward(Tensor net, Tensor coords, int radius) {
-  need_cuda(net, "net"); need_cuda(coords, "coords");
-  c10::cuda::CUDAGuard guard(net.device());
+  const Args arg("cuda_corr.patchify_forward", net, "net");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  coords = arg.as(coords, "coords", at::kFloat);
   TORCH_CHECK(net.dim() == 4 && coords.dim() == 3 && coords.size(2) == 2, "patchify: net [B,C,H,W], coords [B,M,2]");
-  coords = f32c(coords);
   const int B = coords.size(0), M = coords.size(1), C = net.size(1), D = 2 * radius + 2;
   Tensor patches = torch::empty({B, M, C, D, D}, net.options());
   std::vector<int64_t> s = {net.stride(0), net.stride(1), net.stride(2), net.stride(3)};
@@ -109,10 +152,10 @@ std::vector<Tensor> patchify_forward(Tensor net, Tensor coords, int radius) {
 }
 
 std::vector<Tensor> patchify_backward(Tensor net, Tensor coords, Tensor gradient, int radius) {
-  need_cuda(net, "net"); need_cuda(gradient, "gradient");
-  c10::cuda::CUDAGuard guard(net.device());
-  coords = f32c(coords);
-  gradient = gradient.to(net.scalar_type()).contiguous();
+  const Args arg("cuda_corr.patchify_backward", net, "net");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  coords = arg.as(coords, "coords", at::kFloat);
+  gradient = arg.as(gradient, "gradient", net.scalar_type());
   const int B = coords.size(0), M = coords.size(1), C = net.size(1);
   Tensor g = torch::zeros(net.sizes(), net.options());
   check(dpvo_patchify_backward(gradient.data_ptr(), coords.data_ptr<float>(), g.data_ptr(), dt(net), B, M, C,
@@ -126,16 +169,16 @@ std::vector<Tensor> group_edges(Tensor key_a, c10::optional<Tensor> key_b, c10::
 std::vector<Tensor> ba_forward(Tensor poses, Tensor patches, Tensor intrinsics, Tensor target, Tensor weight,
                                Tensor lmbda, Tensor ii, Tensor jj, Tensor kk, int PPF, int t0, int t1,
                                int iterations, bool eff_impl) {
-  need_cuda(poses, "poses"); need_cuda(patches, "patches");
-  c10::cuda::CUDAGuard guard(poses.device());
-  TORCH_CHECK(poses.is_contiguous() && patches.is_contiguous(), "cuda_ba.forward updates poses/patches in place: they must be contiguous");
-  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat, "cuda_ba.forward: poses/patches must be float32");
+  // poses and patches are updated in place
+  const Args arg("cuda_ba.forward", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(poses, "poses", at::kFloat); arg.need(patches, "patches", at::kFloat);
   const int P = patches.size(-1);
-  intrinsics = f32c(intrinsics).view({-1, 4});
-  target = f32c(target).view({-1, 2});
-  weight = f32c(weight).view({-1, 2});
-  lmbda = f32c(lmbda).view({-1});
-  ii = i64c(ii); jj = i64c(jj); kk = i64c(kk);
+  intrinsics = arg.as(intrinsics, "intrinsics", at::kFloat).view({-1, 4});
+  target = arg.as(target, "target", at::kFloat).view({-1, 2});
+  weight = arg.as(weight, "weight", at::kFloat).view({-1, 2});
+  lmbda = arg.as(lmbda, "lmbda", at::kFloat).view({-1});
+  ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong); kk = arg.as(kk, "kk", at::kLong);
   const int64_t E = ii.numel();
   TORCH_CHECK(jj.numel() == E && kk.numel() == E && target.size(0) == E && weight.size(0) == E, "cuda_ba.forward: edge arrays disagree in length");
   const int64_t n_poses = poses.numel() / 7, n_patches = patches.numel() / (3 * P * P);
@@ -178,9 +221,9 @@ std::vector<Tensor> ba_forward(Tensor poses, Tensor patches, Tensor intrinsics, 
 }
 
 std::vector<Tensor> ba_neighbors(Tensor ii, Tensor jj) {
-  need_cuda(ii, "ii"); need_cuda(jj, "jj");
-  c10::cuda::CUDAGuard guard(ii.device());
-  ii = i64c(ii); jj = i64c(jj);
+  const Args arg("cuda_ba.neighbors", ii, "ii");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong);
   const int64_t E = ii.numel();
   TORCH_CHECK(jj.numel() == E, "cuda_ba.neighbors: length mismatch");
   Tensor ix = torch::empty({E}, ii.options()), jx = torch::empty({E}, ii.options());
@@ -192,33 +235,34 @@ std::vector<Tensor> ba_neighbors(Tensor ii, Tensor jj) {
   return {ix, jx};
 }
 
-Tensor reproject_impl(Tensor poses, Tensor patches, Tensor intrinsics, Tensor ii, Tensor jj, Tensor kk, int clamp) {
-  need_cuda(poses, "poses"); need_cuda(patches, "patches");
-  c10::cuda::CUDAGuard guard(poses.device());
+Tensor reproject_impl(Tensor poses, Tensor patches, Tensor intrinsics, Tensor ii, Tensor jj, Tensor kk, int clamp, const char* op) {
+  const Args arg(op, poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int P = patches.size(-1);
-  poses = f32c(poses); patches = f32c(patches); intrinsics = f32c(intrinsics);
-  ii = i64c(ii); jj = i64c(jj); kk = i64c(kk);
+  poses = arg.as(poses, "poses", at::kFloat); patches = arg.as(patches, "patches", at::kFloat);
+  intrinsics = arg.as(intrinsics, "intrinsics", at::kFloat);
+  ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong); kk = arg.as(kk, "kk", at::kLong);
   const int64_t E = ii.numel();
   Tensor coords = torch::empty({1, E, 2, P, P}, poses.options());
   check(dpvo_reproject(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(),
                        ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), coords.data_ptr<float>(), E, P,
                        clamp, stream()),
-        "cuda_ba.reproject");
+        op);
   return coords;
 }
 Tensor ba_reproject(Tensor poses, Tensor patches, Tensor intrinsics, Tensor ii, Tensor jj, Tensor kk) {
-  return reproject_impl(poses, patches, intrinsics, ii, jj, kk, 0);
+  return reproject_impl(poses, patches, intrinsics, ii, jj, kk, 0, "cuda_ba.reproject");
 }
 
 // cuda_ba.solve_system (ba.cpp:120-180): pose-graph Gauss-Newton step of the loop-closure back end.  The normal
 // equations are assembled on the device in fp64 (the reference: Eigen sparse, fp64, on the CPU); the leading
 // 7*freen block is solved by a dense Cholesky and the remaining poses get a zero step (ba.cpp:101-118).
 std::vector<Tensor> ba_solve_system(Tensor J_Ginv_i, Tensor J_Ginv_j, Tensor ii, Tensor jj, Tensor res, float ep, float lm, int freen) {
-  need_cuda(res, "res");
-  c10::cuda::CUDAGuard guard(res.device());
-  J_Ginv_i = f32c(J_Ginv_i.to(res.device())); J_Ginv_j = f32c(J_Ginv_j.to(res.device()));
-  ii = i64c(ii.to(res.device())); jj = i64c(jj.to(res.device()));
-  Tensor r32 = f32c(res).view({-1, 7});
+  const Args arg("cuda_ba.solve_system", res, "res");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  J_Ginv_i = arg.as(J_Ginv_i, "J_Ginv_i", at::kFloat); J_Ginv_j = arg.as(J_Ginv_j, "J_Ginv_j", at::kFloat);
+  ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong);
+  Tensor r32 = arg.as(res, "res", at::kFloat).view({-1, 7});
   const int64_t r = r32.size(0);
   TORCH_CHECK(J_Ginv_i.numel() == r * 49 && J_Ginv_j.numel() == r * 49 && ii.numel() == r && jj.numel() == r, "cuda_ba.solve_system: shape mismatch");
   TORCH_CHECK(r > 0, "cuda_ba.solve_system: no residuals");
@@ -239,8 +283,6 @@ std::vector<Tensor> ba_solve_system(Tensor J_Ginv_i, Tensor J_Ginv_j, Tensor ii,
 }
 
 // ------------------------------------------------------------------------ lietorch_backends
-#define CHECK_CONTIGUOUS(x) TORCH_CHECK(x.is_contiguous(), #x " must be contiguous")
-
 int emb_dim(int g) { return g == DPVO_SO3 ? 4 : g == DPVO_RXSO3 ? 5 : g == DPVO_SE3 ? 7 : 8; }
 int tan_dim(int g) { return g == DPVO_SO3 ? 3 : g == DPVO_RXSO3 ? 4 : g == DPVO_SE3 ? 6 : 7; }
 
@@ -250,32 +292,36 @@ typedef int (*unb_fn)(int, int, const void*, const void*, void*, int64_t, void*)
 typedef int (*binb_fn)(int, int, const void*, const void*, const void*, void*, void*, int64_t, void*);
 
 Tensor lie_unary(un_fn f, int g, Tensor x, int out_dim, const char* name) {
-  CHECK_CONTIGUOUS(x); need_cuda(x, name);
-  c10::cuda::CUDAGuard guard(x.device());
+  const Args arg(name, x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(x, "x");
   Tensor y = torch::empty({x.size(0), out_dim}, x.options());
   check(f(g, dt(x), x.data_ptr(), y.data_ptr(), x.size(0), stream()), name);
   return y;
 }
 Tensor lie_binary(bin_fn f, int g, Tensor x, Tensor y, int out_dim, const char* name) {
-  CHECK_CONTIGUOUS(x); CHECK_CONTIGUOUS(y); need_cuda(x, name);
-  c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.scalar_type() == y.scalar_type() && x.size(0) == y.size(0), name, ": operand mismatch");
+  const Args arg(name, x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(x, "x"); arg.need(y, "y", x.scalar_type());
+  TORCH_CHECK(x.size(0) == y.size(0), name, ": operand mismatch");
   Tensor z = torch::empty({x.size(0), out_dim}, x.options());
   check(f(g, dt(x), x.data_ptr(), y.data_ptr(), z.data_ptr(), x.size(0), stream()), name);
   return z;
 }
 std::vector<Tensor> lie_unary_bwd(unb_fn f, int g, Tensor grad, Tensor x, const char* name) {
-  CHECK_CONTIGUOUS(x); CHECK_CONTIGUOUS(grad); need_cuda(x, name);
-  c10::cuda::CUDAGuard guard(x.device());
-  grad = grad.to(x.scalar_type());
+  const Args arg(name, x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(x, "x");
+  grad = arg.need(grad, "grad").to(x.scalar_type());
   Tensor dx = torch::empty(x.sizes(), x.options());
   check(f(g, dt(x), grad.data_ptr(), x.data_ptr(), dx.data_ptr(), x.size(0), stream()), name);
   return {dx};
 }
 std::vector<Tensor> lie_binary_bwd(binb_fn f, int g, Tensor grad, Tensor x, Tensor y, const char* name) {
-  CHECK_CONTIGUOUS(x); CHECK_CONTIGUOUS(y); CHECK_CONTIGUOUS(grad); need_cuda(x, name);
-  c10::cuda::CUDAGuard guard(x.device());
-  grad = grad.to(x.scalar_type());
+  const Args arg(name, x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(x, "x"); arg.need(y, "y");
+  grad = arg.need(grad, "grad").to(x.scalar_type());
   Tensor dx = torch::empty(x.sizes(), x.options()), dy = torch::empty(y.sizes(), y.options());
   check(f(g, dt(x), grad.data_ptr(), x.data_ptr(), y.data_ptr(), dx.data_ptr(), dy.data_ptr(), x.size(0), stream()), name);
   return {dx, dy};
@@ -298,15 +344,17 @@ std::vector<Tensor> l_act_b(int g, Tensor grad, Tensor X, Tensor p) { return lie
 Tensor l_act4(int g, Tensor X, Tensor p) { return lie_binary(dpvo_lie_act4, g, X, p, 4, "lietorch_backends.act4"); }
 std::vector<Tensor> l_act4_b(int g, Tensor grad, Tensor X, Tensor p) { return lie_binary_bwd(dpvo_lie_act4_backward, g, grad, X, p, "lietorch_backends.act4_backward"); }
 Tensor l_as_matrix(int g, Tensor X) {
-  CHECK_CONTIGUOUS(X); need_cuda(X, "X");
-  c10::cuda::CUDAGuard guard(X.device());
+  const Args arg("lietorch_backends.as_matrix", X, "X");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(X, "X");
   Tensor T = torch::empty({X.size(0), 4, 4}, X.options());
   check(dpvo_lie_as_matrix(g, dt(X), X.data_ptr(), T.data_ptr(), X.size(0), stream()), "lietorch_backends.as_matrix");
   return T;
 }
 Tensor l_projector(int g, Tensor X) {
-  CHECK_CONTIGUOUS(X); need_cuda(X, "X");
-  c10::cuda::CUDAGuard guard(X.device());
+  const Args arg("lietorch_backends.projector", X, "X");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(X, "X");
   const int n = emb_dim(g);
   Tensor Pm = torch::empty({X.size(0), n, n}, X.options());
   check(dpvo_lie_projector(g, dt(X), X.data_ptr(), Pm.data_ptr(), X.size(0), stream()), "lietorch_backends.projector");
@@ -318,21 +366,18 @@ Tensor l_jinv(int g, Tensor X, Tensor a) { return lie_binary(dpvo_lie_jinv, g, X
 // DPVO.corr (dpvo.py:200-207) in one launch: returns [1, E, 882]-compatible [B,M,O,O,P,P,2]
 Tensor corr_pyramid2(Tensor fmap1, Tensor fmap2_l0, Tensor fmap2_l1, Tensor coords, Tensor ii, Tensor jj, int radius, double div, int64_t pad_to,
                      c10::optional<Tensor> out_buf) {
-  need_cuda(fmap1, "fmap1");
-  c10::cuda::CUDAGuard guard(fmap1.device());
-  coords = f32c(coords); ii = i64c(ii); jj = i64c(jj);
+  const Args arg("dpvo_b200_ext.corr_pyramid2", fmap1, "fmap1");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(fmap2_l0, "fmap2_l0"); arg.on(fmap2_l1, "fmap2_l1");
+  coords = arg.as(coords, "coords", at::kFloat); ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong);
   const int B = coords.size(0), M = coords.size(1), P = coords.size(3), C = fmap1.size(2), O = 2 * radius + 1;
   const int64_t feat = (int64_t)O * O * P * P * 2;
   const int64_t row = pad_to > feat ? pad_to : feat;
   // padded rows ([B, M, row], zero tail) feed the wgmma dense layer directly; unpadded keep the 7-d view
   // out_buf: a caller-owned [B, M, row] buffer whose padding columns are already zero (reused every update)
-  Tensor out;
-  if (out_buf.has_value()) {
-    out = *out_buf;
-    TORCH_CHECK(out.is_contiguous() && out.scalar_type() == fmap1.scalar_type() && out.numel() == (int64_t)B * M * row, "corr_pyramid2: out buffer must be contiguous [B, M, ", row, "]");
-  } else {
-    out = (row == feat) ? torch::empty({B, M, O, O, P, P, 2}, fmap1.options()) : torch::zeros({B, M, row}, fmap1.options());
-  }
+  Tensor out = arg.need(out_buf, "out", fmap1.scalar_type());
+  if (!out.defined()) out = (row == feat) ? torch::empty({B, M, O, O, P, P, 2}, fmap1.options()) : torch::zeros({B, M, row}, fmap1.options());
+  TORCH_CHECK(out.numel() == (int64_t)B * M * row, "corr_pyramid2: out buffer must be [B, M, ", row, "]");
   auto s1 = strides5(fmap1), s20 = strides5(fmap2_l0), s21 = strides5(fmap2_l1);
   const int64_t wsb = dpvo_corr_pyramid2_workspace_bytes(M);
   Tensor ws = torch::empty({wsb}, torch::dtype(torch::kUInt8).device(fmap1.device()));
@@ -347,13 +392,11 @@ Tensor corr_pyramid2(Tensor fmap1, Tensor fmap2_l0, Tensor fmap2_l1, Tensor coor
 
 // returns (order, group_of, group_start, key_a, key_b, n_groups) -- all device tensors
 std::vector<Tensor> group_edges(Tensor key_a, c10::optional<Tensor> key_b, c10::optional<Tensor> sec) {
-  need_cuda(key_a, "key_a");
-  c10::cuda::CUDAGuard guard(key_a.device());
-  key_a = i64c(key_a);
+  const Args arg("dpvo_b200_ext.group_edges", key_a, "key_a");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  key_a = arg.as(key_a, "key_a", at::kLong);
   const int64_t E = key_a.numel();
-  Tensor kb, sc;
-  if (key_b.has_value()) kb = i64c(*key_b);
-  if (sec.has_value()) sc = i64c(*sec);
+  Tensor kb = arg.as(key_b, "key_b", at::kLong), sc = arg.as(sec, "sec", at::kLong);
   auto oi = key_a.options().dtype(at::kInt);
   Tensor order = torch::empty({E}, oi), gof = torch::empty({E}, oi), gstart = torch::empty({E + 1}, oi);
   Tensor ka = torch::empty({E}, key_a.options()), kbo = torch::empty({E}, key_a.options()), ng = torch::empty({1}, oi);
@@ -370,16 +413,13 @@ std::vector<Tensor> group_edges(Tensor key_a, c10::optional<Tensor> key_b, c10::
 // both groupings of an update in one launch; returns the two 6-tuples of group_edges concatenated
 std::vector<Tensor> group_edges_pair(Tensor a0, c10::optional<Tensor> b0, c10::optional<Tensor> s0, Tensor a1, c10::optional<Tensor> b1,
                                      c10::optional<Tensor> s1) {
-  need_cuda(a0, "key_a0");
-  c10::cuda::CUDAGuard guard(a0.device());
-  a0 = i64c(a0); a1 = i64c(a1);
+  const Args arg("dpvo_b200_ext.group_edges_pair", a0, "key_a0");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  a0 = arg.as(a0, "key_a0", at::kLong); a1 = arg.as(a1, "key_a1", at::kLong);
   const int64_t E = a0.numel();
   TORCH_CHECK(a1.numel() == E, "group_edges_pair: both problems group the same edges");
-  Tensor kb[2], sc[2];
-  if (b0.has_value()) kb[0] = i64c(*b0);
-  if (s0.has_value()) sc[0] = i64c(*s0);
-  if (b1.has_value()) kb[1] = i64c(*b1);
-  if (s1.has_value()) sc[1] = i64c(*s1);
+  Tensor kb[2] = {arg.as(b0, "key_b0", at::kLong), arg.as(b1, "key_b1", at::kLong)};
+  Tensor sc[2] = {arg.as(s0, "sec0", at::kLong), arg.as(s1, "sec1", at::kLong)};
   auto oi = a0.options().dtype(at::kInt);
   const int64_t wsb = dpvo_group_workspace_bytes(E);
   std::vector<Tensor> out;
@@ -399,18 +439,30 @@ std::vector<Tensor> group_edges_pair(Tensor a0, c10::optional<Tensor> b0, c10::o
   return out;
 }
 
+// the operands of ba_forward_grouped / _batched: poses and patches are updated in place, the rest converted as read
+void ba_args(const Args& arg, const Tensor& poses, const Tensor& patches, Tensor& intrinsics, Tensor& target, Tensor& weight,
+             Tensor& lmbda, Tensor& ii, Tensor& jj, Tensor& kk, const Tensor& k_order, const Tensor& k_start, const Tensor& k_key,
+             const Tensor& k_n, const Tensor& p_order, const Tensor& p_start, const Tensor& p_key_i, const Tensor& p_key_j,
+             const Tensor& p_n) {
+  arg.need(poses, "poses", at::kFloat); arg.need(patches, "patches", at::kFloat);
+  intrinsics = arg.as(intrinsics, "intrinsics", at::kFloat); target = arg.as(target, "target", at::kFloat);
+  weight = arg.as(weight, "weight", at::kFloat); lmbda = arg.as(lmbda, "lmbda", at::kFloat);
+  ii = arg.as(ii, "ii", at::kLong); jj = arg.as(jj, "jj", at::kLong); kk = arg.as(kk, "kk", at::kLong);
+  arg.need(k_order, "k_order", at::kInt); arg.need(k_start, "k_start", at::kInt); arg.need(k_key, "k_key", at::kLong);
+  arg.need(k_n, "k_n", at::kInt); arg.need(p_order, "p_order", at::kInt); arg.need(p_start, "p_start", at::kInt);
+  arg.need(p_key_i, "p_key_i", at::kLong); arg.need(p_key_j, "p_key_j", at::kLong); arg.need(p_n, "p_n", at::kInt);
+}
+
 // fastba.BA on groupings built once per update (order, group_start, key_a[, key_b], n of EdgeGroups)
 void ba_forward_grouped(Tensor poses, Tensor patches, Tensor intrinsics, Tensor target, Tensor weight, Tensor lmbda,
                         Tensor ii, Tensor jj, Tensor kk, int t0, int t1, int iterations,
                         Tensor k_order, Tensor k_start, Tensor k_key, Tensor k_n,
                         Tensor p_order, Tensor p_start, Tensor p_key_i, Tensor p_key_j, Tensor p_n) {
-  need_cuda(poses, "poses"); need_cuda(patches, "patches");
-  c10::cuda::CUDAGuard guard(poses.device());
-  TORCH_CHECK(poses.is_contiguous() && patches.is_contiguous(), "ba_forward_grouped updates poses/patches in place: they must be contiguous");
-  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat, "ba_forward_grouped: poses/patches must be float32");
+  const Args arg("dpvo_b200_ext.ba_forward_grouped", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  ba_args(arg, poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, k_order, k_start, k_key, k_n, p_order, p_start,
+          p_key_i, p_key_j, p_n);
   const int P = patches.size(-1);
-  intrinsics = f32c(intrinsics); target = f32c(target); weight = f32c(weight); lmbda = f32c(lmbda);
-  ii = i64c(ii); jj = i64c(jj); kk = i64c(kk);
   const int64_t E = ii.numel();
   const int64_t wsb = dpvo_ba_grouped_workspace_bytes(E, t1 - t0);
   Tensor ws = byte_ws(wsb, poses);
@@ -428,10 +480,10 @@ void ba_forward_batched(Tensor poses, Tensor patches, Tensor intrinsics, Tensor 
                         Tensor ii, Tensor jj, Tensor kk, int64_t frames_per_stream, std::vector<int> t0, std::vector<int> t1,
                         int iterations, Tensor k_order, Tensor k_start, Tensor k_key, Tensor k_n,
                         Tensor p_order, Tensor p_start, Tensor p_key_i, Tensor p_key_j, Tensor p_n) {
-  need_cuda(poses, "poses"); need_cuda(patches, "patches");
-  c10::cuda::CUDAGuard guard(poses.device());
-  TORCH_CHECK(poses.is_contiguous() && patches.is_contiguous(), "ba_forward_batched updates poses/patches in place: they must be contiguous");
-  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat, "ba_forward_batched: poses/patches must be float32");
+  const Args arg("dpvo_b200_ext.ba_forward_batched", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  ba_args(arg, poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, k_order, k_start, k_key, k_n, p_order, p_start,
+          p_key_i, p_key_j, p_n);
   TORCH_CHECK(t0.size() == t1.size() && !t0.empty(), "ba_forward_batched: t0 and t1 need one entry per stream");
   const int B = (int)t0.size();
   const int64_t n_frames = poses.numel() / 7, n_patches = patches.numel() / (3 * patches.size(-1) * patches.size(-1));
@@ -440,8 +492,6 @@ void ba_forward_batched(Tensor poses, Tensor patches, Tensor intrinsics, Tensor 
               frames_per_stream, " frames with the same number of patches each");
   TORCH_CHECK(intrinsics.numel() == 4 * n_frames, "ba_forward_batched: intrinsics need one row per frame");
   const int P = patches.size(-1);
-  intrinsics = f32c(intrinsics); target = f32c(target); weight = f32c(weight); lmbda = f32c(lmbda);
-  ii = i64c(ii); jj = i64c(jj); kk = i64c(kk);
   const int64_t E = ii.numel();
   int max_n = 0;
   for (int b = 0; b < B; ++b) max_n = std::max(max_n, t1[b] - t0[b]);
@@ -462,7 +512,7 @@ int64_t ba_batched_workspace_bytes(int64_t E, int64_t B, int64_t max_free_poses)
 }
 
 Tensor reproject_clamped(Tensor poses, Tensor patches, Tensor intrinsics, Tensor ii, Tensor jj, Tensor kk) {
-  return reproject_impl(poses, patches, intrinsics, ii, jj, kk, 1);
+  return reproject_impl(poses, patches, intrinsics, ii, jj, kk, 1, "dpvo_b200_ext.reproject_clamped");
 }
 
 
@@ -475,22 +525,22 @@ int dt16or32(const Tensor& t) {
 std::vector<Tensor> add_layernorm(Tensor a, c10::optional<Tensor> b, c10::optional<Tensor> c, Tensor gamma, Tensor beta,
                                   double eps, bool relu, bool want32, bool want16, c10::optional<Tensor> b_index, bool inplace32,
                                   c10::optional<Tensor> c_scale) {
-  need_cuda(a, "a");
-  c10::cuda::CUDAGuard guard(a.device());
+  const Args arg("dpvo_b200_ext.add_layernorm", a, "a");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int dim = a.size(-1);
   const int64_t rows = a.numel() / dim;
-  a = a.contiguous();
-  Tensor bb, cc;
+  a = arg.as(a, "a");
+  Tensor bb = arg.as(b, "b"), cc = arg.as(c, "c"), bidx = arg.as(b_index, "b_index", at::kLong);
+  gamma = arg.as(gamma, "gamma", at::kFloat); beta = arg.as(beta, "beta", at::kFloat);
+  Tensor csc = arg.on(c_scale, "c_scale", at::kHalf);
   int dts[3] = {dt16or32(a), 0, 0};
-  Tensor bidx;
-  if (b_index.has_value()) { bidx = i64c(*b_index); TORCH_CHECK(bidx.numel() == rows, "add_layernorm: b_index length"); }
-  if (b.has_value()) { bb = b->contiguous(); dts[1] = dt16or32(bb); TORCH_CHECK(bidx.defined() || bb.numel() == a.numel(), "add_layernorm: shape mismatch"); }
-  if (c.has_value()) { cc = c->contiguous(); dts[2] = dt16or32(cc); TORCH_CHECK(cc.numel() == a.numel(), "add_layernorm: shape mismatch"); }
-  gamma = f32c(gamma); beta = f32c(beta);
-  Tensor csc; int64_t ld_cs = 0;
-  if (c_scale.has_value()) {
-    csc = c_scale->reshape({-1, dim});
-    TORCH_CHECK(csc.scalar_type() == at::kHalf && csc.stride(1) == 1 && csc.size(0) == rows && cc.defined(), "add_layernorm: c_scale must be fp16 [rows, dim] next to operand c");
+  if (bidx.defined()) TORCH_CHECK(bidx.numel() == rows, "add_layernorm: b_index length");
+  if (bb.defined()) { dts[1] = dt16or32(bb); TORCH_CHECK(bidx.defined() || bb.numel() == a.numel(), "add_layernorm: shape mismatch"); }
+  if (cc.defined()) { dts[2] = dt16or32(cc); TORCH_CHECK(cc.numel() == a.numel(), "add_layernorm: shape mismatch"); }
+  int64_t ld_cs = 0;
+  if (csc.defined()) {
+    csc = csc.reshape({-1, dim});
+    TORCH_CHECK(csc.stride(1) == 1 && csc.size(0) == rows && cc.defined(), "add_layernorm: c_scale must be fp16 [rows, dim] next to operand c");
     ld_cs = csc.stride(0);
   }
   Tensor y32, y16;
@@ -508,9 +558,9 @@ std::vector<Tensor> add_layernorm(Tensor a, c10::optional<Tensor> b, c10::option
 }
 
 Tensor gather_rows_masked(Tensor x, Tensor idx, bool half_out) {
-  need_cuda(x, "x");
-  c10::cuda::CUDAGuard guard(x.device());
-  x = x.contiguous(); idx = i64c(idx);
+  const Args arg("dpvo_b200_ext.gather_rows_masked", x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  x = arg.as(x, "x"); idx = arg.as(idx, "idx", at::kLong);
   const int dim = x.size(-1);
   const int64_t rows = idx.numel();
   Tensor y = torch::empty({1, rows, dim}, x.options().dtype(half_out ? at::kHalf : at::kFloat));
@@ -520,14 +570,14 @@ Tensor gather_rows_masked(Tensor x, Tensor idx, bool half_out) {
 }
 
 Tensor residual_add_(Tensor net32, Tensor u, c10::optional<Tensor> group_of, bool want16) {
-  need_cuda(net32, "net");
-  c10::cuda::CUDAGuard guard(net32.device());
-  TORCH_CHECK(net32.is_contiguous() && net32.scalar_type() == at::kFloat, "residual_add_: net must be contiguous float32");
-  u = u.contiguous();
+  const Args arg("dpvo_b200_ext.residual_add_", net32, "net");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(net32, "net", at::kFloat);
+  u = arg.as(u, "u");
+  Tensor gof = arg.as(group_of, "group_of", at::kInt), n16;
   const int dim = net32.size(-1);
   const int64_t rows = net32.numel() / dim;
-  Tensor gof, n16;
-  if (group_of.has_value()) { gof = group_of->to(at::kInt).contiguous(); TORCH_CHECK(gof.numel() == rows, "residual_add_: group_of length"); }
+  if (gof.defined()) { TORCH_CHECK(gof.numel() == rows, "residual_add_: group_of length"); }
   else TORCH_CHECK(u.numel() == net32.numel(), "residual_add_: shape mismatch");
   if (want16) n16 = torch::empty(net32.sizes(), net32.options().dtype(at::kHalf));
   check(dpvo_residual_add(net32.data_ptr(), u.data_ptr(), dt16or32(u), gof.defined() ? gof.data_ptr<int>() : nullptr,
@@ -538,14 +588,14 @@ Tensor residual_add_(Tensor net32, Tensor u, c10::optional<Tensor> group_of, boo
 
 // fp16( net32 + u[group_of] ) without updating net32
 Tensor residual_sum16(Tensor net32, Tensor u, c10::optional<Tensor> group_of) {
-  need_cuda(net32, "net");
-  c10::cuda::CUDAGuard guard(net32.device());
-  TORCH_CHECK(net32.is_contiguous() && net32.scalar_type() == at::kFloat, "residual_sum16: net must be contiguous float32");
-  u = u.contiguous();
+  const Args arg("dpvo_b200_ext.residual_sum16", net32, "net");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(net32, "net", at::kFloat);
+  u = arg.as(u, "u");
+  Tensor gof = arg.as(group_of, "group_of", at::kInt);
   const int dim = net32.size(-1);
   const int64_t rows = net32.numel() / dim;
-  Tensor gof;
-  if (group_of.has_value()) { gof = group_of->to(at::kInt).contiguous(); TORCH_CHECK(gof.numel() == rows, "residual_sum16: group_of length"); }
+  if (gof.defined()) { TORCH_CHECK(gof.numel() == rows, "residual_sum16: group_of length"); }
   else TORCH_CHECK(u.numel() == net32.numel(), "residual_sum16: shape mismatch");
   Tensor n16 = torch::empty(net32.sizes(), net32.options().dtype(at::kHalf));
   check(dpvo_residual_sum16(net32.data_ptr(), u.data_ptr(), dt16or32(u), gof.defined() ? gof.data_ptr<int>() : nullptr, n16.data_ptr(), rows, dim, stream()),
@@ -554,11 +604,10 @@ Tensor residual_sum16(Tensor net32, Tensor u, c10::optional<Tensor> group_of) {
 }
 
 std::vector<Tensor> gated_residual(Tensor x32, Tensor gate16, Tensor res16, bool want_relu16) {
-  need_cuda(x32, "x");
-  c10::cuda::CUDAGuard guard(x32.device());
-  TORCH_CHECK(x32.scalar_type() == at::kFloat && gate16.scalar_type() == at::kHalf && res16.scalar_type() == at::kHalf,
-              "gated_residual: expects (float32, float16, float16)");
-  x32 = x32.contiguous(); gate16 = gate16.contiguous(); res16 = res16.contiguous();
+  const Args arg("dpvo_b200_ext.gated_residual", x32, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  x32 = arg.on(x32, "x", at::kFloat).contiguous();
+  gate16 = arg.on(gate16, "gate", at::kHalf).contiguous(); res16 = arg.on(res16, "res", at::kHalf).contiguous();
   const int dim = x32.size(-1);
   const int64_t rows = x32.numel() / dim;
   Tensor y = torch::empty_like(x32), r16;
@@ -571,16 +620,16 @@ std::vector<Tensor> gated_residual(Tensor x32, Tensor gate16, Tensor res16, bool
 
 // fg: [.., E, 2*dim] fp16 = [f | g] (one GEMM with the f and g weights stacked)
 Tensor softagg_reduce(Tensor fg, Tensor order, Tensor group_start, Tensor n_groups, int64_t max_groups) {
-  need_cuda(fg, "fg");
-  c10::cuda::CUDAGuard guard(fg.device());
-  TORCH_CHECK(fg.scalar_type() == at::kHalf && fg.is_contiguous() && fg.size(-1) % 2 == 0, "softagg_reduce: expects contiguous float16 [E, 2*dim]");
+  const Args arg("dpvo_b200_ext.softagg_reduce", fg, "fg");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(fg, "fg", at::kHalf);
+  TORCH_CHECK(fg.size(-1) % 2 == 0, "softagg_reduce: expects [E, 2*dim]");
   const int dim = fg.size(-1) / 2;
   const int64_t E = fg.numel() / fg.size(-1);
-  TORCH_CHECK(order.is_cuda() && order.scalar_type() == at::kInt && order.is_contiguous() && order.numel() == E,
-              "softagg_reduce: order must be a contiguous int32 CUDA tensor with one entry per row of fg");
-  TORCH_CHECK(group_start.is_cuda() && group_start.scalar_type() == at::kInt && group_start.is_contiguous() && group_start.numel() >= max_groups + 1,
-              "softagg_reduce: group_start must be int32 with at least max_groups + 1 entries");
-  TORCH_CHECK(n_groups.is_cuda() && n_groups.scalar_type() == at::kInt && n_groups.numel() == 1, "softagg_reduce: n_groups must be a device int32 scalar");
+  arg.need(order, "order (one entry per row of fg)", at::kInt, E);
+  arg.need(group_start, "group_start", at::kInt);
+  arg.need(n_groups, "n_groups", at::kInt, 1);
+  TORCH_CHECK(group_start.numel() >= max_groups + 1, "softagg_reduce: group_start must have at least max_groups + 1 entries");
   TORCH_CHECK(max_groups >= 0 && max_groups <= E, "softagg_reduce: max_groups must be in [0, E]");
   Tensor y = torch::empty({1, max_groups, dim}, fg.options());   // rows past the group count are zeroed by the kernel itself
   const at::Half* base = fg.data_ptr<at::Half>();
@@ -593,26 +642,26 @@ Tensor softagg_reduce(Tensor fg, Tensor order, Tensor group_start, Tensor n_grou
 // x: [.., E, dim] fp16; w [2*dim, dim] fp16 / bias [2*dim] fp32 with the f and g rows interleaved by 96-channel slice
 Tensor softagg_fused(Tensor x, Tensor order, Tensor group_of, Tensor group_start, Tensor n_groups, int64_t max_groups, Tensor w,
                      Tensor bias, c10::optional<Tensor> workspace) {
-  need_cuda(x, "x");
-  c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.scalar_type() == at::kHalf && x.stride(-1) == 1, "softagg_fused: x must be float16 with contiguous rows");
+  const Args arg("dpvo_b200_ext.softagg_fused", x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(x, "x", at::kHalf);
+  TORCH_CHECK(x.stride(-1) == 1, "softagg_fused: x must have contiguous rows");
   const int dim = x.size(-1);
   Tensor x2 = x.dim() == 2 ? x : x.reshape({-1, dim});
   const int64_t E = x2.size(0);
-  TORCH_CHECK(w.is_cuda() && w.scalar_type() == at::kHalf && w.is_contiguous() && w.dim() == 2 && w.size(0) == 2 * dim && w.size(1) == dim,
-              "softagg_fused: w must be a contiguous float16 CUDA tensor [2*dim, dim]");
-  TORCH_CHECK(bias.is_cuda() && bias.scalar_type() == at::kFloat && bias.is_contiguous() && bias.numel() == 2 * dim,
-              "softagg_fused: bias must be a contiguous float32 CUDA tensor [2*dim]");
-  for (const Tensor* t : {&order, &group_of})
-    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kInt && t->is_contiguous() && t->numel() == E,
-                "softagg_fused: order and group_of must be contiguous int32 CUDA tensors with one entry per row of x");
-  TORCH_CHECK(group_start.is_cuda() && group_start.scalar_type() == at::kInt && group_start.is_contiguous() && group_start.numel() >= max_groups + 1,
-              "softagg_fused: group_start must be int32 with at least max_groups + 1 entries");
-  TORCH_CHECK(n_groups.is_cuda() && n_groups.scalar_type() == at::kInt && n_groups.numel() == 1, "softagg_fused: n_groups must be a device int32 scalar");
+  arg.need(w, "w", at::kHalf);
+  TORCH_CHECK(w.dim() == 2 && w.size(0) == 2 * dim && w.size(1) == dim, "softagg_fused: w must be float16 [2*dim, dim]");
+  arg.need(bias, "bias [2*dim]", at::kFloat, 2 * dim);
+  arg.need(order, "order (one entry per row of x)", at::kInt, E);
+  arg.need(group_of, "group_of (one entry per row of x)", at::kInt, E);
+  arg.need(group_start, "group_start", at::kInt);
+  arg.need(n_groups, "n_groups", at::kInt, 1);
+  Tensor ws = arg.need(workspace, "workspace");
+  TORCH_CHECK(group_start.numel() >= max_groups + 1, "softagg_fused: group_start must have at least max_groups + 1 entries");
   TORCH_CHECK(max_groups >= 0 && max_groups <= E, "softagg_fused: max_groups must be in [0, E]");
   const int64_t wsb = dpvo_softagg_fused_workspace_bytes(E);
-  Tensor ws = workspace.has_value() ? *workspace : byte_ws(wsb, x);
-  TORCH_CHECK(ws.is_cuda() && ws.is_contiguous() && (int64_t)(ws.numel() * ws.element_size()) >= wsb, "softagg_fused: workspace too small");
+  if (!ws.defined()) ws = byte_ws(wsb, x);
+  TORCH_CHECK((int64_t)(ws.numel() * ws.element_size()) >= wsb, "softagg_fused: workspace too small");
   Tensor y = torch::empty({1, max_groups, dim}, x.options());   // rows past the group count are zeroed by the op itself
   check(dpvo_softagg_fused(x2.data_ptr(), x2.stride(0), order.data_ptr<int>(), group_of.data_ptr<int>(), group_start.data_ptr<int>(),
                            n_groups.data_ptr<int>(), w.data_ptr(), bias.data_ptr<float>(), E, max_groups, y.data_ptr(),
@@ -627,25 +676,24 @@ int64_t softagg_fused_workspace_bytes(int64_t E) { return dpvo_softagg_fused_wor
 Tensor linear_f16(Tensor x, Tensor w, c10::optional<Tensor> bias, int64_t epilogue, c10::optional<Tensor> res,
                   c10::optional<Tensor> gate, c10::optional<Tensor> gather, bool out_f32, c10::optional<Tensor> out,
                   c10::optional<Tensor> out16) {
-  need_cuda(x, "x");
-  c10::cuda::CUDAGuard guard(x.device());
-  TORCH_CHECK(x.scalar_type() == at::kHalf && w.scalar_type() == at::kHalf, "linear_f16: fp16 operands expected");
+  const Args arg("dpvo_b200_ext.linear_f16", x, "x");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(x, "x", at::kHalf); arg.on(w, "w", at::kHalf);
+  Tensor gi = arg.as(gather, "gather", at::kLong), b = arg.as(bias, "bias", at::kFloat), r = arg.on(res, "res");
+  Tensor g = arg.on(gate, "gate", at::kHalf);
+  Tensor y = arg.need(out, "out", out_f32 ? at::kFloat : at::kHalf), y16 = arg.need(out16, "out16", at::kHalf);
   TORCH_CHECK(x.stride(-1) == 1 && w.dim() == 2 && w.stride(1) == 1, "linear_f16: K must be contiguous");
   const int K = w.size(1), N = w.size(0);
   TORCH_CHECK(x.size(-1) == K, "linear_f16: X has ", x.size(-1), " columns, W expects ", K);
   Tensor x2 = x.dim() == 2 ? x : x.reshape({-1, K});
   TORCH_CHECK(x2.stride(1) == 1, "linear_f16: X rows must be dense");
-  Tensor gi, b, r, g;
-  int64_t rows = x2.size(0);
-  if (gather.has_value()) { gi = i64c(*gather); rows = gi.numel(); }
-  if (bias.has_value()) b = f32c(*bias);
+  const int64_t rows = gi.defined() ? gi.numel() : x2.size(0);
   int res_dt = DPVO_F32; int64_t ldres = 0, ldgate = 0;
-  if (res.has_value()) { r = res->reshape({-1, N}); TORCH_CHECK(r.stride(1) == 1 && r.size(0) == rows, "linear_f16: res shape"); res_dt = dt16or32(r); ldres = r.stride(0); }
-  if (gate.has_value()) { g = gate->reshape({-1, N}); TORCH_CHECK(g.scalar_type() == at::kHalf && g.stride(1) == 1 && g.size(0) == rows, "linear_f16: gate shape"); ldgate = g.stride(0); }
-  Tensor y = out.has_value() ? *out : torch::empty({1, rows, N}, x.options().dtype(out_f32 ? at::kFloat : at::kHalf));
-  TORCH_CHECK(y.is_contiguous() && y.numel() == rows * N && y.scalar_type() == (out_f32 ? at::kFloat : at::kHalf), "linear_f16: out tensor");
-  Tensor y16;
-  if (out16.has_value()) { y16 = *out16; TORCH_CHECK(y16.is_contiguous() && y16.numel() == rows * N && y16.scalar_type() == at::kHalf, "linear_f16: out16 tensor"); }
+  if (r.defined()) { r = r.reshape({-1, N}); TORCH_CHECK(r.stride(1) == 1 && r.size(0) == rows, "linear_f16: res shape"); res_dt = dt16or32(r); ldres = r.stride(0); }
+  if (g.defined()) { g = g.reshape({-1, N}); TORCH_CHECK(g.stride(1) == 1 && g.size(0) == rows, "linear_f16: gate shape"); ldgate = g.stride(0); }
+  if (!y.defined()) y = torch::empty({1, rows, N}, x.options().dtype(out_f32 ? at::kFloat : at::kHalf));
+  TORCH_CHECK(y.numel() == rows * N, "linear_f16: out tensor");
+  if (y16.defined()) TORCH_CHECK(y16.numel() == rows * N, "linear_f16: out16 tensor");
   check(dpvo_linear_f16(x2.data_ptr(), x2.stride(0), gi.defined() ? gi.data_ptr<int64_t>() : nullptr, w.data_ptr(), w.stride(0),
                         b.defined() ? b.data_ptr<float>() : nullptr, r.defined() ? r.data_ptr() : nullptr, res_dt, ldres,
                         g.defined() ? g.data_ptr() : nullptr, ldgate, y.data_ptr(), out_f32 ? DPVO_F32 : DPVO_F16, N,
@@ -655,8 +703,9 @@ Tensor linear_f16(Tensor x, Tensor w, c10::optional<Tensor> bias, int64_t epilog
 }
 
 std::vector<Tensor> neighbors_from_groups(Tensor order, Tensor group_of) {
-  need_cuda(order, "order");
-  c10::cuda::CUDAGuard guard(order.device());
+  const Args arg("dpvo_b200_ext.neighbors_from_groups", order, "order");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(order, "order", at::kInt); arg.need(group_of, "group_of", at::kInt);
   const int64_t E = order.numel();
   auto ol = order.options().dtype(at::kLong);
   Tensor ix = torch::empty({E}, ol), jx = torch::empty({E}, ol);
@@ -668,25 +717,25 @@ std::vector<Tensor> neighbors_from_groups(Tensor order, Tensor group_of) {
 
 std::vector<Tensor> update_heads(Tensor net32, Tensor W4, Tensor b4, c10::optional<Tensor> coords, c10::optional<Tensor> gate,
                                  c10::optional<Tensor> res) {
-  need_cuda(net32, "net");
-  c10::cuda::CUDAGuard guard(net32.device());
-  TORCH_CHECK(net32.scalar_type() == at::kFloat, "update_heads: net must be float32");
+  const Args arg("dpvo_b200_ext.update_heads", net32, "net");
+  c10::cuda::CUDAGuard guard(arg.dev);
   TORCH_CHECK(gate.has_value() == res.has_value(), "update_heads: gate and res come together");
-  TORCH_CHECK(!gate.has_value() || net32.is_contiguous(), "update_heads: the gated form updates net in place and needs it contiguous");
-  net32 = net32.contiguous(); W4 = f32c(W4); b4 = f32c(b4);
+  // the gated form updates net in place
+  net32 = gate.has_value() ? arg.need(net32, "net", at::kFloat) : arg.on(net32, "net", at::kFloat).contiguous();
+  W4 = arg.as(W4, "W4", at::kFloat); b4 = arg.as(b4, "b4", at::kFloat);
+  Tensor cd = arg.as(coords, "coords", at::kFloat), g2 = arg.on(gate, "gate", at::kHalf), r2 = arg.on(res, "res", at::kHalf);
   const int dim = net32.size(-1);
   const int64_t rows = net32.numel() / dim;
   TORCH_CHECK(W4.numel() == 4 * dim && b4.numel() == 4, "update_heads: W4 [4,dim], b4 [4]");
-  Tensor delta = torch::empty({1, rows, 2}, net32.options()), weight = torch::empty({1, rows, 2}, net32.options());
-  Tensor cd; int P = 1;
-  if (coords.has_value()) { cd = f32c(*coords); P = cd.size(-1); TORCH_CHECK(cd.numel() == rows * 2 * P * P, "update_heads: coords must be [rows,2,P,P]"); }
-  Tensor g2, r2; int64_t ldg = 0, ldr = 0;
-  if (gate.has_value()) {
-    g2 = gate->reshape({-1, dim}); r2 = res->reshape({-1, dim});
-    TORCH_CHECK(g2.scalar_type() == at::kHalf && r2.scalar_type() == at::kHalf && g2.stride(1) == 1 && r2.stride(1) == 1 && g2.size(0) == rows && r2.size(0) == rows,
-                "update_heads: gate / res must be fp16 [rows, dim]");
+  int P = 1;
+  if (cd.defined()) { P = cd.size(-1); TORCH_CHECK(cd.numel() == rows * 2 * P * P, "update_heads: coords must be [rows,2,P,P]"); }
+  int64_t ldg = 0, ldr = 0;
+  if (g2.defined()) {
+    g2 = g2.reshape({-1, dim}); r2 = r2.reshape({-1, dim});
+    TORCH_CHECK(g2.stride(1) == 1 && r2.stride(1) == 1 && g2.size(0) == rows && r2.size(0) == rows, "update_heads: gate / res must be fp16 [rows, dim]");
     ldg = g2.stride(0); ldr = r2.stride(0);
   }
+  Tensor delta = torch::empty({1, rows, 2}, net32.options()), weight = torch::empty({1, rows, 2}, net32.options());
   check(dpvo_update_heads(net32.data_ptr(), g2.defined() ? g2.data_ptr() : nullptr, ldg, r2.defined() ? r2.data_ptr() : nullptr, ldr,
                           W4.data_ptr<float>(), b4.data_ptr<float>(), cd.defined() ? cd.data_ptr<float>() : nullptr, P,
                           delta.data_ptr<float>(),
@@ -696,24 +745,20 @@ std::vector<Tensor> update_heads(Tensor net32, Tensor W4, Tensor b4, c10::option
 }
 
 // ---- fused layer chains of the update operator (include/dpvo_b200.h, "fused layer chains")
-static void chain_check(const Tensor& t, at::ScalarType st, const char* what) {
-  TORCH_CHECK(t.is_cuda() && t.is_contiguous() && t.scalar_type() == st, "dpvo_b200 update chain: ", what, " must be a contiguous CUDA tensor of the expected dtype");
-}
 Tensor update_corr_norm(Tensor corr16, Tensor W0, Tensor W25, Tensor params, Tensor net32, Tensor inp16, c10::optional<Tensor> inp_index,
                         c10::optional<Tensor> net16_out) {
-  need_cuda(net32, "net");
-  c10::cuda::CUDAGuard guard(net32.device());
-  chain_check(W0, at::kHalf, "W0"); chain_check(W25, at::kHalf, "W25"); chain_check(params, at::kFloat, "params");
-  chain_check(net32, at::kFloat, "net32"); chain_check(inp16, at::kHalf, "inp16");
+  const Args arg("dpvo_b200_ext.update_corr_norm", net32, "net32");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(corr16, "corr16", at::kHalf); arg.need(W0, "W0", at::kHalf); arg.need(W25, "W25", at::kHalf);
+  arg.need(params, "params", at::kFloat); arg.need(net32, "net32", at::kFloat); arg.need(inp16, "inp16", at::kHalf);
+  Tensor idx = arg.as(inp_index, "inp_index", at::kLong), n16 = arg.need(net16_out, "net16_out", at::kHalf);
   const int64_t E = net32.numel() / 384;
   Tensor c2 = corr16.reshape({-1, corr16.size(-1)});
-  TORCH_CHECK(c2.scalar_type() == at::kHalf && c2.stride(1) == 1 && c2.size(0) == E && c2.size(1) == 896, "update_corr_norm: corr must be fp16 [E, 896] (zero padded)");
+  TORCH_CHECK(c2.stride(1) == 1 && c2.size(0) == E && c2.size(1) == 896, "update_corr_norm: corr must be fp16 [E, 896] (zero padded)");
   TORCH_CHECK(net32.size(-1) == 384 && W0.numel() == 384 * 896 && W25.numel() == 768 * 384 && params.numel() == 7 * 384 && inp16.size(-1) == 384, "update_corr_norm: shapes");
-  Tensor idx;
-  if (inp_index.has_value()) { idx = i64c(*inp_index); TORCH_CHECK(idx.numel() == E, "update_corr_norm: inp_index length"); }
+  if (idx.defined()) { TORCH_CHECK(idx.numel() == E, "update_corr_norm: inp_index length"); }
   else TORCH_CHECK(inp16.numel() == E * 384, "update_corr_norm: inp must have one row per edge when no index is given");
-  Tensor n16 = net16_out.has_value() ? *net16_out : torch::empty({1, E, 384}, net32.options().dtype(at::kHalf));
-  chain_check(n16, at::kHalf, "net16_out");
+  if (!n16.defined()) n16 = torch::empty({1, E, 384}, net32.options().dtype(at::kHalf));
   TORCH_CHECK(n16.numel() == E * 384, "update_corr_norm: net16_out shape");
   check(dpvo_update_corr_norm(c2.data_ptr(), c2.stride(0), W0.data_ptr(), W25.data_ptr(), params.data_ptr<float>(), net32.data_ptr<float>(),
                               inp16.data_ptr(), idx.defined() ? idx.data_ptr<int64_t>() : nullptr, n16.data_ptr(), E, stream()),
@@ -722,14 +767,15 @@ Tensor update_corr_norm(Tensor corr16, Tensor W0, Tensor W25, Tensor params, Ten
 }
 
 Tensor update_neighbor_mlp(Tensor net16_in, Tensor index, Tensor Wab, Tensor params, Tensor net32, c10::optional<Tensor> net16_out) {
-  need_cuda(net32, "net");
-  c10::cuda::CUDAGuard guard(net32.device());
-  chain_check(net16_in, at::kHalf, "net16_in"); chain_check(Wab, at::kHalf, "Wab"); chain_check(params, at::kFloat, "params"); chain_check(net32, at::kFloat, "net32");
+  const Args arg("dpvo_b200_ext.update_neighbor_mlp", net32, "net32");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(net16_in, "net16_in", at::kHalf); arg.need(Wab, "Wab", at::kHalf); arg.need(params, "params", at::kFloat);
+  arg.need(net32, "net32", at::kFloat);
+  index = arg.as(index, "index", at::kLong);
+  Tensor n16 = arg.need(net16_out, "net16_out", at::kHalf);
   const int64_t E = net32.numel() / 384;
-  index = i64c(index);
   TORCH_CHECK(net32.size(-1) == 384 && net16_in.numel() == E * 384 && index.numel() == E && Wab.numel() == 768 * 384 && params.numel() == 2 * 384, "update_neighbor_mlp: shapes");
-  Tensor n16 = net16_out.has_value() ? *net16_out : torch::empty({1, E, 384}, net32.options().dtype(at::kHalf));
-  chain_check(n16, at::kHalf, "net16_out");
+  if (!n16.defined()) n16 = torch::empty({1, E, 384}, net32.options().dtype(at::kHalf));
   TORCH_CHECK(n16.numel() == E * 384, "update_neighbor_mlp: net16_out shape");
   check(dpvo_update_neighbor_mlp(net16_in.data_ptr(), index.data_ptr<int64_t>(), Wab.data_ptr(), params.data_ptr<float>(), net32.data_ptr<float>(),
                                  n16.data_ptr(), E, stream()),
@@ -740,33 +786,25 @@ Tensor update_neighbor_mlp(Tensor net16_in, Tensor index, Tensor Wab, Tensor par
 std::vector<Tensor> update_gru_heads(Tensor net32, c10::optional<Tensor> hij16, c10::optional<Tensor> group_of, Tensor W6, Tensor params,
                                      c10::optional<Tensor> coords, c10::optional<Tensor> workspace, c10::optional<Tensor> hkk16, c10::optional<Tensor> group_kk,
                                      c10::optional<Tensor> delta_out, c10::optional<Tensor> weight_out) {
-  need_cuda(net32, "net");
-  c10::cuda::CUDAGuard guard(net32.device());
-  chain_check(net32, at::kFloat, "net32"); chain_check(W6, at::kHalf, "W6"); chain_check(params, at::kFloat, "params");
+  const Args arg("dpvo_b200_ext.update_gru_heads", net32, "net32");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(net32, "net32", at::kFloat); arg.need(W6, "W6", at::kHalf); arg.need(params, "params", at::kFloat);
+  Tensor hij = arg.need(hij16, "hij16", at::kHalf), gof = arg.as(group_of, "group_of", at::kInt);
+  Tensor hkk = arg.need(hkk16, "hkk16", at::kHalf), gkk = arg.as(group_kk, "group_kk", at::kInt);
+  Tensor cd = arg.as(coords, "coords", at::kFloat), ws = arg.need(workspace, "workspace");
+  Tensor delta = arg.need(delta_out, "delta_out", at::kFloat), weight = arg.need(weight_out, "weight_out", at::kFloat);
   const int64_t E = net32.numel() / 384;
   TORCH_CHECK(net32.size(-1) == 384 && W6.numel() == 6 * 384 * 384 && params.numel() == 14 * 384 + 4, "update_gru_heads: shapes");
-  TORCH_CHECK(hij16.has_value() == group_of.has_value(), "update_gru_heads: group rows and group ids come together");
-  Tensor hij, gof;
-  if (hij16.has_value()) {
-    hij = *hij16; gof = group_of->to(at::kInt).contiguous();
-    chain_check(hij, at::kHalf, "hij16");
-    TORCH_CHECK(hij.size(-1) == 384 && gof.numel() == E, "update_gru_heads: group operand shapes");
-  }
-  TORCH_CHECK(hkk16.has_value() == group_kk.has_value(), "update_gru_heads: group rows and group ids come together");
-  Tensor hkk, gkk;
-  if (hkk16.has_value()) {
-    hkk = *hkk16; gkk = group_kk->to(at::kInt).contiguous();
-    chain_check(hkk, at::kHalf, "hkk16");
-    TORCH_CHECK(hkk.size(-1) == 384 && gkk.numel() == E, "update_gru_heads: group operand shapes");
-  }
-  Tensor cd; int P = 1;
-  if (coords.has_value()) { cd = f32c(*coords); P = cd.size(-1); TORCH_CHECK(cd.numel() == E * 2 * P * P, "update_gru_heads: coords must be [E,2,P,P]"); }
+  TORCH_CHECK(hij.defined() == gof.defined() && hkk.defined() == gkk.defined(), "update_gru_heads: group rows and group ids come together");
+  if (hij.defined()) TORCH_CHECK(hij.size(-1) == 384 && gof.numel() == E, "update_gru_heads: group operand shapes");
+  if (hkk.defined()) TORCH_CHECK(hkk.size(-1) == 384 && gkk.numel() == E, "update_gru_heads: group operand shapes");
+  int P = 1;
+  if (cd.defined()) { P = cd.size(-1); TORCH_CHECK(cd.numel() == E * 2 * P * P, "update_gru_heads: coords must be [E,2,P,P]"); }
   const int64_t wsb = dpvo_update_gru_workspace_bytes();
-  Tensor ws = workspace.has_value() ? *workspace : byte_ws(wsb, net32);
-  TORCH_CHECK(ws.is_cuda() && ws.is_contiguous() && (int64_t)(ws.numel() * ws.element_size()) >= wsb, "update_gru_heads: workspace too small");
-  Tensor delta = delta_out.has_value() ? *delta_out : torch::empty({1, E, 2}, net32.options());
-  Tensor weight = weight_out.has_value() ? *weight_out : torch::empty({1, E, 2}, net32.options());
-  chain_check(delta, at::kFloat, "delta_out"); chain_check(weight, at::kFloat, "weight_out");
+  if (!ws.defined()) ws = byte_ws(wsb, net32);
+  TORCH_CHECK((int64_t)(ws.numel() * ws.element_size()) >= wsb, "update_gru_heads: workspace too small");
+  if (!delta.defined()) delta = torch::empty({1, E, 2}, net32.options());
+  if (!weight.defined()) weight = torch::empty({1, E, 2}, net32.options());
   TORCH_CHECK(delta.numel() == E * 2 && weight.numel() == E * 2, "update_gru_heads: delta_out / weight_out must hold [E, 2]");
   check(dpvo_update_gru_heads(net32.data_ptr<float>(), hij.defined() ? hij.data_ptr() : nullptr, gof.defined() ? gof.data_ptr<int>() : nullptr,
                               hkk.defined() ? hkk.data_ptr() : nullptr, gkk.defined() ? gkk.data_ptr<int>() : nullptr, W6.data_ptr(), params.data_ptr<float>(), cd.defined() ? cd.data_ptr<float>() : nullptr, P,
@@ -777,43 +815,36 @@ std::vector<Tensor> update_gru_heads(Tensor net32, c10::optional<Tensor> hij16, 
 int64_t update_gru_workspace_bytes() { return dpvo_update_gru_workspace_bytes(); }
 
 // ---- device-resident patch-graph bookkeeping (include/dpvo_b200.h)
-static void pg_check(const Tensor& ii, const Tensor& jj, const Tensor& kk, const Tensor& active) {
-  TORCH_CHECK(ii.is_cuda() && ii.scalar_type() == at::kLong && ii.is_contiguous() && jj.scalar_type() == at::kLong && jj.is_contiguous() &&
-              kk.scalar_type() == at::kLong && kk.is_contiguous() && active.scalar_type() == at::kByte && active.is_contiguous() &&
-              jj.numel() == ii.numel() && kk.numel() == ii.numel() && active.numel() == ii.numel(), "pgraph: ii / jj / kk int64 and active uint8, one entry per slot");
+// the fixed-capacity edge store: ii / jj / kk int64 and active uint8, one entry per slot
+static void edge_store(const Args& arg, const Tensor& ii, const Tensor& jj, const Tensor& kk, const Tensor& active) {
+  arg.need(ii, "ii", at::kLong); arg.need(jj, "jj", at::kLong, ii.numel()); arg.need(kk, "kk", at::kLong, ii.numel());
+  arg.need(active, "active", at::kByte, ii.numel());
 }
 void pgraph_remove(Tensor ii, Tensor jj, Tensor kk, Tensor active, int64_t rule, Tensor frame, int64_t param, c10::optional<Tensor> enable,
                    int64_t dummy_frame, int64_t dummy_patch, int64_t M, Tensor n_active) {
-  need_cuda(ii, "ii");
-  c10::cuda::CUDAGuard guard(ii.device());
-  pg_check(ii, jj, kk, active);
-  TORCH_CHECK(frame.is_cuda() && frame.scalar_type() == at::kLong && frame.numel() == 1 && n_active.is_cuda() && n_active.scalar_type() == at::kInt && n_active.numel() == 1,
-              "pgraph_remove: frame is a device int64 scalar, n_active a device int32 scalar");
-  const int32_t* en = nullptr;
-  if (enable.has_value()) { TORCH_CHECK(enable->is_cuda() && enable->scalar_type() == at::kInt && enable->numel() == 1, "pgraph_remove: enable is a device int32 scalar"); en = enable->data_ptr<int>(); }
+  const Args arg("dpvo_b200_ext.pgraph_remove", ii, "ii");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  edge_store(arg, ii, jj, kk, active);
+  arg.need(frame, "frame", at::kLong, 1); arg.need(n_active, "n_active", at::kInt, 1);
+  Tensor e = arg.need(enable, "enable", at::kInt, 1);
+  const int32_t* en = e.defined() ? e.data_ptr<int>() : nullptr;
   check(dpvo_pgraph_remove(ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(), (int)rule,
                            frame.data_ptr<int64_t>(), param, en, dummy_frame, dummy_patch, (int)M, n_active.data_ptr<int>(), stream()),
         "dpvo_b200_ext.pgraph_remove");
 }
 Tensor pgraph_append(Tensor ii, Tensor jj, Tensor kk, Tensor active, Tensor new_ii, Tensor new_jj, Tensor new_kk, c10::optional<Tensor> enable,
                      c10::optional<Tensor> state, Tensor n_active, Tensor overflow) {
-  need_cuda(ii, "ii");
-  c10::cuda::CUDAGuard guard(ii.device());
-  pg_check(ii, jj, kk, active);
-  new_ii = i64c(new_ii); new_jj = i64c(new_jj); new_kk = i64c(new_kk);
+  const Args arg("dpvo_b200_ext.pgraph_append", ii, "ii");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  edge_store(arg, ii, jj, kk, active);
+  new_ii = arg.as(new_ii, "new_ii", at::kLong); new_jj = arg.as(new_jj, "new_jj", at::kLong); new_kk = arg.as(new_kk, "new_kk", at::kLong);
+  arg.need(n_active, "n_active", at::kInt, 1); arg.need(overflow, "overflow", at::kInt, 1);
+  Tensor e = arg.need(enable, "enable", at::kInt, 1), s = arg.need(state, "state [cap, 384]", at::kFloat, ii.numel() * 384);
   const int64_t n_new = new_ii.numel();
   TORCH_CHECK(new_jj.numel() == n_new && new_kk.numel() == n_new, "pgraph_append: new edge lists differ in length");
-  TORCH_CHECK(n_active.is_cuda() && n_active.scalar_type() == at::kInt && n_active.numel() == 1 && overflow.is_cuda() && overflow.scalar_type() == at::kInt && overflow.numel() == 1,
-              "pgraph_append: n_active / overflow are device int32 scalars");
-  const int32_t* en = nullptr;
-  if (enable.has_value()) { TORCH_CHECK(enable->is_cuda() && enable->scalar_type() == at::kInt && enable->numel() == 1, "pgraph_append: enable is a device int32 scalar"); en = enable->data_ptr<int>(); }
+  const int32_t* en = e.defined() ? e.data_ptr<int>() : nullptr;
+  float* st = s.defined() ? s.data_ptr<float>() : nullptr;
   Tensor slots = torch::empty({n_new}, ii.options().dtype(at::kInt));
-  float* st = nullptr;
-  if (state.has_value()) {
-    TORCH_CHECK(state->is_cuda() && state->scalar_type() == at::kFloat && state->is_contiguous() && state->numel() == ii.numel() * 384,
-                "pgraph_append: state must be the contiguous fp32 [cap, 384] recurrent state");
-    st = state->data_ptr<float>();
-  }
   check(dpvo_pgraph_append(ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(),
                            new_ii.data_ptr<int64_t>(), new_jj.data_ptr<int64_t>(), new_kk.data_ptr<int64_t>(), n_new, en, st, slots.data_ptr<int>(),
                            n_active.data_ptr<int>(), overflow.data_ptr<int>(), stream()),
@@ -821,9 +852,9 @@ Tensor pgraph_append(Tensor ii, Tensor jj, Tensor kk, Tensor active, Tensor new_
   return slots;
 }
 std::vector<Tensor> pgraph_new_edges(Tensor n_dev, int64_t M, int64_t r) {
-  need_cuda(n_dev, "n");
-  c10::cuda::CUDAGuard guard(n_dev.device());
-  TORCH_CHECK(n_dev.scalar_type() == at::kLong && n_dev.numel() == 1, "pgraph_new_edges: n is a device int64 scalar");
+  const Args arg("dpvo_b200_ext.pgraph_new_edges", n_dev, "n");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(n_dev, "n", at::kLong, 1);
   const int64_t total = M * (2 * r - 1);
   Tensor ii = torch::empty({total}, n_dev.options()), jj = torch::empty({total}, n_dev.options()), kk = torch::empty({total}, n_dev.options());
   check(dpvo_pgraph_new_edges(n_dev.data_ptr<int64_t>(), (int)M, (int)r, ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), stream()),
@@ -832,22 +863,13 @@ std::vector<Tensor> pgraph_new_edges(Tensor n_dev, int64_t M, int64_t r) {
 }
 
 // ---- proximity loop closure (include/dpvo_b200.h, csrc/loop.cu)
-static void dev_scalar(const Tensor& t, at::ScalarType ty, const char* what) {
-  TORCH_CHECK(t.is_cuda() && t.scalar_type() == ty && t.numel() == 1, what);
-}
-static void f32_rows(const Tensor& t, int64_t rows, int64_t cols, const char* what) {
-  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == rows * cols, what);
-}
 Tensor loop_scores(Tensor poses, Tensor patches, Tensor intrinsics, Tensor n_dev, Tensor last_ba, int64_t M, int64_t removal,
                    int64_t max_age, int64_t freq, int64_t kf_index) {
-  need_cuda(poses, "poses");
-  c10::cuda::CUDAGuard guard(poses.device());
-  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat && intrinsics.scalar_type() == at::kFloat &&
-              poses.is_contiguous() && patches.is_contiguous() && intrinsics.is_contiguous() && patches.is_cuda() && intrinsics.is_cuda(),
-              "loop_scores: poses / patches / intrinsics are contiguous fp32 CUDA tensors");
+  const Args arg("dpvo_b200_ext.loop_scores", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(poses, "poses", at::kFloat); arg.need(patches, "patches", at::kFloat); arg.need(intrinsics, "intrinsics", at::kFloat);
+  arg.need(n_dev, "n", at::kLong, 1); arg.need(last_ba, "last_global_ba", at::kLong, 1);
   TORCH_CHECK(patches.numel() % 27 == 0 && patches.size(-1) == 3, "loop_scores: patches are [K, 3, 3, 3]");
-  dev_scalar(n_dev, at::kLong, "loop_scores: n is a device int64 scalar");
-  dev_scalar(last_ba, at::kLong, "loop_scores: last_global_ba is a device int64 scalar");
   const int64_t S = dpvo_loop_candidates((int)max_age, (int)freq, (int)kf_index);
   Tensor scores = torch::empty({std::max<int64_t>(S, 1)}, poses.options());
   check(dpvo_loop_scores(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(), n_dev.data_ptr<int64_t>(),
@@ -859,23 +881,17 @@ Tensor loop_scores(Tensor poses, Tensor patches, Tensor intrinsics, Tensor n_dev
 void loop_select(Tensor scores, Tensor n_dev, Tensor last_ba, int64_t M, int64_t removal, int64_t max_age, int64_t freq, int64_t kf_index,
                  double thresh, Tensor pairs, Tensor n_pairs, Tensor ii, Tensor jj, Tensor kk, Tensor active, c10::optional<Tensor> state,
                  Tensor n_active, Tensor overflow) {
-  need_cuda(scores, "scores");
-  c10::cuda::CUDAGuard guard(scores.device());
+  const Args arg("dpvo_b200_ext.loop_select", scores, "scores");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int64_t S = dpvo_loop_candidates((int)max_age, (int)freq, (int)kf_index);
-  f32_rows(scores, S, 1, "loop_select: scores are the fp32 [J * max_age] output of loop_scores");
-  dev_scalar(n_dev, at::kLong, "loop_select: n is a device int64 scalar");
-  dev_scalar(last_ba, at::kLong, "loop_select: last_global_ba is a device int64 scalar");
-  dev_scalar(n_pairs, at::kInt, "loop_select: n_pairs is a device int32 scalar");
-  dev_scalar(n_active, at::kInt, "loop_select: n_active is a device int32 scalar");
-  dev_scalar(overflow, at::kInt, "loop_select: overflow is a device int32 scalar");
-  TORCH_CHECK(pairs.is_cuda() && pairs.scalar_type() == at::kLong && pairs.is_contiguous() && pairs.dim() == 2 && pairs.size(1) == 2,
-              "loop_select: pairs is a contiguous device int64 [max_pairs, 2]");
-  pg_check(ii, jj, kk, active);
-  float* st = nullptr;
-  if (state.has_value()) {
-    f32_rows(*state, ii.numel(), 384, "loop_select: state must be the contiguous fp32 [region, 384] recurrent state of the loop region");
-    st = state->data_ptr<float>();
-  }
+  arg.need(scores, "scores (the [J * max_age] output of loop_scores)", at::kFloat, S);
+  arg.need(n_dev, "n", at::kLong, 1); arg.need(last_ba, "last_global_ba", at::kLong, 1); arg.need(n_pairs, "n_pairs", at::kInt, 1);
+  arg.need(n_active, "n_active", at::kInt, 1); arg.need(overflow, "overflow", at::kInt, 1);
+  arg.need(pairs, "pairs", at::kLong);
+  TORCH_CHECK(pairs.dim() == 2 && pairs.size(1) == 2, "loop_select: pairs is a device int64 [max_pairs, 2]");
+  edge_store(arg, ii, jj, kk, active);
+  Tensor s = arg.need(state, "state (the [region, 384] recurrent state of the loop region)", at::kFloat, ii.numel() * 384);
+  float* st = s.defined() ? s.data_ptr<float>() : nullptr;
   check(dpvo_loop_select(scores.data_ptr<float>(), n_dev.data_ptr<int64_t>(), last_ba.data_ptr<int64_t>(), (int)M, (int)removal, (int)max_age,
                          (int)freq, (int)kf_index, (float)thresh, (int)pairs.size(0), pairs.data_ptr<int64_t>(), n_pairs.data_ptr<int>(),
                          ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(), st,
@@ -885,23 +901,17 @@ void loop_select(Tensor scores, Tensor n_dev, Tensor last_ba, int64_t M, int64_t
 void pgraph_remove_store(Tensor ii, Tensor jj, Tensor kk, Tensor active, Tensor target, Tensor weight, Tensor n_dev, int64_t removal,
                          int64_t opt_window, c10::optional<Tensor> enable, int64_t dummy_frame, int64_t dummy_patch, int64_t M, Tensor n_active,
                          Tensor s_ii, Tensor s_jj, Tensor s_kk, Tensor s_target, Tensor s_weight, Tensor s_count, Tensor s_overflow) {
-  need_cuda(ii, "ii");
-  c10::cuda::CUDAGuard guard(ii.device());
-  pg_check(ii, jj, kk, active);
+  const Args arg("dpvo_b200_ext.pgraph_remove_store", ii, "ii");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  edge_store(arg, ii, jj, kk, active);
   const int64_t cap = ii.numel(), sc = s_ii.numel();
-  f32_rows(target, cap, 2, "pgraph_remove_store: target is the contiguous fp32 [cap, 2] of the active store");
-  f32_rows(weight, cap, 2, "pgraph_remove_store: weight is the contiguous fp32 [cap, 2] of the active store");
-  TORCH_CHECK(s_ii.is_cuda() && s_ii.scalar_type() == at::kLong && s_ii.is_contiguous() && s_jj.scalar_type() == at::kLong && s_jj.is_contiguous() &&
-              s_kk.scalar_type() == at::kLong && s_kk.is_contiguous() && s_jj.numel() == sc && s_kk.numel() == sc,
-              "pgraph_remove_store: the inactive ii / jj / kk are contiguous device int64, one entry per slot");
-  f32_rows(s_target, sc, 2, "pgraph_remove_store: the inactive target is contiguous fp32 [store, 2]");
-  f32_rows(s_weight, sc, 2, "pgraph_remove_store: the inactive weight is contiguous fp32 [store, 2]");
-  dev_scalar(n_dev, at::kLong, "pgraph_remove_store: n is a device int64 scalar");
-  dev_scalar(n_active, at::kInt, "pgraph_remove_store: n_active is a device int32 scalar");
-  dev_scalar(s_count, at::kInt, "pgraph_remove_store: the store count is a device int32 scalar");
-  dev_scalar(s_overflow, at::kInt, "pgraph_remove_store: the store overflow flag is a device int32 scalar");
-  const int32_t* en = nullptr;
-  if (enable.has_value()) { dev_scalar(*enable, at::kInt, "pgraph_remove_store: enable is a device int32 scalar"); en = enable->data_ptr<int>(); }
+  arg.need(target, "target [cap, 2]", at::kFloat, cap * 2); arg.need(weight, "weight [cap, 2]", at::kFloat, cap * 2);
+  arg.need(s_ii, "s_ii", at::kLong); arg.need(s_jj, "s_jj", at::kLong, sc); arg.need(s_kk, "s_kk", at::kLong, sc);
+  arg.need(s_target, "s_target [store, 2]", at::kFloat, sc * 2); arg.need(s_weight, "s_weight [store, 2]", at::kFloat, sc * 2);
+  arg.need(n_dev, "n", at::kLong, 1); arg.need(n_active, "n_active", at::kInt, 1);
+  arg.need(s_count, "s_count", at::kInt, 1); arg.need(s_overflow, "s_overflow", at::kInt, 1);
+  Tensor e = arg.need(enable, "enable", at::kInt, 1);
+  const int32_t* en = e.defined() ? e.data_ptr<int>() : nullptr;
   check(dpvo_pgraph_remove_store(ii.data_ptr<int64_t>(), jj.data_ptr<int64_t>(), kk.data_ptr<int64_t>(), active.data_ptr<uint8_t>(),
                                  target.data_ptr<float>(), weight.data_ptr<float>(), cap, n_dev.data_ptr<int64_t>(), (int)removal, (int)opt_window,
                                  en, dummy_frame, dummy_patch, (int)M, n_active.data_ptr<int>(), s_ii.data_ptr<int64_t>(), s_jj.data_ptr<int64_t>(),
@@ -910,62 +920,52 @@ void pgraph_remove_store(Tensor ii, Tensor jj, Tensor kk, Tensor active, Tensor 
         "dpvo_b200_ext.pgraph_remove_store");
 }
 void loop_flags(Tensor ii, Tensor active, int64_t normal, int64_t n, int64_t removal, c10::optional<Tensor> s_count, Tensor flags) {
-  need_cuda(ii, "ii");
-  c10::cuda::CUDAGuard guard(ii.device());
-  TORCH_CHECK(ii.scalar_type() == at::kLong && ii.is_contiguous() && active.is_cuda() && active.scalar_type() == at::kByte &&
-              active.is_contiguous() && active.numel() == ii.numel(), "loop_flags: ii int64 and active uint8, one entry per slot");
-  TORCH_CHECK(flags.is_cuda() && flags.scalar_type() == at::kLong && flags.is_contiguous() && flags.numel() == 4, "loop_flags: flags is device int64 [4]");
-  const int32_t* sc = nullptr;
-  if (s_count.has_value()) { dev_scalar(*s_count, at::kInt, "loop_flags: the store count is a device int32 scalar"); sc = s_count->data_ptr<int>(); }
+  const Args arg("dpvo_b200_ext.loop_flags", ii, "ii");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(ii, "ii", at::kLong); arg.need(active, "active", at::kByte, ii.numel()); arg.need(flags, "flags", at::kLong, 4);
+  Tensor c = arg.need(s_count, "s_count", at::kInt, 1);
+  const int32_t* sc = c.defined() ? c.data_ptr<int>() : nullptr;
   check(dpvo_loop_flags(ii.data_ptr<int64_t>(), active.data_ptr<uint8_t>(), ii.numel(), normal, n, (int)removal, sc, flags.data_ptr<int64_t>(), stream()),
         "dpvo_b200_ext.loop_flags");
 }
 void loop_normalize(Tensor poses, Tensor patches, int64_t n, int64_t M, c10::optional<Tensor> delta) {
-  need_cuda(poses, "poses");
-  c10::cuda::CUDAGuard guard(poses.device());
-  TORCH_CHECK(poses.scalar_type() == at::kFloat && patches.scalar_type() == at::kFloat && poses.is_contiguous() && patches.is_contiguous() &&
-              patches.is_cuda() && patches.dim() >= 3 && patches.size(-3) == 3, "loop_normalize: contiguous fp32 poses [N, 7] and patches [K, 3, P, P]");
+  const Args arg("dpvo_b200_ext.loop_normalize", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
+  arg.need(poses, "poses", at::kFloat); arg.need(patches, "patches", at::kFloat);
+  Tensor d = arg.need(delta, "delta", at::kFloat);
+  TORCH_CHECK(patches.dim() >= 3 && patches.size(-3) == 3, "loop_normalize: poses [N, 7] and patches [K, 3, P, P]");
   const int64_t P = patches.size(-1);
   TORCH_CHECK(n >= 0 && poses.numel() >= 7 * n && patches.numel() >= n * M * 3 * P * P, "loop_normalize: n = ", n, " frames exceed the buffers");
-  if (!delta.has_value()) {
+  if (!d.defined()) {
     check(dpvo_loop_normalize(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, stream()), "dpvo_b200_ext.loop_normalize");
     return;
   }
-  TORCH_CHECK(delta->is_cuda() && delta->scalar_type() == at::kFloat && delta->is_contiguous() && delta->numel() % 7 == 0,
-              "loop_normalize: delta is a contiguous fp32 [T, 7] table of relative poses");
-  check(dpvo_loop_normalize_deltas(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, delta->data_ptr<float>(),
-                                   delta->numel() / 7, stream()),
+  TORCH_CHECK(d.numel() % 7 == 0, "loop_normalize: delta is a [T, 7] table of relative poses");
+  check(dpvo_loop_normalize_deltas(poses.data_ptr<float>(), patches.data_ptr<float>(), n, (int)M, (int)P, d.data_ptr<float>(),
+                                   d.numel() / 7, stream()),
         "dpvo_b200_ext.loop_normalize");
 }
 
 // ---- keyframe culling (include/dpvo_b200.h, csrc/keyframe.cu)
-static void i64_rows(const Tensor& t, int64_t n, const char* what) {
-  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kLong && t.is_contiguous() && t.numel() == n, what);
-}
 void keyframe_motion(Tensor poses, Tensor patches, Tensor intrinsics, int64_t F, Tensor ii, Tensor jj, Tensor kk, Tensor active,
                      Tensor n, Tensor tstamp, Tensor delta, Tensor delta_src, int64_t ki, double thresh, Tensor flag, Tensor k, Tensor m,
                      Tensor overflow) {
-  need_cuda(poses, "poses");
-  c10::cuda::CUDAGuard guard(poses.device());
+  const Args arg("dpvo_b200_ext.keyframe_motion", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int64_t B = n.numel();
   TORCH_CHECK(B >= 1 && F >= 2, "keyframe_motion: one frame count per stream and at least 2 frame slots");
-  f32_rows(poses, B * F, 7, "keyframe_motion: poses are contiguous fp32 [B F, 7]");
-  f32_rows(intrinsics, B * F, 4, "keyframe_motion: intrinsics are contiguous fp32 [B F, 4]");
-  TORCH_CHECK(patches.is_cuda() && patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() % (B * F * 27) == 0 &&
-              patches.size(-1) == 3, "keyframe_motion: patches are contiguous fp32 [B F M, 3, 3, 3]");
-  pg_check(ii, jj, kk, active);
-  TORCH_CHECK(ii.is_cuda() && ii.numel() % B == 0, "keyframe_motion: the edge store holds one slice of slots per stream");
-  i64_rows(n, B, "keyframe_motion: n is a device int64 [B]");
-  i64_rows(tstamp, B * F, "keyframe_motion: tstamp is a contiguous device int64 [B, F]");
-  TORCH_CHECK(delta_src.is_cuda() && delta_src.scalar_type() == at::kLong && delta_src.is_contiguous() && delta_src.numel() % B == 0,
-              "keyframe_motion: delta_src is a contiguous device int64 [B, T]");
+  arg.need(poses, "poses [B F, 7]", at::kFloat, B * F * 7); arg.need(intrinsics, "intrinsics [B F, 4]", at::kFloat, B * F * 4);
+  arg.need(patches, "patches", at::kFloat);
+  TORCH_CHECK(patches.numel() % (B * F * 27) == 0 && patches.size(-1) == 3, "keyframe_motion: patches are [B F M, 3, 3, 3]");
+  edge_store(arg, ii, jj, kk, active);
+  TORCH_CHECK(ii.numel() % B == 0, "keyframe_motion: the edge store holds one slice of slots per stream");
+  arg.need(n, "n", at::kLong); arg.need(tstamp, "tstamp [B, F]", at::kLong, B * F);
+  arg.need(delta_src, "delta_src", at::kLong);
+  TORCH_CHECK(delta_src.numel() % B == 0, "keyframe_motion: delta_src is [B, T]");
   const int64_t T = delta_src.numel() / B;
-  f32_rows(delta, B * T, 7, "keyframe_motion: delta is a contiguous fp32 [B, T, 7]");
-  TORCH_CHECK(flag.is_cuda() && flag.scalar_type() == at::kInt && flag.is_contiguous() && flag.numel() == B, "keyframe_motion: flag is a device int32 [B]");
-  TORCH_CHECK(overflow.is_cuda() && overflow.scalar_type() == at::kInt && overflow.is_contiguous() && overflow.numel() == B,
-              "keyframe_motion: overflow is a device int32 [B]");
-  i64_rows(k, B, "keyframe_motion: k is a device int64 [B]");
-  TORCH_CHECK(m.is_cuda() && m.scalar_type() == at::kDouble && m.is_contiguous() && m.numel() == B, "keyframe_motion: m is a device fp64 [B]");
+  arg.need(delta, "delta [B, T, 7]", at::kFloat, B * T * 7);
+  arg.need(flag, "flag", at::kInt, B); arg.need(overflow, "overflow", at::kInt, B); arg.need(k, "k", at::kLong, B);
+  arg.need(m, "m", at::kDouble, B);
   const int64_t wsb = dpvo_keyframe_motion_workspace_bytes((int)B);
   Tensor ws = torch::empty({wsb}, poses.options().dtype(at::kByte));
   check(dpvo_keyframe_motion(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(), F, (int)B,
@@ -977,18 +977,18 @@ void keyframe_motion(Tensor poses, Tensor patches, Tensor intrinsics, int64_t F,
 }
 // each buffer is a dense tensor whose outermost dimension in memory holds B * rows slots of equal size, in order
 void keyframe_shift(std::vector<Tensor> bufs, std::vector<int64_t> rows, int64_t F, int64_t ki, Tensor flag, Tensor k) {
-  need_cuda(flag, "flag");
-  c10::cuda::CUDAGuard guard(flag.device());
+  const Args arg("dpvo_b200_ext.keyframe_shift", flag, "flag");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int64_t B = flag.numel();
-  TORCH_CHECK(flag.scalar_type() == at::kInt && flag.is_contiguous() && B >= 1, "keyframe_shift: flag is a device int32 [B]");
-  i64_rows(k, B, "keyframe_shift: k is a device int64 [B]");
+  arg.need(flag, "flag", at::kInt); arg.need(k, "k", at::kLong, B);
+  for (const Tensor& t : bufs) arg.on(t, "every buffer");
+  TORCH_CHECK(B >= 1, "keyframe_shift: flag is a device int32 [B]");
   TORCH_CHECK(bufs.size() == rows.size(), "keyframe_shift: one slot count per buffer");
   std::vector<void*> bases;
   std::vector<int64_t> rb, rw;
   for (size_t q = 0; q < bufs.size(); ++q) {
     const Tensor& t = bufs[q];
-    TORCH_CHECK(t.is_cuda() && t.device() == flag.device() && t.numel() > 0 && t.is_non_overlapping_and_dense(),
-                "keyframe_shift: buffer ", q, " must be a dense CUDA tensor on the flag's device");
+    TORCH_CHECK(t.numel() > 0 && t.is_non_overlapping_and_dense(), "keyframe_shift: buffer ", q, " must be a dense CUDA tensor");
     // dense: the memory order is row-major over the dimensions sorted by stride, so the slots are contiguous blocks
     // when the leading dimensions of that order hold a multiple of B * rows blocks
     std::vector<int> dims;
@@ -1007,35 +1007,28 @@ void keyframe_shift(std::vector<Tensor> bufs, std::vector<int64_t> rows, int64_t
         "dpvo_b200_ext.keyframe_shift");
 }
 void keyframe_count(int64_t mode, Tensor n, Tensor tstamp, int64_t F, Tensor counter, Tensor delta, Tensor delta_src, Tensor overflow) {
-  need_cuda(counter, "counter");
-  c10::cuda::CUDAGuard guard(counter.device());
+  const Args arg("dpvo_b200_ext.keyframe_count", counter, "counter");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int64_t B = counter.numel();
-  i64_rows(counter, B, "keyframe_count: counter is a device int64 [B]");
-  i64_rows(n, B, "keyframe_count: n is a device int64 [B]");
-  i64_rows(tstamp, B * F, "keyframe_count: tstamp is a contiguous device int64 [B, F]");
-  TORCH_CHECK(delta_src.is_cuda() && delta_src.scalar_type() == at::kLong && delta_src.is_contiguous() && delta_src.numel() % B == 0,
-              "keyframe_count: delta_src is a contiguous device int64 [B, T]");
+  arg.need(counter, "counter", at::kLong); arg.need(n, "n", at::kLong, B); arg.need(tstamp, "tstamp [B, F]", at::kLong, B * F);
+  arg.need(delta_src, "delta_src", at::kLong);
+  TORCH_CHECK(delta_src.numel() % B == 0, "keyframe_count: delta_src is [B, T]");
   const int64_t T = delta_src.numel() / B;
-  f32_rows(delta, B * T, 7, "keyframe_count: delta is a contiguous fp32 [B, T, 7]");
-  TORCH_CHECK(overflow.is_cuda() && overflow.scalar_type() == at::kInt && overflow.numel() == B, "keyframe_count: overflow is a device int32 [B]");
+  arg.need(delta, "delta [B, T, 7]", at::kFloat, B * T * 7); arg.need(overflow, "overflow", at::kInt, B);
   check(dpvo_keyframe_count((int)mode, n.data_ptr<int64_t>(), tstamp.data_ptr<int64_t>(), F, (int)B, counter.data_ptr<int64_t>(),
                             delta.data_ptr<float>(), delta_src.data_ptr<int64_t>(), T, overflow.data_ptr<int>(), stream()),
         "dpvo_b200_ext.keyframe_count");
 }
 Tensor keyframe_trajectory(Tensor poses, Tensor tstamp, Tensor n, int64_t F, Tensor delta, Tensor delta_src, Tensor counter, Tensor error) {
-  need_cuda(poses, "poses");
-  c10::cuda::CUDAGuard guard(poses.device());
+  const Args arg("dpvo_b200_ext.keyframe_trajectory", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int64_t B = n.numel();
-  i64_rows(n, B, "keyframe_trajectory: n is a device int64 [B]");
-  f32_rows(poses, B * F, 7, "keyframe_trajectory: poses are contiguous fp32 [B F, 7]");
-  i64_rows(tstamp, B * F, "keyframe_trajectory: tstamp is a contiguous device int64 [B, F]");
-  i64_rows(counter, B, "keyframe_trajectory: counter is a device int64 [B]");
-  TORCH_CHECK(delta_src.is_cuda() && delta_src.scalar_type() == at::kLong && delta_src.is_contiguous() && delta_src.numel() % B == 0,
-              "keyframe_trajectory: delta_src is a contiguous device int64 [B, T]");
+  arg.need(n, "n", at::kLong); arg.need(poses, "poses [B F, 7]", at::kFloat, B * F * 7);
+  arg.need(tstamp, "tstamp [B, F]", at::kLong, B * F); arg.need(counter, "counter", at::kLong, B);
+  arg.need(delta_src, "delta_src", at::kLong);
+  TORCH_CHECK(delta_src.numel() % B == 0, "keyframe_trajectory: delta_src is [B, T]");
   const int64_t T = delta_src.numel() / B;
-  f32_rows(delta, B * T, 7, "keyframe_trajectory: delta is a contiguous fp32 [B, T, 7]");
-  TORCH_CHECK(error.is_cuda() && error.scalar_type() == at::kInt && error.is_contiguous() && error.numel() == B,
-              "keyframe_trajectory: error is a device int32 [B]");
+  arg.need(delta, "delta [B, T, 7]", at::kFloat, B * T * 7); arg.need(error, "error", at::kInt, B);
   Tensor map = torch::empty({B, T}, poses.options().dtype(at::kInt));
   Tensor out = torch::empty({B, T, 7}, poses.options());
   check(dpvo_keyframe_trajectory(poses.data_ptr<float>(), tstamp.data_ptr<int64_t>(), n.data_ptr<int64_t>(), F, (int)B, delta.data_ptr<float>(),
@@ -1049,16 +1042,6 @@ Tensor keyframe_trajectory(Tensor poses, Tensor tstamp, Tensor n, int64_t F, Ten
 struct EncShape { int ks, s, cin, cout; };
 const EncShape kEncShapes[] = {{7, 2, 3, 32}, {3, 1, 32, 32}, {3, 2, 32, 64}, {1, 2, 32, 64}, {3, 1, 64, 64}, {1, 1, 64, 128}, {1, 1, 64, 384}};
 
-void enc_f16(const Tensor& t, const char* name) {
-  need_cuda(t, name);
-  TORCH_CHECK(t.scalar_type() == at::kHalf && t.is_contiguous(), "encoder_conv: ", name, " must be a contiguous float16 CUDA tensor");
-}
-void enc_f32(const Tensor& t, int64_t n, const char* name) {
-  need_cuda(t, name);
-  TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_contiguous() && t.numel() == n, "encoder_conv: ", name,
-              " must be a contiguous float32 CUDA tensor of ", n, " elements");
-}
-
 // one layer of one encoder; returns (y [Ho, Wo, cout], stats [2, cout] or None, joined [H, W, cin] or None, pool or None)
 std::vector<c10::optional<Tensor>> encoder_conv(int64_t shape, Tensor x, Tensor w, Tensor bias, c10::optional<Tensor> x_stats, bool x_relu,
                                                 c10::optional<Tensor> skip, c10::optional<Tensor> skip_stats, bool skip_relu,
@@ -1066,27 +1049,28 @@ std::vector<c10::optional<Tensor>> encoder_conv(int64_t shape, Tensor x, Tensor 
   TORCH_CHECK(shape >= 0 && shape < 7, "encoder_conv: unknown shape ", shape);
   const EncShape sh = kEncShapes[shape];
   const bool stem = shape == DPVO_ENC_STEM;
-  need_cuda(x, "x");
+  const Args arg("dpvo_b200_ext.encoder_conv", x, "x");
+  const c10::cuda::CUDAGuard guard(arg.dev);
   int H, W;
   dpvo_encoder_conv_io io{};
   if (stem) {
-    TORCH_CHECK(x.scalar_type() == at::kByte && x.dim() == 3 && x.size(0) == 3, "encoder_conv: the stem takes a uint8 image [3, H, W]");
+    arg.on(x, "x (the stem's image)", at::kByte);
+    TORCH_CHECK(x.dim() == 3 && x.size(0) == 3, "encoder_conv: the stem takes a uint8 image [3, H, W]");
     H = (int)x.size(1); W = (int)x.size(2);
     io.x_strides[0] = x.stride(0); io.x_strides[1] = x.stride(1); io.x_strides[2] = x.stride(2);
   } else {
-    enc_f16(x, "x");
+    arg.need(x, "x", at::kHalf);
     TORCH_CHECK(x.dim() == 3 && x.size(2) == sh.cin, "encoder_conv: x must be NHWC [H, W, ", sh.cin, "]");
     H = (int)x.size(0); W = (int)x.size(1);
   }
   const int Ho = (H + 2 * (sh.ks / 2) - sh.ks) / sh.s + 1, Wo = (W + 2 * (sh.ks / 2) - sh.ks) / sh.s + 1;
-  enc_f16(w, "w");
+  arg.need(w, "w", at::kHalf);
   const int64_t taps = stem ? 1 : sh.ks * sh.ks, kc = stem ? 20 : sh.cin / 8;
   TORCH_CHECK(w.numel() == taps * kc * sh.cout * 8, "encoder_conv: w must hold the packed layer (", taps * kc * sh.cout * 8, " halves)");
-  enc_f32(bias, sh.cout, "bias");
-  Tensor xs, ss, sk;
-  if (x_stats.has_value()) { xs = *x_stats; enc_f32(xs, 2 * sh.cin, "x_stats"); }
-  if (skip.has_value()) { sk = *skip; enc_f16(sk, "skip"); TORCH_CHECK(sk.sizes() == x.sizes(), "encoder_conv: skip must match x"); }
-  if (skip_stats.has_value()) { ss = *skip_stats; enc_f32(ss, 2 * sh.cin, "skip_stats"); }
+  arg.need(bias, "bias", at::kFloat, sh.cout);
+  Tensor xs = arg.need(x_stats, "x_stats", at::kFloat, 2 * sh.cin), sk = arg.need(skip, "skip", at::kHalf);
+  Tensor ss = arg.need(skip_stats, "skip_stats", at::kFloat, 2 * sh.cin);
+  if (sk.defined()) TORCH_CHECK(sk.sizes() == x.sizes(), "encoder_conv: skip must match x");
   auto opt16 = x.options().dtype(at::kHalf);
   Tensor y = torch::empty({Ho, Wo, sh.cout}, opt16);
   c10::optional<Tensor> st, jn, pl;
@@ -1102,47 +1086,50 @@ std::vector<c10::optional<Tensor>> encoder_conv(int64_t shape, Tensor x, Tensor 
   io.stats = st ? st->data_ptr<float>() : nullptr; io.scale = (float)scale;
   const int64_t wsb = dpvo_encoder_conv_workspace_bytes((int)shape, H, W);
   Tensor ws = byte_ws(wsb, x);
-  const c10::cuda::CUDAGuard guard(x.device());
   check(dpvo_encoder_conv((int)shape, H, W, 1, &io, ws.data_ptr(), wsb, stream()), "dpvo_b200_ext.encoder_conv");
   return {y, st, jn, pl};
 }
 
-// the viewer colours of M patch rows: a contiguous CUDA uint8 tensor of M x 3 bytes ([M, 3], or [F, M, 3] rows)
-static uint8_t* color_rows(const c10::optional<Tensor>& colors, int64_t rows, const Tensor& like, const char* what) {
-  if (!colors.has_value()) return nullptr;
-  const Tensor& c = *colors;
-  TORCH_CHECK(c.is_cuda() && c.device() == like.device() && c.scalar_type() == at::kByte && c.is_contiguous() && c.dim() >= 2 &&
-              c.size(-1) == 3 && c.numel() == rows * 3, what, ": colors must be a contiguous uint8 CUDA tensor of ", rows,
-              " rows of 3 bytes on the image's device");
+// the tensors both encode entry points take (images and rings, or one image and its slots); returns the colors or an
+// undefined tensor
+Tensor encode_args(const Args& arg, const Tensor& image, const Tensor& w16, const Tensor& b32, const Tensor& coords, const Tensor& fmap1,
+                   const Tensor& fmap2, const Tensor& gmap, const Tensor& imap, const Tensor& patches, const Tensor& workspace,
+                   const c10::optional<Tensor>& colors) {
+  arg.on(image, "image", at::kByte); arg.need(w16, "w16", at::kHalf); arg.need(b32, "b32 [2, 11, 384]", at::kFloat, 2 * 11 * 384);
+  arg.need(coords, "coords", at::kFloat); arg.on(fmap1, "fmap1", at::kHalf); arg.on(fmap2, "fmap2", at::kHalf);
+  arg.on(gmap, "gmap", at::kHalf); arg.on(imap, "imap", at::kHalf); arg.need(patches, "patches", at::kFloat);
+  arg.need(workspace, "workspace");
+  return arg.need(colors, "colors", at::kByte);
+}
+
+// the viewer colours of the patch rows: rows x 3 bytes ([M, 3], or [F, M, 3])
+uint8_t* color_rows(const Tensor& c, int64_t rows, const char* op) {
+  if (!c.defined()) return nullptr;
+  TORCH_CHECK(c.dim() >= 2 && c.size(-1) == 3 && c.numel() == rows * 3, op, ": colors must be ", rows, " rows of 3 bytes");
   return c.data_ptr<uint8_t>();
 }
 
 void encode_frame(Tensor image, Tensor w16, Tensor b32, Tensor coords, Tensor fmap1, Tensor fmap2, Tensor gmap, Tensor imap,
                   Tensor patches, Tensor workspace, c10::optional<Tensor> colors) {
-  for (auto* t : {&image, &w16, &b32, &coords, &fmap1, &fmap2, &gmap, &imap, &patches, &workspace})
-    TORCH_CHECK(t->is_cuda(), "encode_frame: every tensor must be a CUDA tensor (this build has no CPU path)");
-  TORCH_CHECK(image.scalar_type() == at::kByte && image.dim() == 3 && image.size(0) == 3, "encode_frame: image must be uint8 [3, H, W]");
+  const Args arg("dpvo_b200_ext.encode_frame", image, "image");
+  const c10::cuda::CUDAGuard guard(arg.dev);
+  const Tensor clr = encode_args(arg, image, w16, b32, coords, fmap1, fmap2, gmap, imap, patches, workspace, colors);
+  TORCH_CHECK(image.dim() == 3 && image.size(0) == 3, "encode_frame: image must be uint8 [3, H, W]");
   const int H = (int)image.size(1), W = (int)image.size(2);
   const int h = ((H - 1) / 2 + 1 - 1) / 2 + 1, w = ((W - 1) / 2 + 1 - 1) / 2 + 1;
-  TORCH_CHECK(w16.scalar_type() == at::kHalf && w16.is_contiguous(), "encode_frame: w16 must be contiguous float16");
-  TORCH_CHECK(b32.scalar_type() == at::kFloat && b32.is_contiguous() && b32.numel() == 2 * 11 * 384, "encode_frame: b32 must be float32 [2, 11, 384]");
-  TORCH_CHECK(coords.scalar_type() == at::kFloat && coords.is_contiguous() && coords.dim() == 2 && coords.size(1) == 2, "encode_frame: coords must be contiguous float32 [M, 2]");
+  TORCH_CHECK(coords.dim() == 2 && coords.size(1) == 2, "encode_frame: coords must be contiguous float32 [M, 2]");
   const int64_t M = coords.size(0);
-  TORCH_CHECK(fmap1.scalar_type() == at::kHalf && fmap1.dim() == 3 && fmap1.size(2) == 128 && fmap1.stride(2) == 1,
-              "encode_frame: fmap1 must be a channels-last float16 slot [h, w, 128]");
+  TORCH_CHECK(fmap1.dim() == 3 && fmap1.size(2) == 128 && fmap1.stride(2) == 1, "encode_frame: fmap1 must be a channels-last float16 slot [h, w, 128]");
   TORCH_CHECK(fmap1.size(0) == h && fmap1.size(1) == w, "encode_frame: a ", H, "x", W, " image encodes to ", h, "x", w,
               ", the fmap1 slot is ", fmap1.size(0), "x", fmap1.size(1));
-  TORCH_CHECK(fmap2.scalar_type() == at::kHalf && fmap2.dim() == 3 && fmap2.size(0) == h / 4 && fmap2.size(1) == w / 4 && fmap2.size(2) == 128 &&
-              fmap2.stride(2) == 1, "encode_frame: fmap2 must be a channels-last float16 slot [h/4, w/4, 128]");
-  TORCH_CHECK(gmap.scalar_type() == at::kHalf && gmap.dim() == 4 && gmap.size(0) == M && gmap.size(1) == 3 && gmap.size(2) == 3 &&
-              gmap.size(3) == 128 && gmap.stride(3) == 1, "encode_frame: gmap must be a channels-last float16 slot [M, 3, 3, 128]");
-  TORCH_CHECK(imap.scalar_type() == at::kHalf && imap.dim() == 2 && imap.size(0) == M && imap.size(1) == 384 && imap.stride(1) == 1,
-              "encode_frame: imap must be float16 [M, 384] with contiguous rows");
-  TORCH_CHECK(patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() == M * 27, "encode_frame: patches must be contiguous float32 [M, 3, 3, 3]");
-  TORCH_CHECK(workspace.is_contiguous(), "encode_frame: workspace must be contiguous");
-  const c10::cuda::CUDAGuard guard(image.device());
-  if (colors.has_value()) {
-    uint8_t* cp = color_rows(colors, M, image, "encode_frame");
+  TORCH_CHECK(fmap2.dim() == 3 && fmap2.size(0) == h / 4 && fmap2.size(1) == w / 4 && fmap2.size(2) == 128 && fmap2.stride(2) == 1,
+              "encode_frame: fmap2 must be a channels-last float16 slot [h/4, w/4, 128]");
+  TORCH_CHECK(gmap.dim() == 4 && gmap.size(0) == M && gmap.size(1) == 3 && gmap.size(2) == 3 && gmap.size(3) == 128 && gmap.stride(3) == 1,
+              "encode_frame: gmap must be a channels-last float16 slot [M, 3, 3, 128]");
+  TORCH_CHECK(imap.dim() == 2 && imap.size(0) == M && imap.size(1) == 384 && imap.stride(1) == 1, "encode_frame: imap must be float16 [M, 384] with contiguous rows");
+  TORCH_CHECK(patches.numel() == M * 27, "encode_frame: patches must be contiguous float32 [M, 3, 3, 3]");
+  if (clr.defined()) {
+    uint8_t* cp = color_rows(clr, M, "encode_frame");
     const int64_t row0 = 0;
     check(dpvo_encode_frames_colors(image.data_ptr<uint8_t>(), 0, image.stride(0), image.stride(1), image.stride(2), 1, H, W,
                                     w16.data_ptr(), b32.data_ptr<float>(), coords.data_ptr<float>(), (int)M,
@@ -1168,42 +1155,33 @@ int64_t encode_frame_workspace_bytes(int64_t H, int64_t W) { return dpvo_encode_
 void encode_frames(Tensor images, Tensor w16, Tensor b32, Tensor coords, Tensor fmap1, Tensor fmap2, Tensor gmap, Tensor imap,
                    Tensor patches, std::vector<int64_t> frame_rows, std::vector<int64_t> feat_rows, std::vector<int64_t> patch_rows,
                    c10::optional<Tensor> depth, Tensor workspace, c10::optional<Tensor> colors) {
-  for (auto* t : {&images, &w16, &b32, &coords, &fmap1, &fmap2, &gmap, &imap, &patches, &workspace})
-    TORCH_CHECK(t->is_cuda(), "encode_frames: every tensor must be a CUDA tensor (this build has no CPU path)");
-  TORCH_CHECK(images.scalar_type() == at::kByte && images.dim() == 4 && images.size(1) == 3, "encode_frames: images must be uint8 [B, 3, H, W]");
+  const Args arg("dpvo_b200_ext.encode_frames", images, "images");
+  const c10::cuda::CUDAGuard guard(arg.dev);
+  const Tensor clr = encode_args(arg, images, w16, b32, coords, fmap1, fmap2, gmap, imap, patches, workspace, colors);
+  const Tensor dep = arg.need(depth, "depth", at::kFloat);
+  TORCH_CHECK(images.dim() == 4 && images.size(1) == 3, "encode_frames: images must be uint8 [B, 3, H, W]");
   const int64_t B = images.size(0);
   const int H = (int)images.size(2), W = (int)images.size(3);
   const int h = ((H - 1) / 2 + 1 - 1) / 2 + 1, w = ((W - 1) / 2 + 1 - 1) / 2 + 1;
-  TORCH_CHECK(w16.scalar_type() == at::kHalf && w16.is_contiguous(), "encode_frames: w16 must be contiguous float16");
-  TORCH_CHECK(b32.scalar_type() == at::kFloat && b32.is_contiguous() && b32.numel() == 2 * 11 * 384, "encode_frames: b32 must be float32 [2, 11, 384]");
-  TORCH_CHECK(coords.scalar_type() == at::kFloat && coords.is_contiguous() && coords.dim() == 3 && coords.size(0) == B && coords.size(2) == 2,
-              "encode_frames: coords must be contiguous float32 [B, M, 2] with B = ", B);
+  TORCH_CHECK(coords.dim() == 3 && coords.size(0) == B && coords.size(2) == 2, "encode_frames: coords must be contiguous float32 [B, M, 2] with B = ", B);
   const int64_t M = coords.size(1);
-  TORCH_CHECK(fmap1.scalar_type() == at::kHalf && fmap1.dim() == 4 && fmap1.size(3) == 128 && fmap1.stride(3) == 1,
-              "encode_frames: fmap1 must be a channels-last float16 ring [R, h, w, 128]");
+  TORCH_CHECK(fmap1.dim() == 4 && fmap1.size(3) == 128 && fmap1.stride(3) == 1, "encode_frames: fmap1 must be a channels-last float16 ring [R, h, w, 128]");
   TORCH_CHECK(fmap1.size(1) == h && fmap1.size(2) == w, "encode_frames: a ", H, "x", W, " image encodes to ", h, "x", w,
               ", the fmap1 ring holds ", fmap1.size(1), "x", fmap1.size(2));
-  TORCH_CHECK(fmap2.scalar_type() == at::kHalf && fmap2.dim() == 4 && fmap2.size(0) == fmap1.size(0) && fmap2.size(1) == h / 4 &&
-              fmap2.size(2) == w / 4 && fmap2.size(3) == 128 && fmap2.stride(3) == 1,
-              "encode_frames: fmap2 must be a channels-last float16 ring [R, h/4, w/4, 128] with fmap1's R");
-  TORCH_CHECK(gmap.scalar_type() == at::kHalf && gmap.dim() == 4 && gmap.size(1) == 3 && gmap.size(2) == 3 && gmap.size(3) == 128 &&
-              gmap.stride(3) == 1, "encode_frames: gmap must be a channels-last float16 ring [Rg, 3, 3, 128]");
-  TORCH_CHECK(imap.scalar_type() == at::kHalf && imap.dim() == 2 && imap.size(0) == gmap.size(0) && imap.size(1) == 384 && imap.stride(1) == 1,
+  TORCH_CHECK(fmap2.dim() == 4 && fmap2.size(0) == fmap1.size(0) && fmap2.size(1) == h / 4 && fmap2.size(2) == w / 4 && fmap2.size(3) == 128 &&
+              fmap2.stride(3) == 1, "encode_frames: fmap2 must be a channels-last float16 ring [R, h/4, w/4, 128] with fmap1's R");
+  TORCH_CHECK(gmap.dim() == 4 && gmap.size(1) == 3 && gmap.size(2) == 3 && gmap.size(3) == 128 && gmap.stride(3) == 1,
+              "encode_frames: gmap must be a channels-last float16 ring [Rg, 3, 3, 128]");
+  TORCH_CHECK(imap.dim() == 2 && imap.size(0) == gmap.size(0) && imap.size(1) == 384 && imap.stride(1) == 1,
               "encode_frames: imap must be float16 [Rg, 384] with contiguous rows and gmap's Rg");
-  TORCH_CHECK(patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.dim() == 4 && patches.size(1) == 3 &&
-              patches.size(2) == 3 && patches.size(3) == 3, "encode_frames: patches must be contiguous float32 [Rp, 3, 3, 3]");
+  TORCH_CHECK(patches.dim() == 4 && patches.size(1) == 3 && patches.size(2) == 3 && patches.size(3) == 3,
+              "encode_frames: patches must be contiguous float32 [Rp, 3, 3, 3]");
   TORCH_CHECK((int64_t)frame_rows.size() == B && (int64_t)feat_rows.size() == B && (int64_t)patch_rows.size() == B,
               "encode_frames: one frame row, one patch-feature row and one patch row per image (", B, " images)");
-  const float* dp = nullptr;
-  if (depth.has_value()) {
-    TORCH_CHECK(depth->is_cuda() && depth->scalar_type() == at::kFloat && depth->is_contiguous() && depth->dim() == 2 &&
-                depth->size(0) == B && depth->size(1) == M, "encode_frames: depth must be a contiguous float32 CUDA tensor [B, M]");
-    dp = depth->data_ptr<float>();
-  }
-  TORCH_CHECK(workspace.is_contiguous(), "encode_frames: workspace must be contiguous");
-  const c10::cuda::CUDAGuard guard(images.device());
-  if (colors.has_value()) {
-    uint8_t* cp = color_rows(colors, patches.size(0), images, "encode_frames");
+  if (dep.defined()) TORCH_CHECK(dep.dim() == 2 && dep.size(0) == B && dep.size(1) == M, "encode_frames: depth must be float32 [B, M]");
+  const float* dp = dep.defined() ? dep.data_ptr<float>() : nullptr;
+  if (clr.defined()) {
+    uint8_t* cp = color_rows(clr, patches.size(0), "encode_frames");
     check(dpvo_encode_frames_colors(images.data_ptr<uint8_t>(), images.stride(0), images.stride(1), images.stride(2), images.stride(3),
                                     (int)B, H, W, w16.data_ptr(), b32.data_ptr<float>(), coords.data_ptr<float>(), (int)M,
                                     fmap1.data_ptr(), fmap1.stride(0), fmap1.stride(1), fmap1.stride(2),
@@ -1232,18 +1210,15 @@ int64_t encode_frames_workspace_bytes(int64_t B, int64_t H, int64_t W) {
 // points [B F M, 3] rows [b F M, b F M + n[b] M) of every stream b = 0 .. len(n) - 1, from poses [B F, 7], patches
 // [B F M, 3, 3, 3] and intrinsics [B F, 4]
 void point_cloud(Tensor poses, Tensor patches, Tensor intrinsics, int64_t F, std::vector<int64_t> n, Tensor points) {
-  need_cuda(poses, "poses");
-  c10::cuda::CUDAGuard guard(poses.device());
+  const Args arg("dpvo_b200_ext.point_cloud", poses, "poses");
+  c10::cuda::CUDAGuard guard(arg.dev);
   const int64_t B = (int64_t)n.size();
   TORCH_CHECK(B >= 1 && F >= 1, "point_cloud: one frame count per stream and F >= 1 needed");
-  f32_rows(poses, B * F, 7, "point_cloud: poses are contiguous fp32 [B F, 7]");
-  f32_rows(intrinsics, B * F, 4, "point_cloud: intrinsics are contiguous fp32 [B F, 4]");
-  TORCH_CHECK(patches.is_cuda() && patches.scalar_type() == at::kFloat && patches.is_contiguous() && patches.numel() % (B * F * 27) == 0 &&
-              patches.numel() > 0, "point_cloud: patches are contiguous fp32 [B F M, 3, 3, 3]");
+  arg.need(poses, "poses [B F, 7]", at::kFloat, B * F * 7); arg.need(intrinsics, "intrinsics [B F, 4]", at::kFloat, B * F * 4);
+  arg.need(patches, "patches", at::kFloat);
+  TORCH_CHECK(patches.numel() % (B * F * 27) == 0 && patches.numel() > 0, "point_cloud: patches are [B F M, 3, 3, 3]");
   const int64_t M = patches.numel() / (B * F * 27);
-  f32_rows(points, B * F * M, 3, "point_cloud: points are contiguous fp32 [B F M, 3]");
-  for (const Tensor* t : {&patches, &intrinsics, &points})
-    TORCH_CHECK(t->device() == poses.device(), "point_cloud: every tensor must be on the poses' device");
+  arg.need(points, "points [B F M, 3]", at::kFloat, B * F * M * 3);
   check(dpvo_point_cloud(poses.data_ptr<float>(), patches.data_ptr<float>(), intrinsics.data_ptr<float>(), F, (int)M, (int)B, n.data(),
                          points.data_ptr<float>(), stream()),
         "dpvo_b200_ext.point_cloud");
