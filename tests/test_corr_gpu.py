@@ -32,11 +32,10 @@ def _case(seed, M, C=128, S1=40, S2=5, H=30, W=40, dtype=torch.float32, spread=1
 @pytest.mark.parametrize("spread", [1.0, 0.25, 2.7])
 def test_corr_forward_fp32(ext, cl, spread):
     f1, f2, coords, ii, jj, f1d, f2d = _case(1, 300, spread=spread, cl=cl)
-    ref = OC.corr_forward(f1.double(), f2.double(), coords, ii, jj, 3)
+    ref, b = OC.corr_bar(f1, f2, coords, ii, jj, 3, OC.acc_generic(128))
     out, = ext[0].forward(f1d, f2d, coords.to(DEV), ii.to(DEV), jj.to(DEV), 3)
     assert out.shape == ref.shape
-    err = (out.cpu().double() - ref).abs().max().item()
-    assert err <= 1e-5 * ref.abs().max().item(), err      # fp32 accumulate vs fp64 oracle
+    assert bool(OC.within(out.cpu(), ref, b).all()), OC.bar_use(out.cpu(), ref, b).max().item()
 
 
 def test_corr_forward_fp64(ext):
@@ -49,15 +48,13 @@ def test_corr_forward_fp64(ext):
 @pytest.mark.parametrize("cl", [False, True])
 @pytest.mark.parametrize("spread", [1.0, 0.25, 2.7])
 def test_corr_forward_fp16(ext, cl, spread):
-    """cl=True, C=128 takes the tensor-core kernel; the rest the generic one.  Tolerance: one fp16
-    rounding of the result (2^-11 relative) plus fp32 accumulation noise -- the reference, which
-    accumulates in fp16 (correlation_kernel.cu:121-131), is far outside this bound itself."""
+    """cl=True, C=128 takes the mma.sync kernel; the rest the generic one.  Per element within the bar of
+    oracle/corr.py (the kernel's fp32 accumulation and blend, then one fp16 rounding) -- the reference, which
+    accumulates in fp16 (correlation_kernel.cu:121-131), is outside it (tests/test_corr_ref_cpu.py)."""
     f1, f2, coords, ii, jj, f1d, f2d = _case(3, 500, dtype=torch.half, spread=spread, cl=cl)
-    ref = OC.corr_forward(f1.double(), f2.double(), coords, ii, jj, 3)
+    ref, b = OC.corr_bar(f1, f2, coords, ii, jj, 3, OC.ACC_MMA if cl else OC.acc_generic(128))
     out, = ext[0].forward(f1d, f2d, coords.to(DEV), ii.to(DEV), jj.to(DEV), 3)
-    err = (out.cpu().double() - ref).abs()
-    tol = 2.0 ** -10 * ref.abs() + 1e-4 * ref.abs().max()
-    assert bool((err <= tol).all()), float((err - tol).max())
+    assert bool(OC.within(out.cpu(), ref, b).all()), OC.bar_use(out.cpu(), ref, b).max().item()
 
 
 def test_corr_forward_oob_is_zero(ext):
@@ -67,8 +64,8 @@ def test_corr_forward_oob_is_zero(ext):
     coords[0, 16:32] -= 1000.0
     out, = ext[0].forward(f1d, f2d, coords.to(DEV), ii.to(DEV), jj.to(DEV), 3)
     assert float(out[0, :32].abs().max()) == 0.0
-    ref = OC.corr_forward(f1.double(), f2.double(), coords, ii, jj, 3)
-    assert (out.cpu().double() - ref).abs().max().item() <= 2.0 ** -9 * ref.abs().max().item()
+    ref, b = OC.corr_bar(f1, f2, coords, ii, jj, 3, OC.ACC_MMA)
+    assert bool(OC.within(out.cpu(), ref, b).all())
 
 
 def test_corr_forward_nonfinite_coords_do_not_crash(ext):
@@ -115,9 +112,11 @@ def test_corr_pyramid2_matches_two_calls(ext, dtype):
     if dtype == torch.float32:
         assert torch.equal(fused, ref)
     else:
-        # fp16 features: the fused call runs on wgmma (fp32 accumulation in another order than mma.sync),
-        # results agree to fp16 rounding
-        assert torch.allclose(fused.float(), ref.float(), atol=2e-3, rtol=2e-3)
+        # fp16 features: level 0 of the fused call runs on wgmma (fp32 accumulation in another order than mma.sync):
+        # both levels within the bar of the fp64 oracle
+        for lev, (fm, c, n) in enumerate(((l0, coords, OC.ACC_WGMMA), (l1, OC.level_coords(coords, 4.0), OC.ACC_MMA))):
+            want, b = OC.corr_bar(f1, fm, c, ii, jj, 3, n)
+            assert bool(OC.within(fused[..., lev], want, b).all())
 
 
 @pytest.mark.parametrize("M,stretch,pad,fx,fy", [(1, 0, 0, 1, 1), (149, 3, 896, 2.7, 2.7), (5000, 7, 896, 2.7, 2.7), (3000, 0, 0, 1, 1),
@@ -133,24 +132,18 @@ def test_corr_tcgen05_vs_oracle(ext, M, stretch, pad, fx, fy):
         assert out.shape == (1, M, pad)
         assert torch.count_nonzero(out[..., 882:]) == 0
         out = out[..., :882].reshape(1, M, 7, 7, 3, 3, 2)
-    c = coords.cpu()
-    want0 = OC.corr_forward(f1.cpu().double(), l0.cpu().double(), c, ii.cpu(), jj.cpu(), 3)
-    want1 = OC.corr_forward(f1.cpu().double(), l1.cpu().double(), c / 4, ii.cpu(), jj.cpu(), 3)
-    want = torch.stack([want0, want1], -1)
-    err = (out.cpu().double() - want).abs()
-    tol = 2.0 ** -10 * want.abs() + 1e-4 * want.abs().max()    # one fp16 rounding + fp32 accumulation noise
-    assert bool((err <= tol).all()), float((err - tol).max())
+    # level 0: wgmma, or the mma.sync list kernel for stretched edges (the larger bar); level 1: mma.sync order
+    for lev, (fm, c, n) in enumerate(((l0, coords, OC.ACC_WGMMA), (l1, OC.level_coords(coords, 4.0), OC.ACC_MMA))):
+        want, b = OC.corr_bar(f1, fm, c, ii, jj, 3, n)
+        assert bool(OC.within(out[..., lev], want, b).all()), (lev, OC.bar_use(out[..., lev], want, b).max().item())
 
 
 def test_corr_tcgen05_non_pow2_divisor(ext):
     """level-1 divisor that is not a power of two takes the true-division instantiation"""
     f1, l0, l1, coords, ii, jj = _pyramid_inputs(torch.half, 700, seed=5)
     out = ext[3].corr_pyramid2(f1, l0, l1, coords, ii, jj, 3, 3.0)
-    c = coords.cpu()
-    want1 = OC.corr_forward(f1.cpu().double(), l1.cpu().double(), c / 3.0, ii.cpu(), jj.cpu(), 3)
-    err = (out[..., 1].cpu().double() - want1).abs()
-    tol = 2.0 ** -10 * want1.abs() + 1e-4 * want1.abs().max()
-    assert bool((err <= tol).all()), float((err - tol).max())
+    want1, b = OC.corr_bar(f1, l1, OC.level_coords(coords, 3.0), ii, jj, 3, OC.ACC_MMA)
+    assert bool(OC.within(out[..., 1], want1, b).all()), OC.bar_use(out[..., 1], want1, b).max().item()
 
 
 def test_corr_tcgen05_far_outside(ext):
@@ -169,12 +162,9 @@ def test_corr_backward_fp32(ext, cl):
     f1, f2, coords, ii, jj, f1d, f2d = _case(8, 60, C=128, S1=20, S2=3, H=20, W=24, cl=cl)
     g = torch.Generator().manual_seed(9)
     grad = torch.randn(1, 60, 7, 7, 3, 3, generator=g)
-    a = f1.double().requires_grad_(True)
-    b = f2.double().requires_grad_(True)
-    OC.corr_forward(a, b, coords, ii, jj, 3).backward(grad.double())
+    r1, r2, b1, b2 = OC.corr_backward_bar(f1, f2, coords, ii, jj, grad, 3)
     g1, g2 = ext[0].backward(f1d, f2d, coords.to(DEV), ii.to(DEV), jj.to(DEV), grad.to(DEV), 3)
-    assert (g1.cpu().double() - a.grad).abs().max().item() <= 2e-5 * a.grad.abs().max().item()
-    assert (g2.cpu().double() - b.grad).abs().max().item() <= 2e-5 * b.grad.abs().max().item()
+    assert bool(OC.within(g1.cpu(), r1, b1).all()) and bool(OC.within(g2.cpu(), r2, b2).all())
 
 
 @pytest.mark.parametrize("radius,C", [(0, 384), (1, 128), (0, 1), (1, 3)])
@@ -215,12 +205,10 @@ def test_altcorr_corr_autograd_with_dropout_matches_oracle(ext):
         out.backward(grad.to(DEV))
         torch.manual_seed(99)
         keep = (torch.rand(M, device=DEV) < dropout).cpu() if dropout < 1 else torch.ones(M, dtype=torch.bool)
-        a64, b64 = f1.double().requires_grad_(True), f2.double().requires_grad_(True)
-        ref = OC.corr_forward(a64, b64, coords, ii, jj, 3)
-        (ref * grad.double() * keep[None, :, None, None, None, None]).sum().backward()
-        assert (out.detach().cpu().double() - ref.detach()).abs().max().item() <= 1e-5 * ref.abs().max().item()
-        for mine, theirs in ((a.grad, a64.grad), (b.grad, b64.grad)):
-            assert (mine.cpu().double() - theirs).abs().max().item() <= 3e-5 * theirs.abs().max().item()
+        ref, bar = OC.corr_bar(f1, f2, coords, ii, jj, 3, OC.acc_generic(128))
+        assert bool(OC.within(out.detach().cpu(), ref, bar).all())
+        r1, r2, b1, b2 = OC.corr_backward_bar(f1, f2, coords, ii, jj, grad * keep[None, :, None, None, None, None], 3)
+        assert bool(OC.within(a.grad.cpu(), r1, b1).all()) and bool(OC.within(b.grad.cpu(), r2, b2).all())
 
 
 def test_altcorr_patchify_bilinear_autograd_matches_oracle(ext):

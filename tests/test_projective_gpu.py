@@ -108,3 +108,43 @@ def test_flow_mag_and_point_cloud(ext):
     pc = pops.point_cloud(SE3(poses.float().to(DEV)), patches[:, :ix.numel()].float().to(DEV), intr.float().to(DEV), ix.to(DEV))
     refpc = OL.GROUPS[3].act4(OL.GROUPS[3].inv(poses[:, ix])[:, :, None, None], OB.iproj(patches[:, :ix.numel()], intr[:, ix]))
     assert (pc.cpu().double() - refpc).abs().max().item() < 1e-4 * refpc.abs().max().item()
+
+
+def test_reproject_clamped_depth_clamp_branch(ext):
+    """reproject_clamped (the correlation's input) where the depth clamp 1 / max(Z, 0.1) acts: Z in {-1, 0, 0.05, just
+    below and above 0.1, 0.2} (frame 1 is frame 0 moved by -1 along z, so Z = 1 - d exactly in fp32), edges with
+    ii = jj, and a frame whose quaternion is 1e-3 off unit length; against oracle/ba.py's transform within a bar that
+    scales with the magnitudes: out = f X / max(Z, 0.1) + c with X, Z from fp32 rotations of |p| + |d| |t|"""
+    P = 3
+    d_just = [float(torch.tensor(0.9, dtype=torch.float32)), float(torch.nextafter(torch.tensor(0.9), torch.tensor(1.0)))]
+    depths = torch.tensor([2.0, 1.0, 0.95] + d_just + [0.8, 0.5])
+    q = torch.tensor([0.1, 0.2, 0.05, 0.97])
+    q = q / q.norm() * (1 + 1e-3)
+    poses = torch.tensor([[0, 0, 0, 0, 0, 0, 1.0], [0, 0, -1.0, 0, 0, 0, 1.0], [0.3, -0.2, -0.9] + q.tolist()])
+    intr = torch.tensor([[320.0, 300.0, 320.0, 240.0]]).repeat(3, 1)
+    g = torch.Generator().manual_seed(7)
+    N = depths.numel()
+    patches = torch.zeros(N, 3, P, P)
+    patches[:, 0] = 320 + 60 * torch.randn(N, P, P, generator=g)
+    patches[:, 1] = 240 + 60 * torch.randn(N, P, P, generator=g)
+    patches[:, 2] = depths[:, None, None]
+    pairs = [(0, 1), (1, 1), (0, 0), (0, 2), (2, 2), (2, 1), (1, 0)]
+    ii = torch.tensor([a for a, _ in pairs for _ in range(N)])
+    jj = torch.tensor([b for _, b in pairs for _ in range(N)])
+    kk = torch.arange(N).repeat(len(pairs))
+    out = ext[3].reproject_clamped(poses.to(DEV)[None], patches.to(DEV)[None], intr.to(DEV)[None], ii.to(DEV), jj.to(DEV),
+                                   kk.to(DEV))[0].cpu().double().permute(0, 2, 3, 1)           # [E, P, P, 2]
+    p64, x64, k64 = poses.double()[None], patches.double()[None], intr.double()[None]
+    ref = OB.transform(p64, x64, k64, ii, jj, kk)[0]
+    X0 = OB.iproj(x64[:, kk], k64[:, ii])
+    X1 = OL.se3_act4(OL.se3_mul(p64[:, jj], OL.se3_inv(p64[:, ii]))[:, :, None, None], X0)[0]
+    Z = X1[..., 2]
+    assert bool((Z < 0.1).any() & (Z > 0.1).any() & (Z <= 0).any() & ((Z - 0.1).abs() < 1e-7).any())
+    Zc = Z.clamp(min=0.1)
+    mag = X0[0, ..., :3].norm(dim=-1) + x64[0, kk, 2].abs() * (p64[0, ii, :3].norm(dim=-1) + p64[0, jj, :3].norm(dim=-1))[:, None, None]
+    f, c = k64[0, jj, :2][:, None, None], k64[0, jj, 2:][:, None, None]
+    XY = X1[..., :2].abs()
+    bar = 16 * 2.0 ** -24 * (f * (mag[..., None] + XY * mag[..., None] / Zc[..., None] + XY) / Zc[..., None] +
+                             f * XY / Zc[..., None] + c.abs())
+    err = (out - ref).abs()
+    assert bool((err <= bar).all()), float((err / bar).max())
