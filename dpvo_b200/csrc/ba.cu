@@ -890,42 +890,72 @@ __global__ void reproject_kernel(const float* __restrict__ poses, const float* _
 
 using namespace dpvo;
 
-// ---- workspace layout ---------------------------------------------------------------------
+// ---- workspaces and kernel arguments ---------------------------------------------------------
 namespace {
-struct BaWs {
-  int32_t *k_order, *k_of, *k_start, *k_n; int64_t* k_key;
-  int32_t *p_order, *p_of, *p_start, *p_n; int64_t *p_key_i, *p_key_j;
-  float *Ed, *Qk, *uk, *rec, *dX;
-  void* gws_k; void* gws_p; int64_t gws_bytes;
-};
-int64_t ba_ws_layout(int64_t E, int N, char* base, BaWs* w) {
-  char* p = base;
-  auto take = [&](int64_t bytes) { char* r = p; p += align256(bytes); return r; };
-  const int64_t gb = dpvo_group_workspace_bytes(E);
-  char* k_order = take(E * 4); char* k_of = take(E * 4); char* k_start = take((E + 1) * 4);
-  char* k_key = take(E * 8); char* k_n = take(4);
-  char* p_order = take(E * 4); char* p_of = take(E * 4); char* p_start = take((E + 1) * 4);
-  char* p_ki = take(E * 8); char* p_kj = take(E * 8); char* p_n = take(4);
-  char* Ed = take(E * 6 * (int64_t)std::max(N, 1) * 4);
-  char* Qk = take(E * 4); char* uk = take(E * 4);
-  char* rec = take(E * (int64_t)BA_REC * 4);
-  char* dX = take(6 * BA_MAX_N * 4);
-  char* gk = take(gb); char* gp = take(gb);
-  if (w) {
-    w->k_order = (int32_t*)k_order; w->k_of = (int32_t*)k_of; w->k_start = (int32_t*)k_start;
-    w->k_key = (int64_t*)k_key; w->k_n = (int32_t*)k_n;
-    w->p_order = (int32_t*)p_order; w->p_of = (int32_t*)p_of; w->p_start = (int32_t*)p_start;
-    w->p_key_i = (int64_t*)p_ki; w->p_key_j = (int64_t*)p_kj; w->p_n = (int32_t*)p_n;
-    w->Ed = (float*)Ed; w->Qk = (float*)Qk; w->uk = (float*)uk; w->rec = (float*)rec; w->dX = (float*)dX;
-    w->gws_k = gk; w->gws_p = gp; w->gws_bytes = gb;
-  }
-  return (int64_t)(p - base);
+// an edge grouping as dpvo_group_edges leaves it; key_j is the target frame of the pair grouping, NULL for the patches
+struct BaGroups { const int32_t* order; const int32_t* start; const int64_t* key_i; const int64_t* key_j; const int32_t* n; };
+
+// scratch of the reduce and solve kernels: Ed rows of 6 max(N, 1) floats, one dX per stream
+struct BaScratch { float *Ed, *Qk, *uk, *rec, *dX; };
+BaScratch ba_scratch_layout(int64_t E, int N, int streams, WsLayout& L) {
+  BaScratch s;
+  s.Ed = L.take<float>(E * 6 * std::max(N, 1)); s.Qk = L.take<float>(E); s.uk = L.take<float>(E);
+  s.rec = L.take<float>(E * BA_REC); s.dX = L.take<float>((int64_t)streams * 6 * BA_MAX_N);
+  return s;
 }
+
+// dpvo_ba_forward: the outputs of its two groupings (key_j: pairs only), the scratch, the two groupings' workspaces
+struct BaGrouping {
+  int32_t *order, *of, *start, *n; int64_t *key_i, *key_j;
+  BaGroups groups() const { return {order, start, key_i, key_j, n}; }
+};
+struct BaForwardWs { BaGrouping k, p; BaScratch s; void *gws_k, *gws_p; };
+BaForwardWs ba_forward_layout(int64_t E, int N, WsLayout& L) {
+  BaForwardWs w;
+  for (BaGrouping* g : {&w.k, &w.p}) {
+    g->order = L.take<int32_t>(E); g->of = L.take<int32_t>(E); g->start = L.take<int32_t>(E + 1);
+    g->key_i = L.take<int64_t>(E); g->key_j = g == &w.p ? L.take<int64_t>(E) : nullptr; g->n = L.take<int32_t>(1);
+  }
+  w.s = ba_scratch_layout(E, N, 1, L);
+  w.gws_k = L.take<char>(dpvo_group_workspace_bytes(E)); w.gws_p = L.take<char>(dpvo_group_workspace_bytes(E));
+  return w;
+}
+
+// batched: the stream bounds, then the scratch with Ed rows of 6 max_b N_b floats and one dX per stream, then
+// (every N_b <= BA_FAST_MAX_N) B x sm_count partial reduced systems
+int64_t ba_batched_part_floats(int max_free_poses) {
+  return (max_free_poses > 0 && max_free_poses <= BA_FAST_MAX_N) ? (int64_t)sm_count() * ba_packed_entries(6 * max_free_poses) : 0;
+}
+struct BaBatchedWs { int32_t* bounds; BaScratch s; float* part; };
+BaBatchedWs ba_batched_layout(int64_t E, int B, int max_free_poses, WsLayout& L) {
+  BaBatchedWs w;
+  w.bounds = L.take<int32_t>(2 * (int64_t)(B + 1)); w.s = ba_scratch_layout(E, max_free_poses, B, L);
+  w.part = L.take<float>((int64_t)B * ba_batched_part_floats(max_free_poses));
+  return w;
+}
+
+BaArgs ba_args(float* poses, float* patches, const float* intrinsics, const float* target, const float* weight,
+               const float* lmbda, const int64_t* ii, const int64_t* jj, const int64_t* kk, int64_t E, int P, int t0, int N,
+               const BaGroups& k, const BaGroups& p, const BaScratch& s) {
+  BaArgs a;
+  a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
+  a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = t0; a.N = N;
+  a.k_order = k.order; a.k_start = k.start; a.k_key = k.key_i; a.k_n = k.n;
+  a.p_order = p.order; a.p_start = p.start; a.p_key_i = p.key_i; a.p_key_j = p.key_j; a.p_n = p.n;
+  a.Ed = s.Ed; a.Qk = s.Qk; a.uk = s.uk; a.rec = s.rec; a.dX = s.dX;
+  a.part = nullptr; a.n_part = 0; a.dbg = nullptr;
+  return a;
+}
+
+// fast-path reduce, windows of up to N free poses: per warp an E row, a pair record and a packed reduced system
+size_t ba_fast_smem(int N) { return (size_t)BA_FAST_WARPS * (6 * BA_MAX_N + 96 + (size_t)ba_packed_entries(6 * N)) * sizeof(float); }
 }  // namespace
 
 extern "C" int64_t dpvo_ba_workspace_bytes(int64_t E, int n_free_poses) {
   if (E < 0) E = 0;
-  return ba_ws_layout(E, n_free_poses, nullptr, nullptr) + 256;
+  WsLayout L;
+  ba_forward_layout(E, n_free_poses, L);
+  return L.bytes() + 256;
 }
 
 static int ba_run(BaArgs& a, int iterations, cudaStream_t st) {
@@ -951,7 +981,7 @@ static int ba_run(BaArgs& a, int iterations, cudaStream_t st) {
     a.n_part = sm_count();
   }
   const bool fast = a.part != nullptr;
-  const size_t fast_smem = fast ? (size_t)BA_FAST_WARPS * (6 * BA_MAX_N + 96 + (size_t)ba_packed_entries(6 * a.N)) * sizeof(float) : 0;
+  const size_t fast_smem = fast ? ba_fast_smem(a.N) : 0;
   if (fast) {
     cudaError_t e = cudaFuncSetAttribute(ba_reduce_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem);
     if (e != cudaSuccess) return check_cuda(e, "ba_forward: cudaFuncSetAttribute (reduce)");
@@ -982,8 +1012,9 @@ static int ba_run(BaArgs& a, int iterations, cudaStream_t st) {
 
 extern "C" int64_t dpvo_ba_grouped_workspace_bytes(int64_t E, int n_free_poses) {
   if (E < 0) E = 0;
-  return align256(E * 6 * (int64_t)std::max(n_free_poses, 1) * 4) + 2 * align256(E * 4) + align256(E * (int64_t)BA_REC * 4) +
-         align256(6 * BA_MAX_N * 4) + 512;
+  WsLayout L;
+  ba_scratch_layout(E, n_free_poses, 1, L);
+  return L.bytes() + 512;
 }
 
 extern "C" int dpvo_ba_forward_grouped(float* poses, float* patches, const float* intrinsics,
@@ -1002,32 +1033,19 @@ extern "C" int dpvo_ba_forward_grouped(float* poses, float* patches, const float
   DPVO_REQUIRE(N == 0 || (p_order && p_start && p_key_i && p_key_j && p_n), "ba_forward_grouped: pair grouping missing");
   if (N > BA_MAX_N) { set_error("ba_forward_grouped: %d free poses > %d", N, BA_MAX_N); return DPVO_ERR_UNSUPPORTED; }
   if (workspace_bytes < dpvo_ba_grouped_workspace_bytes(E, N)) { set_error("ba_forward_grouped: workspace too small"); return DPVO_ERR_WORKSPACE; }
-  char* p = align256(workspace);
-  BaArgs a;
-  a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
-  a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = t0; a.N = N;
-  a.k_order = k_order; a.k_start = k_start; a.k_key = k_key; a.k_n = k_n;
-  a.p_order = p_order; a.p_start = p_start; a.p_key_i = p_key_i; a.p_key_j = p_key_j; a.p_n = p_n;
-  a.Ed = (float*)p; p += align256(E * 6 * (int64_t)std::max(N, 1) * 4);
-  a.Qk = (float*)p; p += align256(E * 4);
-  a.uk = (float*)p; p += align256(E * 4);
-  a.rec = (float*)p; p += align256(E * (int64_t)BA_REC * 4);
-  a.dX = (float*)p;
+  WsLayout L(align256(workspace));
+  const BaScratch s = ba_scratch_layout(E, N, 1, L);
+  BaArgs a = ba_args(poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, E, P, t0, N,
+                     {k_order, k_start, k_key, nullptr, k_n}, {p_order, p_start, p_key_i, p_key_j, p_n}, s);
   return ba_run(a, iterations, (cudaStream_t)stream);
-}
-
-// batched workspace: the stream bounds, then the grouped layout with Ed rows of 6 max_b N_b floats and one dX per stream,
-// then (every N_b <= BA_FAST_MAX_N) B x sm_count partial reduced systems
-static int64_t ba_batched_part_floats(int max_free_poses) {
-  return (max_free_poses > 0 && max_free_poses <= BA_FAST_MAX_N) ? (int64_t)sm_count() * ba_packed_entries(6 * max_free_poses) : 0;
 }
 
 extern "C" int64_t dpvo_ba_batched_workspace_bytes(int64_t E, int B, int max_free_poses) {
   if (E < 0) E = 0;
   if (B < 1) B = 1;
-  return align256(2 * (int64_t)(B + 1) * 4) + align256(E * 6 * (int64_t)std::max(max_free_poses, 1) * 4) + 2 * align256(E * 4) +
-         align256(E * (int64_t)BA_REC * 4) + align256((int64_t)B * 6 * BA_MAX_N * 4) +
-         align256((int64_t)B * ba_batched_part_floats(max_free_poses) * 4) + 256;
+  WsLayout L;
+  ba_batched_layout(E, B, max_free_poses, L);
+  return L.bytes() + 256;
 }
 
 extern "C" int dpvo_ba_forward_batched(float* poses, float* patches, const float* intrinsics,
@@ -1060,36 +1078,27 @@ extern "C" int dpvo_ba_forward_batched(float* poses, float* patches, const float
                k_start && k_key && k_n && p_order && p_start && p_key_i && p_key_j && p_n, "ba_forward_batched: null pointer");
   if (workspace_bytes < dpvo_ba_batched_workspace_bytes(E, B, max_n)) { set_error("ba_forward_batched: workspace too small"); return DPVO_ERR_WORKSPACE; }
   cudaStream_t st = (cudaStream_t)stream;
-  char* p = align256(workspace);
-  int32_t* bounds = (int32_t*)p; p += align256(2 * (int64_t)(B + 1) * 4);
-  BaArgs a;
-  a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
-  a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = 0; a.N = max_n;
-  a.k_order = k_order; a.k_start = k_start; a.k_key = k_key; a.k_n = k_n;
-  a.p_order = p_order; a.p_start = p_start; a.p_key_i = p_key_i; a.p_key_j = p_key_j; a.p_n = p_n;
-  a.Ed = (float*)p; p += align256(E * 6 * (int64_t)max_n * 4);
-  a.Qk = (float*)p; p += align256(E * 4);
-  a.uk = (float*)p; p += align256(E * 4);
-  a.rec = (float*)p; p += align256(E * (int64_t)BA_REC * 4);
-  a.dX = (float*)p; p += align256((int64_t)B * 6 * BA_MAX_N * 4);
-  a.dbg = nullptr;
+  WsLayout L(align256(workspace));
+  const BaBatchedWs w = ba_batched_layout(E, B, max_n, L);
+  BaArgs a = ba_args(poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, E, P, 0, max_n,
+                     {k_order, k_start, k_key, nullptr, k_n}, {p_order, p_start, p_key_i, p_key_j, p_n}, w.s);
   // the fast path applies to the whole batch when every window fits it, the general path otherwise
   const bool fast = max_n <= BA_FAST_MAX_N;
-  a.part = fast ? (float*)p : nullptr;
+  a.part = fast ? w.part : nullptr;
   a.n_part = fast ? sm_count() : 0;
   bb.part_stride = ba_batched_part_floats(max_n);
   bb.ed_pitch = 6 * (int64_t)max_n;
-  bb.bounds = bounds;
+  bb.bounds = w.bounds;
   {
     const int64_t items = E + 2;                 // at most Gk + 1 + Gp + 1 <= E + 2
     const unsigned grid = (unsigned)std::min<int64_t>((items + 255) / 256, (int64_t)sm_count() * 4);
-    ba_stream_bounds_kernel<<<grid, 256, 0, st>>>(k_key, k_n, p_key_i, p_n, bb.FM, bb.F, B, bounds);
+    ba_stream_bounds_kernel<<<grid, 256, 0, st>>>(k_key, k_n, p_key_i, p_n, bb.FM, bb.F, B, w.bounds);
     DPVO_LAUNCH_CHECK("ba_stream_bounds_kernel");
   }
   cudaError_t e = cudaFuncSetAttribute(ba_solve_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SolveSmem));
   if (e != cudaSuccess) return check_cuda(e, "ba_forward_batched: cudaFuncSetAttribute");
   // shared memory sized for the widest window of the batch
-  const size_t fast_smem = fast ? (size_t)BA_FAST_WARPS * (6 * BA_MAX_N + 96 + (size_t)ba_packed_entries(6 * max_n)) * sizeof(float) : 0;
+  const size_t fast_smem = fast ? ba_fast_smem(max_n) : 0;
   if (fast) {
     e = cudaFuncSetAttribute(ba_reduce_batched_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem);
     if (e != cudaSuccess) return check_cuda(e, "ba_forward_batched: cudaFuncSetAttribute (reduce)");
@@ -1126,25 +1135,17 @@ extern "C" int dpvo_ba_forward(float* poses, float* patches, const float* intrin
     return DPVO_ERR_WORKSPACE;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  char* base = align256(workspace);
-  BaWs w;
-  ba_ws_layout(E, N, base, &w);
-
-  int rc = dpvo_group_edges(kk, nullptr, nullptr, E, w.k_order, w.k_of, w.k_start, w.k_key, nullptr, w.k_n,
-                            w.gws_k, w.gws_bytes, st);
+  WsLayout L(align256(workspace));
+  const BaForwardWs w = ba_forward_layout(E, N, L);
+  const int64_t gb = dpvo_group_workspace_bytes(E);
+  int rc = dpvo_group_edges(kk, nullptr, nullptr, E, w.k.order, w.k.of, w.k.start, w.k.key_i, nullptr, w.k.n, w.gws_k, gb, st);
   if (rc) return rc;
   if (N > 0) {
-    rc = dpvo_group_edges(ii, jj, nullptr, E, w.p_order, w.p_of, w.p_start, w.p_key_i, w.p_key_j, w.p_n,
-                          w.gws_p, w.gws_bytes, st);
+    rc = dpvo_group_edges(ii, jj, nullptr, E, w.p.order, w.p.of, w.p.start, w.p.key_i, w.p.key_j, w.p.n, w.gws_p, gb, st);
     if (rc) return rc;
   }
-
-  BaArgs a;
-  a.poses = poses; a.patches = patches; a.intrinsics = intrinsics; a.target = target; a.weight = weight;
-  a.lmbda = lmbda; a.ii = ii; a.jj = jj; a.kk = kk; a.E = E; a.P = P; a.t0 = t0; a.N = N;
-  a.k_order = w.k_order; a.k_start = w.k_start; a.k_key = w.k_key; a.k_n = w.k_n;
-  a.p_order = w.p_order; a.p_start = w.p_start; a.p_key_i = w.p_key_i; a.p_key_j = w.p_key_j; a.p_n = w.p_n;
-  a.Ed = w.Ed; a.Qk = w.Qk; a.uk = w.uk; a.rec = w.rec; a.dX = w.dX;
+  // from here on the path of dpvo_ba_forward_grouped
+  BaArgs a = ba_args(poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, E, P, t0, N, w.k.groups(), w.p.groups(), w.s);
   return ba_run(a, iterations, st);
 }
 

@@ -66,6 +66,19 @@ inline size_t dtype_size(int dtype) {
 inline int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
 inline char* align256(void* p) { return (char*)(((uintptr_t)p + 255) & ~(uintptr_t)255); }
 
+// Carves a workspace into consecutive arrays, each rounded up to `align` bytes.  On a null base it only measures, so
+// one layout function gives both a workspace's size (bytes()) and, on the real base, its arrays: the two cannot differ.
+struct WsLayout {
+  char* base; int64_t align, used = 0;
+  explicit WsLayout(void* b = nullptr, int64_t a = 256) : base((char*)b), align(a) {}
+  template <typename T> T* take(int64_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+    used += (count * (int64_t)sizeof(T) + align - 1) / align * align;
+    return p;
+  }
+  int64_t bytes() const { return used; }
+};
+
 // ---- scalar conversion ------------------------------------------------------------------
 template <typename T> struct acc_of { using type = float; };
 template <> struct acc_of<double> { using type = double; };

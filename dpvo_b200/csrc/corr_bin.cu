@@ -41,11 +41,8 @@ struct __align__(16) CbWarpSmem {
 };
 constexpr size_t CB_SMEM = CB_REGION_BYTES + 256 + CB_WARPS * sizeof(CbWarpSmem);
 
-// workspace (int32 words): hdr[4] = {list count, binned count, item count, -} | list[M] | order[M] | key[M] | rank[M] |
-// cnt[K] | off[K] | items[I] (int4: key, first index into order, edges), K = 2M + 4096 bins, I = K + ceil(M / CB_ITEM)
 static int64_t cb_key_cap(int64_t M) { return 2 * M + 4096; }
 static int64_t cb_item_cap(int64_t M) { return cb_key_cap(M) + (M + CB_ITEM - 1) / CB_ITEM; }
-int64_t corr_bin_workspace_bytes(int64_t M) { return 4 * (4 + 4 * M + 2 * cb_key_cap(M)) + 16 * cb_item_cap(M) + 16; }
 
 struct CbBinArgs {
   const float* coords; const int64_t* jj;
@@ -53,6 +50,15 @@ struct CbBinArgs {
   int M, S2, nty, ntx;
   int* hdr; int* list; int* order; int* key; int* rank; int* cnt; int* off; int4* items;
 };
+
+// workspace, packed in int32 words: hdr[4] = {list count, binned count, item count, -} | list[M] | order[M] | key[M] |
+// rank[M] | cnt[K] | off[K] | items[I] (int4: key, first index into order, edges), K = 2M + 4096 bins,
+// I = K + ceil(M / CB_ITEM).  8M + 8196 words precede items: 16-byte aligned in a 16-byte aligned workspace.
+static void cb_regions(int64_t M, WsLayout& L, CbBinArgs& b) {
+  b.hdr = L.take<int>(4); b.list = L.take<int>(M); b.order = L.take<int>(M); b.key = L.take<int>(M); b.rank = L.take<int>(M);
+  b.cnt = L.take<int>(cb_key_cap(M)); b.off = L.take<int>(cb_key_cap(M)); b.items = L.take<int4>(cb_item_cap(M));
+}
+int64_t corr_bin_workspace_bytes(int64_t M) { CbBinArgs b; WsLayout L(nullptr, sizeof(int)); cb_regions(M, L, b); return L.bytes() + 16; }
 
 __global__ void __launch_bounds__(256) corr_bin_count(const CbBinArgs a) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -289,9 +295,8 @@ static CbBinArgs cb_layout(void* workspace, int M, int S2, int H1, int W1, float
   CbBinArgs b;
   b.div1 = div1; b.M = M; b.S2 = S2;
   b.nty = (H1 + CB_APRON + CB_T1 - 1) / CB_T1; b.ntx = (W1 + CB_APRON + CB_T1 - 1) / CB_T1;
-  int* w = reinterpret_cast<int*>(workspace);
-  b.hdr = w; b.list = w + 4; b.order = b.list + M; b.key = b.order + M; b.rank = b.key + M;
-  b.cnt = b.rank + M; b.off = b.cnt + cb_key_cap(M); b.items = reinterpret_cast<int4*>(b.off + cb_key_cap(M));
+  WsLayout L(workspace, sizeof(int));
+  cb_regions(M, L, b);
   return b;
 }
 

@@ -316,10 +316,14 @@ __global__ void neighbors_kernel(const int32_t* __restrict__ order, const int32_
   }
 }
 
-static int64_t group_ws_bytes(int64_t E) {
+// the grouping's workspace: header, the two permutation buffers of the radix passes, the tile-major digit histogram
+// and the tile sums of the group-boundary scan
+static void group_layout(int64_t E, WsLayout& L, GroupArgs& a) {
   const int64_t ntiles = (E + G_TILE - 1) / G_TILE;
-  return align256(sizeof(GroupHeader)) + 2 * align256(E * 4) + align256(ntiles * (int64_t)G_BINS * 4) + align256((ntiles + 1) * 4);
+  a.hdr = L.take<GroupHeader>(1); a.buf0 = L.take<int32_t>(E); a.buf1 = L.take<int32_t>(E);
+  a.hist = L.take<unsigned>(ntiles * G_BINS); a.tile_sums = L.take<int32_t>(ntiles + 1);
 }
+static int64_t group_ws_bytes(int64_t E) { GroupArgs a; WsLayout L; group_layout(E, L, a); return L.bytes(); }
 
 struct GroupProblem {
   const int64_t* ka; const int64_t* kb; const int64_t* sec; int64_t E;
@@ -337,12 +341,8 @@ static int group_fill(const GroupProblem& p, GroupArgs& a, cudaStream_t st) {
   a.ka = p.ka; a.kb = p.kb; a.sec = p.sec; a.E = E; a.ntiles = (int)((E + G_TILE - 1) / G_TILE);
   a.order = p.order; a.group_of = p.group_of; a.group_start = p.group_start;
   a.group_key_a = p.gka; a.group_key_b = p.gkb; a.n_groups = p.n_groups;
-  char* q = (char*)p.ws;
-  a.hdr = (GroupHeader*)q; q += align256(sizeof(GroupHeader));
-  a.buf0 = (int32_t*)q; q += align256(E * 4);
-  a.buf1 = (int32_t*)q; q += align256(E * 4);
-  a.hist = (unsigned*)q; q += align256((int64_t)a.ntiles * G_BINS * 4);
-  a.tile_sums = (int32_t*)q;
+  WsLayout L(p.ws);
+  group_layout(E, L, a);
   int rc = check_cuda(cudaMemsetAsync(a.hdr, 0, sizeof(GroupHeader), st), "group_edges: memset");
   if (rc) return rc;
   if (E == 0) {
@@ -377,14 +377,6 @@ static int group_launch_n(const GroupProblem* p0, const GroupProblem* p1, cudaSt
   return DPVO_OK;
 }
 
-static int group_launch(const int64_t* ka, const int64_t* kb, const int64_t* sec, int64_t E,
-                        int32_t* order, int32_t* group_of, int32_t* group_start,
-                        int64_t* gka, int64_t* gkb, int32_t* n_groups,
-                        void* ws, int64_t ws_bytes, cudaStream_t st) {
-  GroupProblem p{ka, kb, sec, E, order, group_of, group_start, gka, gkb, n_groups, ws, ws_bytes};
-  return group_launch_n(&p, nullptr, st);
-}
-
 }  // namespace dpvo
 
 using namespace dpvo;
@@ -398,8 +390,8 @@ extern "C" int dpvo_group_edges(const int64_t* key_a, const int64_t* key_b, cons
   DPVO_REQUIRE(E >= 0, "group_edges: negative E");
   DPVO_REQUIRE(order && group_of && group_start && group_key_a && n_groups && workspace, "group_edges: null pointer");
   DPVO_REQUIRE(E == 0 || key_a, "group_edges: null key");
-  return group_launch(key_a, key_b, sec, E, order, group_of, group_start, group_key_a, group_key_b, n_groups,
-                      workspace, workspace_bytes, (cudaStream_t)stream);
+  GroupProblem p{key_a, key_b, sec, E, order, group_of, group_start, group_key_a, group_key_b, n_groups, workspace, workspace_bytes};
+  return group_launch_n(&p, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int dpvo_group_edges_pair(const int64_t* key_a0, const int64_t* key_b0, const int64_t* sec0,
@@ -419,10 +411,18 @@ extern "C" int dpvo_group_edges_pair(const int64_t* key_a0, const int64_t* key_b
   return group_launch_n(&p0, &p1, (cudaStream_t)stream);
 }
 
+// dpvo_neighbors: the edges grouped by ii and ordered by jj -- the grouping's outputs, then its workspace
+static GroupProblem neighbors_layout(const int64_t* ii, const int64_t* jj, int64_t E, WsLayout& L) {
+  GroupProblem p{ii, nullptr, jj, E};
+  p.order = L.take<int32_t>(E); p.group_of = L.take<int32_t>(E); p.group_start = L.take<int32_t>(E + 1);
+  p.gka = L.take<int64_t>(E); p.n_groups = L.take<int32_t>(1); p.ws = L.take<char>(group_ws_bytes(E));
+  return p;
+}
+
 extern "C" int64_t dpvo_neighbors_workspace_bytes(int64_t E) {
-  if (E < 0) E = 0;
-  // order, group_of, group_start(+1), group_key, n_groups + the grouping workspace
-  return group_ws_bytes(E) + 2 * align256(E * 4) + align256((E + 1) * 4) + align256(E * 8) + 256;
+  WsLayout L;
+  neighbors_layout(nullptr, nullptr, E < 0 ? 0 : E, L);
+  return L.bytes();
 }
 
 extern "C" int dpvo_neighbors(const int64_t* ii, const int64_t* jj, int64_t E,
@@ -435,19 +435,15 @@ extern "C" int dpvo_neighbors(const int64_t* ii, const int64_t* jj, int64_t E,
     set_error("neighbors: workspace too small");
     return DPVO_ERR_WORKSPACE;
   }
-  char* p = (char*)workspace;
-  int32_t* order = (int32_t*)p; p += align256(E * 4);
-  int32_t* group_of = (int32_t*)p; p += align256(E * 4);
-  int32_t* group_start = (int32_t*)p; p += align256((E + 1) * 4);
-  int64_t* gkey = (int64_t*)p; p += align256(E * 8);
-  int32_t* ng = (int32_t*)p; p += 256;
+  WsLayout L(workspace);
+  GroupProblem p = neighbors_layout(ii, jj, E, L);
+  p.ws_bytes = workspace_bytes - ((char*)p.ws - (char*)workspace);
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = group_launch(ii, nullptr, jj, E, order, group_of, group_start, gkey, nullptr, ng, p,
-                        workspace_bytes - (p - (char*)workspace), st);
+  int rc = group_launch_n(&p, nullptr, st);
   if (rc) return rc;
   const int threads = 256;
   const unsigned blocks = (unsigned)std::min<int64_t>((E + threads - 1) / threads, (int64_t)sm_count() * 8);
-  neighbors_kernel<<<blocks, threads, 0, st>>>(order, group_of, E, ix, jx);
+  neighbors_kernel<<<blocks, threads, 0, st>>>(p.order, p.group_of, E, ix, jx);
   DPVO_LAUNCH_CHECK("neighbors_kernel");
   return DPVO_OK;
 }
