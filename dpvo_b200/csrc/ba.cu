@@ -968,10 +968,6 @@ static int ba_run(BaArgs& a, int iterations, cudaStream_t st) {
   const bool timing = false;
   a.dbg = nullptr;
 #endif
-  {   // per-device function attribute: set on every call (a process-wide flag would miss the second GPU)
-    cudaError_t e = cudaFuncSetAttribute(ba_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SolveSmem));
-    if (e != cudaSuccess) return check_cuda(e, "ba_forward: cudaFuncSetAttribute");
-  }
   const int red_blocks = sm_count() * 4;
   // sliding-window sizes: the reduced system is assembled by the reduce kernel (one partial per CTA, stored where the
   // pair records of the general path would go -- the fast path does not materialise them)
@@ -981,17 +977,11 @@ static int ba_run(BaArgs& a, int iterations, cudaStream_t st) {
     a.n_part = sm_count();
   }
   const bool fast = a.part != nullptr;
-  const size_t fast_smem = fast ? ba_fast_smem(a.N) : 0;
-  if (fast) {
-    cudaError_t e = cudaFuncSetAttribute(ba_reduce_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem);
-    if (e != cudaSuccess) return check_cuda(e, "ba_forward: cudaFuncSetAttribute (reduce)");
-  }
   for (int it = 0; it < iterations; ++it) {
-    if (fast) ba_reduce_kernel<true><<<a.n_part, BA_FAST_WARPS * 32, fast_smem, st>>>(a);
-    else ba_reduce_kernel<false><<<red_blocks, BA_RED_WARPS * 32, BA_RED_WARPS * 6 * BA_MAX_N * sizeof(float), st>>>(a);
-    DPVO_LAUNCH_CHECK("ba_reduce_kernel");
-    ba_solve_kernel<<<BA_CLUSTER, BA_SOLVE_THREADS, sizeof(SolveSmem), st>>>(a);
-    DPVO_LAUNCH_CHECK("ba_solve_kernel");
+    int rc = fast ? launch("ba_reduce_kernel", ba_reduce_kernel<true>, a.n_part, BA_FAST_WARPS * 32, ba_fast_smem(a.N), st, a)
+                  : launch("ba_reduce_kernel", ba_reduce_kernel<false>, red_blocks, BA_RED_WARPS * 32, BA_RED_WARPS * 6 * BA_MAX_N * sizeof(float), st, a);
+    if (!rc) rc = launch("ba_solve_kernel", ba_solve_kernel, BA_CLUSTER, BA_SOLVE_THREADS, sizeof(SolveSmem), st, a);
+    if (rc) return rc;
   }
 #ifdef DPVO_B200_PERF_EXPERIMENTS
   if (timing) {
@@ -1092,23 +1082,16 @@ extern "C" int dpvo_ba_forward_batched(float* poses, float* patches, const float
   {
     const int64_t items = E + 2;                 // at most Gk + 1 + Gp + 1 <= E + 2
     const unsigned grid = (unsigned)std::min<int64_t>((items + 255) / 256, (int64_t)sm_count() * 4);
-    ba_stream_bounds_kernel<<<grid, 256, 0, st>>>(k_key, k_n, p_key_i, p_n, bb.FM, bb.F, B, w.bounds);
-    DPVO_LAUNCH_CHECK("ba_stream_bounds_kernel");
-  }
-  cudaError_t e = cudaFuncSetAttribute(ba_solve_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SolveSmem));
-  if (e != cudaSuccess) return check_cuda(e, "ba_forward_batched: cudaFuncSetAttribute");
-  // shared memory sized for the widest window of the batch
-  const size_t fast_smem = fast ? ba_fast_smem(max_n) : 0;
-  if (fast) {
-    e = cudaFuncSetAttribute(ba_reduce_batched_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fast_smem);
-    if (e != cudaSuccess) return check_cuda(e, "ba_forward_batched: cudaFuncSetAttribute (reduce)");
+    const int rc = launch("ba_stream_bounds_kernel", ba_stream_bounds_kernel, grid, 256, 0, st, k_key, k_n, p_key_i, p_n, bb.FM, bb.F, B, w.bounds);
+    if (rc) return rc;
   }
   for (int it = 0; it < iterations; ++it) {
-    if (fast) ba_reduce_batched_kernel<true><<<dim3(a.n_part, B), BA_FAST_WARPS * 32, fast_smem, st>>>(a, bb);
-    else ba_reduce_batched_kernel<false><<<dim3(sm_count() * 4, B), BA_RED_WARPS * 32, BA_RED_WARPS * 6 * BA_MAX_N * sizeof(float), st>>>(a, bb);
-    DPVO_LAUNCH_CHECK("ba_reduce_batched_kernel");
-    ba_solve_batched_kernel<<<BA_CLUSTER * B, BA_SOLVE_THREADS, sizeof(SolveSmem), st>>>(a, bb);
-    DPVO_LAUNCH_CHECK("ba_solve_batched_kernel");
+    // shared memory sized for the widest window of the batch
+    int rc = fast ? launch("ba_reduce_batched_kernel", ba_reduce_batched_kernel<true>, dim3(a.n_part, B), BA_FAST_WARPS * 32, ba_fast_smem(max_n), st, a, bb)
+                  : launch("ba_reduce_batched_kernel", ba_reduce_batched_kernel<false>, dim3(sm_count() * 4, B), BA_RED_WARPS * 32,
+                           BA_RED_WARPS * 6 * BA_MAX_N * sizeof(float), st, a, bb);
+    if (!rc) rc = launch("ba_solve_batched_kernel", ba_solve_batched_kernel, BA_CLUSTER * B, BA_SOLVE_THREADS, sizeof(SolveSmem), st, a, bb);
+    if (rc) return rc;
   }
   return DPVO_OK;
 }
@@ -1157,8 +1140,6 @@ extern "C" int dpvo_reproject(const float* poses, const float* patches, const fl
   DPVO_REQUIRE(poses && patches && intrinsics && ii && jj && kk && coords, "reproject: null pointer");
   const int threads = 128;
   const unsigned blocks = (unsigned)std::min<int64_t>((E + threads - 1) / threads, (int64_t)sm_count() * 16);
-  if (clamp_depth) reproject_kernel<true><<<blocks, threads, 0, (cudaStream_t)stream>>>(poses, patches, intrinsics, ii, jj, kk, coords, E, P);
-  else reproject_kernel<false><<<blocks, threads, 0, (cudaStream_t)stream>>>(poses, patches, intrinsics, ii, jj, kk, coords, E, P);
-  DPVO_LAUNCH_CHECK("reproject_kernel");
-  return DPVO_OK;
+  return launch("reproject_kernel", clamp_depth ? reproject_kernel<true> : reproject_kernel<false>, blocks, threads, 0, (cudaStream_t)stream, poses,
+                patches, intrinsics, ii, jj, kk, coords, E, P);
 }

@@ -277,16 +277,11 @@ extern "C" int dpvo_ba_wide_system(float* poses, float* patches, const float* in
   if (rc) return rc;
   rc = check_cuda(cudaMemsetAsync(y, 0, (size_t)N6 * 4, st), "ba_wide_system: memset");
   if (rc) return rc;
-  if (E > 0) {
-    const size_t smem = bw_smem_bytes(a.max_blocks, PPF);
-    cudaError_t e = cudaFuncSetAttribute(ba_wide_frame_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return check_cuda(e, "ba_wide_system: cudaFuncSetAttribute");
-    ba_wide_frame_kernel<true><<<(unsigned)t1, BW_THREADS, smem, st>>>(a);     // source frames are 0 .. t1-1
-    DPVO_LAUNCH_CHECK("ba_wide_frame_kernel<system>");
+  if (E > 0) {     // source frames are 0 .. t1-1
+    rc = launch("ba_wide_frame_kernel<system>", ba_wide_frame_kernel<true>, (unsigned)t1, BW_THREADS, bw_smem_bytes(a.max_blocks, PPF), st, a);
+    if (rc) return rc;
   }
-  ba_wide_damp_kernel<<<(N6 + 127) / 128, 128, 0, st>>>(S, N6);
-  DPVO_LAUNCH_CHECK("ba_wide_damp_kernel");
-  return DPVO_OK;
+  return launch("ba_wide_damp_kernel", ba_wide_damp_kernel, (N6 + 127) / 128, 128, 0, st, S, N6);
 }
 
 // Apply a solved pose step dX [6 (t1 - t0)]: depth back-substitution + retraction, then pose retraction.
@@ -302,15 +297,10 @@ extern "C" int dpvo_ba_wide_update(float* poses, float* patches, const float* in
   bw_fill(a, poses, patches, intrinsics, target, weight, lmbda, ii, jj, kk, E, P, PPF, t0, t1, p_order, p_start, p_key_i, p_key_j, p_n, status);
   a.dX = dX;
   if (E > 0) {
-    const size_t smem = bw_smem_bytes(a.max_blocks, PPF);
-    cudaError_t e = cudaFuncSetAttribute(ba_wide_frame_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return check_cuda(e, "ba_wide_update: cudaFuncSetAttribute");
-    ba_wide_frame_kernel<false><<<(unsigned)t1, BW_THREADS, smem, st>>>(a);
-    DPVO_LAUNCH_CHECK("ba_wide_frame_kernel<update>");
+    const int rc = launch("ba_wide_frame_kernel<update>", ba_wide_frame_kernel<false>, (unsigned)t1, BW_THREADS, bw_smem_bytes(a.max_blocks, PPF), st, a);
+    if (rc) return rc;
   }
-  ba_wide_pose_kernel<<<(a.N + 63) / 64, 64, 0, st>>>(poses, dX, t0, a.N);
-  DPVO_LAUNCH_CHECK("ba_wide_pose_kernel");
-  return DPVO_OK;
+  return launch("ba_wide_pose_kernel", ba_wide_pose_kernel, (a.N + 63) / 64, 64, 0, st, poses, dX, t0, a.N);
 }
 
 // ---- cuda_ba.solve_system: pose-graph normal equations (ba.cpp:120-167) ---------------------------------------------
@@ -355,10 +345,8 @@ extern "C" int dpvo_posegraph_system(const float* J_i, const float* J_j, const i
   if (rc) return rc;
   if (r > 0) {
     const int64_t total = r * 196;
-    posegraph_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(J_i, J_j, ii, jj, res, r, n, A, b);
-    DPVO_LAUNCH_CHECK("posegraph_kernel");
+    rc = launch("posegraph_kernel", posegraph_kernel, (unsigned)((total + 255) / 256), 256, 0, st, J_i, J_j, ii, jj, res, r, n, A, b);
+    if (rc) return rc;
   }
-  posegraph_damp_kernel<<<(unsigned)((n7 + 127) / 128), 128, 0, st>>>(A, n7, ep, lm);
-  DPVO_LAUNCH_CHECK("posegraph_damp_kernel");
-  return DPVO_OK;
+  return launch("posegraph_damp_kernel", posegraph_damp_kernel, (unsigned)((n7 + 127) / 128), 128, 0, st, A, n7, ep, lm);
 }

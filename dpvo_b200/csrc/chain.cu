@@ -592,7 +592,7 @@ using namespace dpvo;
 struct ChainMaps { CUtensorMap X, W0, W; };
 
 // how many CH_CL-CTA clusters of chain_kernel<CHAIN> the current device runs at once; queried once per device, after the
-// shared-memory attribute is set
+// shared-memory limit is raised
 template <int CHAIN>
 static int chain_max_clusters(int* n) {
   constexpr int kDevices = 64;
@@ -601,6 +601,7 @@ static int chain_max_clusters(int* n) {
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return check_cuda(e, "update chain: cudaGetDevice");
   if (dev < kDevices && (*n = cached[dev].load(std::memory_order_relaxed)) > 0) return DPVO_OK;
+  if (int rc = allow_smem("update chain", chain_kernel<CHAIN>, ChainCfg<CHAIN>::SMEM)) return rc;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(CH_CL);
   cfg.blockDim = dim3(CH_THREADS);
@@ -617,17 +618,13 @@ static int chain_max_clusters(int* n) {
 
 template <int CHAIN>
 static int chain_launch(const ChainMaps& m, const ChainArgs& a, cudaStream_t st) {
-  cudaError_t e = cudaFuncSetAttribute(chain_kernel<CHAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ChainCfg<CHAIN>::SMEM);
-  if (e != cudaSuccess) return check_cuda(e, "update chain: cudaFuncSetAttribute");
   int max_clusters = 0;
   if (int rc = chain_max_clusters<CHAIN>(&max_clusters)) return rc;
   const int64_t groups = ((a.rows + CH_M - 1) / CH_M + CH_CL - 1) / CH_CL;
   // at most one CTA per SM: chain G's scratch holds sm_count() CTA slots, indexed by blockIdx.x
   const int64_t clusters = std::min<int64_t>({groups, (int64_t)max_clusters, (int64_t)(sm_count() / CH_CL)});
   const unsigned grid = (unsigned)(clusters * CH_CL);
-  chain_kernel<CHAIN><<<grid, CH_THREADS, ChainCfg<CHAIN>::SMEM, st>>>(m.X, m.W0, m.W, a);
-  DPVO_LAUNCH_CHECK("chain_kernel");
-  return DPVO_OK;
+  return launch("chain_kernel", chain_kernel<CHAIN>, grid, CH_THREADS, ChainCfg<CHAIN>::SMEM, st, m.X, m.W0, m.W, a);
 }
 
 static bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }

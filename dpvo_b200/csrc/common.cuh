@@ -9,6 +9,7 @@
 #include <atomic>
 #include <algorithm>
 #include <cstdlib>
+#include <utility>
 
 #include "../../include/dpvo_b200.h"
 
@@ -24,17 +25,6 @@ inline int check_cuda(cudaError_t e, const char* what) {
   return DPVO_ERR_CUDA;
 }
 
-// Call after every kernel launch: counts the launch and surfaces launch-configuration errors.
-#define DPVO_LAUNCH_CHECK(name)                                           \
-  do {                                                                    \
-    ::dpvo::g_launches.fetch_add(1, std::memory_order_relaxed);           \
-    cudaError_t _e = cudaPeekAtLastError();                               \
-    if (_e != cudaSuccess) {                                              \
-      cudaGetLastError();                                                 \
-      return ::dpvo::check_cuda(_e, name);                                \
-    }                                                                     \
-  } while (0)
-
 #define DPVO_REQUIRE(cond, ...)                                           \
   do {                                                                    \
     if (!(cond)) {                                                        \
@@ -43,14 +33,49 @@ inline int check_cuda(cudaError_t e, const char* what) {
     }                                                                     \
   } while (0)
 
+// SM count of the current device, asked once per device (132 when it cannot be asked)
 inline int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 132;
-  }
+  constexpr int kDevices = 64;
+  static std::atomic<int> cached[kDevices];                          // 0 = not asked yet
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (dev < kDevices && (n = cached[dev].load(std::memory_order_relaxed)) > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 132;
+  if (dev < kDevices) cached[dev].store(n, std::memory_order_relaxed);
   return n;
+}
+
+// Lets `kernel` take `smem` bytes of dynamic shared memory on the current device.  Above the 48 KiB default this is needed
+// before a launch, and before an occupancy query that is to count such CTAs.  The limit is a per-device attribute, so it
+// is set on every call.
+template <typename K> int allow_smem(const char* name, K* kernel, size_t smem) {
+  if (smem <= 48 * 1024) return DPVO_OK;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess) return DPVO_OK;
+  cudaGetLastError();
+  set_error("%s: cudaFuncSetAttribute: %s", name, cudaGetErrorString(e));
+  return DPVO_ERR_CUDA;
+}
+
+// Launches `kernel` on stream `st` and counts it in dpvo_launch_count().  ATTR, when given, is a launch attribute switched
+// on for this launch (cudaLaunchAttributeCooperative: a grid whose CTAs synchronise).  A failed launch returns its own
+// error as "<name>: <error>" and leaves no pending error behind.
+template <cudaLaunchAttributeID ATTR = cudaLaunchAttributeIgnore, typename... P, typename... A>
+int launch(const char* name, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+  if (int rc = allow_smem(name, kernel, smem)) return rc;
+  cudaLaunchAttribute attr;
+  attr.id = ATTR;
+  attr.val.cooperative = 1;
+  cudaLaunchConfig_t cfg;
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cfg.attrs = &attr; cfg.numAttrs = ATTR == cudaLaunchAttributeIgnore ? 0 : 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return check_cuda(e, name);
+  }
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return DPVO_OK;
 }
 
 inline size_t dtype_size(int dtype) {

@@ -615,15 +615,12 @@ static int launch_bwd(const CorrBwdArgs& a, cudaStream_t st) {
   const int64_t nitems = (int64_t)a.B * a.M;
   if (nitems == 0) return DPVO_OK;
   auto go = [&](auto kern) -> int {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return check_cuda(e, "corr_backward: cudaFuncSetAttribute");
+    if (int rc = allow_smem("corr_bwd_generic", kern, smem)) return rc;   // first: the occupancy query counts no CTA above the limit
     int per_sm = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, GEN_THREADS, smem);
     if (per_sm < 1) per_sm = 1;
     const int64_t grid = std::min<int64_t>(nitems, (int64_t)sm_count() * per_sm * 4);
-    kern<<<(unsigned)grid, GEN_THREADS, smem, st>>>(a, Cpad);
-    DPVO_LAUNCH_CHECK("corr_bwd_generic");
-    return DPVO_OK;
+    return launch("corr_bwd_generic", kern, (unsigned)grid, GEN_THREADS, smem, st, a, Cpad);
   };
   switch (a.P) {
     case 1: return go(corr_bwd_generic<T, G, 1>);
@@ -652,15 +649,12 @@ static int launch_generic(const CorrArgs& a, cudaStream_t st) {
   const int64_t nitems = (int64_t)a.B * a.M;
   if (nitems == 0) return DPVO_OK;
   auto go = [&](auto kern) -> int {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return check_cuda(e, "corr_forward: cudaFuncSetAttribute");
+    if (int rc = allow_smem("corr_fwd_generic", kern, smem)) return rc;   // first: the occupancy query counts no CTA above the limit
     int per_sm = 1;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, GEN_THREADS, smem);
     if (per_sm < 1) per_sm = 1;
     const int64_t grid = std::min<int64_t>(nitems, (int64_t)sm_count() * per_sm * 4);
-    kern<<<(unsigned)grid, GEN_THREADS, smem, st>>>(a, Cpad);
-    DPVO_LAUNCH_CHECK("corr_fwd_generic");
-    return DPVO_OK;
+    return launch("corr_fwd_generic", kern, (unsigned)grid, GEN_THREADS, smem, st, a, Cpad);
   };
   switch (a.P) {
     case 1: return go(corr_fwd_generic<T, 1>);
@@ -689,16 +683,8 @@ static int launch_mma(const CorrArgs& a, bool pair_out, cudaStream_t st) {
   const int64_t need = (nitems + MMA_WARPS - 1) / MMA_WARPS;
   // list mode: the length lives on the device; one CTA per SM drains it
   const int64_t grid = std::min<int64_t>(need, (int64_t)sm_count() * (a.list ? 1 : 2));
-  const size_t smem = sizeof(MmaWarpSmem) * MMA_WARPS;
-  {   // per-device function attribute: set on every call
-    cudaError_t e = pair_out ? cudaFuncSetAttribute(corr_fwd_mma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                             : cudaFuncSetAttribute(corr_fwd_mma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return check_cuda(e, "corr_forward: cudaFuncSetAttribute");
-  }
-  if (pair_out) corr_fwd_mma<true><<<(unsigned)grid, MMA_WARPS * 32, smem, st>>>(a);
-  else corr_fwd_mma<false><<<(unsigned)grid, MMA_WARPS * 32, smem, st>>>(a);
-  DPVO_LAUNCH_CHECK("corr_fwd_mma");
-  return DPVO_OK;
+  return launch("corr_fwd_mma", pair_out ? corr_fwd_mma<true> : corr_fwd_mma<false>, (unsigned)grid, MMA_WARPS * 32, sizeof(MmaWarpSmem) * MMA_WARPS,
+                st, a);
 }
 
 // corr_tc.cu

@@ -308,8 +308,7 @@ int corr_bin_edges(const float* coords, const int64_t* jj, int M, int S2, int H1
   CbBinArgs b = cb_layout(workspace, M, S2, H1, W1, div1);
   const int64_t nkeys = (int64_t)S2 * b.nty * b.ntx;
   if (nkeys > cb_key_cap(M) || ((uintptr_t)workspace & 15)) return DPVO_ERR_UNSUPPORTED;
-  if (cudaFuncSetAttribute(corr_fwd_l1_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CB_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(corr_fwd_l1_tiles, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess) {
+  if (cudaFuncSetAttribute(corr_fwd_l1_tiles, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess) {
     cudaGetLastError();
     return DPVO_ERR_UNSUPPORTED;
   }
@@ -318,12 +317,10 @@ int corr_bin_edges(const float* coords, const int64_t* jj, int M, int S2, int H1
   if (!rc) rc = check_cuda(cudaMemsetAsync(b.cnt, 0, nkeys * sizeof(int), st), "corr_bin: memset");
   if (rc) return rc;
   const unsigned eg = (unsigned)((M + 255) / 256);
-  corr_bin_count<<<eg, 256, 0, st>>>(b);
-  DPVO_LAUNCH_CHECK("corr_bin_count");
-  corr_bin_scan<<<1, 1024, 0, st>>>(b, (int)nkeys);
-  DPVO_LAUNCH_CHECK("corr_bin_scan");
-  corr_bin_scatter<<<eg, 256, 0, st>>>(b);
-  DPVO_LAUNCH_CHECK("corr_bin_scatter");
+  rc = launch("corr_bin_count", corr_bin_count, eg, 256, 0, st, b);
+  if (!rc) rc = launch("corr_bin_scan", corr_bin_scan, 1, 1024, 0, st, b, (int)nkeys);
+  if (!rc) rc = launch("corr_bin_scatter", corr_bin_scatter, eg, 256, 0, st, b);
+  if (rc) return rc;
   *list = b.list; *count = b.hdr; *order = b.order; *ordered = b.hdr + 1;
   return DPVO_OK;
 }
@@ -339,9 +336,7 @@ int corr_bin_level1(const void* fmap1, const void* l1, const int64_t* s21, int H
   a.coords = coords; a.ii = ii; a.out = reinterpret_cast<__half*>(out); a.out_row = out_row; a.div1 = div1;
   a.H1 = H1; a.W1 = W1; a.nty = b.nty; a.ntx = b.ntx; a.order = b.order; a.items = b.items; a.item_count = b.hdr + 2;
   const unsigned grid = (unsigned)((int64_t)S2 * b.nty * b.ntx + (M + CB_ITEM - 1) / CB_ITEM);     // bound on the items
-  corr_fwd_l1_tiles<<<grid, CB_WARPS * 32, CB_SMEM, st>>>(a);
-  DPVO_LAUNCH_CHECK("corr_fwd_l1_tiles");
-  return DPVO_OK;
+  return launch("corr_fwd_l1_tiles", corr_fwd_l1_tiles, grid, CB_WARPS * 32, CB_SMEM, st, a);
 }
 
 }  // namespace dpvo

@@ -320,8 +320,7 @@ int corr_tc_forward(const void* fmap1, const int64_t* s1, int S1, const void* l0
   // per-device function attribute: set on every call
   // the whole carveout as shared memory: a level-1 CTA can then join each SM while this kernel runs (an SM changes
   // its carveout only when idle)
-  if (cudaFuncSetAttribute(corr_fwd_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-      cudaFuncSetAttribute(corr_fwd_tc, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess) {
+  if (cudaFuncSetAttribute(corr_fwd_tc, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess) {
     cudaGetLastError();
     return DPVO_ERR_UNSUPPORTED;
   }
@@ -335,8 +334,8 @@ int corr_tc_forward(const void* fmap1, const int64_t* s1, int S1, const void* l0
   TcArgs a;
   a.coords = coords; a.ii = ii; a.jj = jj; a.out = (__half*)out; a.out_row = out_row; a.order = order; a.count = ordered;
   const unsigned grid = (unsigned)std::min<int64_t>(M, sm_count());
-  corr_fwd_tc<<<grid, TC_THREADS, smem, st>>>(cache.maps, a);
-  DPVO_LAUNCH_CHECK("corr_fwd_tc");
+  rc = launch("corr_fwd_tc", corr_fwd_tc, grid, TC_THREADS, smem, st, cache.maps, a);
+  if (rc) return rc;
   // level 1 on the side stream, launched after level 0 so that the persistent level-0 CTAs are placed first
   rc = check_cuda(cudaStreamWaitEvent(side->s, side->fork, 0), "corr_tc: fork");
   if (!rc) rc = corr_bin_level1(fmap1, l1, s21, H1, W1, S2, div1, coords, ii, out, out_row, M, workspace, side->s);

@@ -533,17 +533,8 @@ static inline int64_t ntiles(int ho, int wo) { return (int64_t)((ho + EC_TH - 1)
 template <int KS, int S, int CIN, int NT, bool STEM>
 static int launch_conv(const EncConvParams& p, int nimg, int cout, const char* name, cudaStream_t st) {
   using C = EncCfg<KS, S, CIN, NT, STEM>;
-  auto kern = enc_conv_kernel<KS, S, CIN, NT, STEM>;
-  static bool attr = false;                                              // per instantiation
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
-    if (e != cudaSuccess) return check_cuda(e, name);
-    attr = true;
-  }
   dim3 grid((unsigned)ntiles(p.Hout, p.Wout), (unsigned)(cout / NT), (unsigned)(nimg * p.nenc));
-  kern<<<grid, EC_THREADS, C::SMEM, st>>>(p, cout);
-  DPVO_LAUNCH_CHECK(name);
-  return DPVO_OK;
+  return launch(name, enc_conv_kernel<KS, S, CIN, NT, STEM>, grid, EC_THREADS, C::SMEM, st, p, cout);
 }
 
 // one launch of layer `shape` over nimg images x p.nenc encoders
@@ -807,9 +798,7 @@ static int encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_
   for (int b = 0; b < B; ++b) {
     c.frame_row[b] = (int)frame_row[b]; c.feat_row[b] = (int)feat_row[b]; c.patch_row[b] = (int)patch_row[b];
   }
-  enc_centroid_kernel<<<dim3(M, B), 128, 0, st>>>(c);
-  DPVO_LAUNCH_CHECK("enc_centroid_kernel");
-  return DPVO_OK;
+  return launch("enc_centroid_kernel", enc_centroid_kernel, dim3(M, B), 128, 0, st, c);
 }
 
 extern "C" int dpvo_encode_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,

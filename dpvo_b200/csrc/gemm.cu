@@ -251,13 +251,7 @@ template <bool GATHER, bool WS, int EPI, int OUT>
 static int launch_out(const GemmMaps& m, const GemmArgs& a, unsigned grid, cudaStream_t st) {
   const size_t smem = (WS ? (size_t)GM_WS_ASTAGES * GM_A_BYTES + (size_t)GM_WS_MAXKB * GM_B_BYTES
                           : (size_t)GM_STAGES * (GM_A_BYTES + GM_B_BYTES)) + sizeof(GemmBars) + 1024;
-  // the opt-in is a per-device function attribute: set it on every launch (a cached flag would be wrong on the
-  // second GPU of a process and is not worth a lock)
-  cudaError_t e = cudaFuncSetAttribute(linear_f16_kernel<GATHER, WS, EPI, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return check_cuda(e, "linear_f16: cudaFuncSetAttribute");
-  linear_f16_kernel<GATHER, WS, EPI, OUT><<<grid, GM_THREADS, smem, st>>>(m.A, m.B, a);
-  DPVO_LAUNCH_CHECK("linear_f16_kernel");
-  return DPVO_OK;
+  return launch("linear_f16_kernel", linear_f16_kernel<GATHER, WS, EPI, OUT>, grid, GM_THREADS, smem, st, m.A, m.B, a);
 }
 
 template <bool GATHER, bool WS, int EPI>

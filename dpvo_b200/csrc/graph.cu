@@ -370,11 +370,7 @@ static int group_launch_n(const GroupProblem* p0, const GroupProblem* p1, cudaSt
   // both y-slices use the same x extent; the tile loops stride by gridDim.x, so any extent >= 1 is correct
   const int want = both ? std::max(a0.ntiles, a1.ntiles) : a0.ntiles;
   const int grid = std::max(1, std::min(want, max_blocks / (both ? 2 : 1)));
-  void* kargs[] = {(void*)&a0, (void*)&a1};
-  cudaError_t e = cudaLaunchCooperativeKernel((const void*)group_edges_kernel, dim3(grid, both ? 2 : 1), dim3(G_THREADS), kargs, 0, st);
-  if (e != cudaSuccess) return check_cuda(e, "group_edges_kernel");
-  DPVO_LAUNCH_CHECK("group_edges_kernel");
-  return DPVO_OK;
+  return launch<cudaLaunchAttributeCooperative>("group_edges_kernel", group_edges_kernel, dim3(grid, both ? 2 : 1), G_THREADS, 0, st, a0, a1);
 }
 
 }  // namespace dpvo
@@ -443,9 +439,7 @@ extern "C" int dpvo_neighbors(const int64_t* ii, const int64_t* jj, int64_t E,
   if (rc) return rc;
   const int threads = 256;
   const unsigned blocks = (unsigned)std::min<int64_t>((E + threads - 1) / threads, (int64_t)sm_count() * 8);
-  neighbors_kernel<<<blocks, threads, 0, st>>>(p.order, p.group_of, E, ix, jx);
-  DPVO_LAUNCH_CHECK("neighbors_kernel");
-  return DPVO_OK;
+  return launch("neighbors_kernel", neighbors_kernel, blocks, threads, 0, st, p.order, p.group_of, E, ix, jx);
 }
 
 extern "C" int dpvo_neighbors_from_groups(const int32_t* order, const int32_t* group_of, int64_t E,
@@ -455,7 +449,5 @@ extern "C" int dpvo_neighbors_from_groups(const int32_t* order, const int32_t* g
   DPVO_REQUIRE(order && group_of && ix && jx, "neighbors_from_groups: null pointer");
   const int threads = 256;
   const unsigned blocks = (unsigned)std::min<int64_t>((E + threads - 1) / threads, (int64_t)sm_count() * 8);
-  neighbors_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(order, group_of, E, ix, jx);
-  DPVO_LAUNCH_CHECK("neighbors_kernel");
-  return DPVO_OK;
+  return launch("neighbors_kernel", neighbors_kernel, blocks, threads, 0, (cudaStream_t)stream, order, group_of, E, ix, jx);
 }

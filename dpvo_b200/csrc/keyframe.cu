@@ -232,13 +232,11 @@ extern "C" int dpvo_keyframe_motion(const float* poses, const float* patches, co
                (long long)workspace_bytes, (long long)dpvo_keyframe_motion_workspace_bytes(B));
   cudaStream_t st = (cudaStream_t)stream;
   double* partial = (double*)workspace;
-  keyframe_motion_partial_kernel<<<dim3(KF_PARTS, B), KF_THREADS, 0, st>>>(poses, patches, intrinsics, F, ii, jj, kk, active, slots,
-                                                                          n, ki, partial);
-  DPVO_LAUNCH_CHECK("keyframe_motion_partial_kernel");
-  keyframe_motion_kernel<<<(B + 63) / 64, 64, 0, st>>>(poses, F, B, partial, n, tstamp, delta, delta_src, T, ki, thresh, flag, k, m,
-                                                       overflow);
-  DPVO_LAUNCH_CHECK("keyframe_motion_kernel");
-  return DPVO_OK;
+  const int rc = launch("keyframe_motion_partial_kernel", keyframe_motion_partial_kernel, dim3(KF_PARTS, B), KF_THREADS, 0, st, poses, patches,
+                        intrinsics, F, ii, jj, kk, active, slots, n, ki, partial);
+  if (rc) return rc;
+  return launch("keyframe_motion_kernel", keyframe_motion_kernel, (B + 63) / 64, 64, 0, st, poses, F, B, partial, n, tstamp, delta, delta_src, T,
+                ki, thresh, flag, k, m, overflow);
 }
 
 // any_bytes: rows of any positive byte count at any alignment, copied 1 byte at a time where 4 does not divide them
@@ -272,8 +270,9 @@ static int keyframe_shift(void* const* bases, const int64_t* row_bytes, const in
   bufs.nbuf = nbuf;
   const int64_t want = std::max<int64_t>(1, std::min<int64_t>((most + 255) / 256, ((int64_t)sm_count() * 4 + B - 1) / B));
   for (int s = 0; s < ki - 1; ++s) {
-    keyframe_shift_kernel<<<dim3((unsigned)want, (unsigned)B), 256, 0, (cudaStream_t)stream>>>(bufs, F, s, flag, k);
-    DPVO_LAUNCH_CHECK("keyframe_shift_kernel");
+    const int rc = launch("keyframe_shift_kernel", keyframe_shift_kernel, dim3((unsigned)want, (unsigned)B), 256, 0, (cudaStream_t)stream, bufs, F,
+                          s, flag, k);
+    if (rc) return rc;
   }
   return DPVO_OK;
 }
@@ -295,9 +294,8 @@ extern "C" int dpvo_keyframe_count(int mode, const int64_t* n, int64_t* tstamp, 
                (long long)T);
   DPVO_REQUIRE(counter && overflow && (mode == 1 || (n && tstamp)) && (mode == 0 || (delta && delta_src)),
                "keyframe_count: null pointer");
-  keyframe_count_kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(mode, n, tstamp, F, B, counter, delta, delta_src, T, overflow);
-  DPVO_LAUNCH_CHECK("keyframe_count_kernel");
-  return DPVO_OK;
+  return launch("keyframe_count_kernel", keyframe_count_kernel, (B + 63) / 64, 64, 0, (cudaStream_t)stream, mode, n, tstamp, F, B, counter, delta,
+                delta_src, T, overflow);
 }
 
 extern "C" int dpvo_keyframe_trajectory(const float* poses, const int64_t* tstamp, const int64_t* n, int64_t F, int B,
@@ -307,7 +305,6 @@ extern "C" int dpvo_keyframe_trajectory(const float* poses, const int64_t* tstam
                (long long)T);
   DPVO_REQUIRE(T <= INT32_MAX, "keyframe_trajectory: %lld timestamps exceed the int32 map", (long long)T);
   DPVO_REQUIRE(poses && tstamp && n && delta && delta_src && counter && map && out && error, "keyframe_trajectory: null pointer");
-  keyframe_trajectory_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(poses, tstamp, n, F, delta, delta_src, T, counter, map, out, error);
-  DPVO_LAUNCH_CHECK("keyframe_trajectory_kernel");
-  return DPVO_OK;
+  return launch("keyframe_trajectory_kernel", keyframe_trajectory_kernel, B, 256, 0, (cudaStream_t)stream, poses, tstamp, n, F, delta, delta_src,
+                T, counter, map, out, error);
 }

@@ -48,26 +48,18 @@ static int lie_launch(int group, int dtype, const LieArgs& A, cudaStream_t st, c
     set_error("%s: dtype %d not supported (f32/f64)", name, dtype);
     return DPVO_ERR_UNSUPPORTED;
   }
-  const int threads = 256;
-  const unsigned blocks = (unsigned)std::min<int64_t>((A.n + threads - 1) / threads, (int64_t)sm_count() * 8);
+  const bool f32 = dtype == DPVO_F32;
   if (group == DPVO_RXSO3 || group == DPVO_SIM3) {
     const unsigned sb = (unsigned)std::min<int64_t>((A.n + 127) / 128, (int64_t)sm_count() * 8);
-    if (group == DPVO_SIM3) {
-      if (dtype == DPVO_F32) lie_scaled_kernel<DPVO_SIM3, float, OP><<<sb, 128, 0, st>>>(A);
-      else lie_scaled_kernel<DPVO_SIM3, double, OP><<<sb, 128, 0, st>>>(A);
-    } else {
-      if (dtype == DPVO_F32) lie_scaled_kernel<DPVO_RXSO3, float, OP><<<sb, 128, 0, st>>>(A);
-      else lie_scaled_kernel<DPVO_RXSO3, double, OP><<<sb, 128, 0, st>>>(A);
-    }
-  } else if (group == DPVO_SE3) {
-    if (dtype == DPVO_F32) lie_kernel<DPVO_SE3, float, OP><<<blocks, threads, 0, st>>>(A);
-    else lie_kernel<DPVO_SE3, double, OP><<<blocks, threads, 0, st>>>(A);
-  } else {
-    if (dtype == DPVO_F32) lie_kernel<DPVO_SO3, float, OP><<<blocks, threads, 0, st>>>(A);
-    else lie_kernel<DPVO_SO3, double, OP><<<blocks, threads, 0, st>>>(A);
+    const auto kern = group == DPVO_SIM3 ? (f32 ? lie_scaled_kernel<DPVO_SIM3, float, OP> : lie_scaled_kernel<DPVO_SIM3, double, OP>)
+                                         : (f32 ? lie_scaled_kernel<DPVO_RXSO3, float, OP> : lie_scaled_kernel<DPVO_RXSO3, double, OP>);
+    return launch(name, kern, sb, 128, 0, st, A);
   }
-  DPVO_LAUNCH_CHECK(name);
-  return DPVO_OK;
+  const int threads = 256;
+  const unsigned blocks = (unsigned)std::min<int64_t>((A.n + threads - 1) / threads, (int64_t)sm_count() * 8);
+  const auto kern = group == DPVO_SE3 ? (f32 ? lie_kernel<DPVO_SE3, float, OP> : lie_kernel<DPVO_SE3, double, OP>)
+                                      : (f32 ? lie_kernel<DPVO_SO3, float, OP> : lie_kernel<DPVO_SO3, double, OP>);
+  return launch(name, kern, blocks, threads, 0, st, A);
 }
 
 }  // namespace dpvo

@@ -330,10 +330,8 @@ extern "C" int dpvo_loop_scores(const float* poses, const float* patches, const 
   DPVO_REQUIRE(poses && patches && intrinsics && n_dev && last_ba && scores, "loop_scores: null pointer");
   const int J = freq - kf_index;
   const int64_t threads = (int64_t)J * max_age * 32;
-  loop_scores_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      poses, patches, intrinsics, n_dev, last_ba, M, removal, max_age, freq, J, scores);
-  DPVO_LAUNCH_CHECK("loop_scores_kernel");
-  return DPVO_OK;
+  return launch("loop_scores_kernel", loop_scores_kernel, (unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream,
+                poses, patches, intrinsics, n_dev, last_ba, M, removal, max_age, freq, J, scores);
 }
 
 extern "C" int dpvo_loop_select(const float* scores, const int64_t* n_dev, int64_t* last_ba, int M, int removal, int max_age,
@@ -352,19 +350,12 @@ extern "C" int dpvo_loop_select(const float* scores, const int64_t* n_dev, int64
   while (p2 < S) p2 <<= 1;
   const size_t smem = (size_t)p2 * 8 + (size_t)S;
   cudaStream_t st = (cudaStream_t)stream;
-  // the attribute belongs to the current device: set it on every call (cheap, and right on any device or thread)
-  const int e = check_cuda(cudaFuncSetAttribute(loop_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                (int)((size_t)LOOP_MAX_KEYS * 8 + LOOP_MAX_KEYS)), "loop_select: smem attribute");
+  const int e = launch("loop_select_kernel", loop_select_kernel, 1, LOOP_THREADS, smem, st, scores, n_dev, last_ba, removal, max_age, freq, J, p2,
+                       thresh, max_pairs, pairs, n_pairs);
   if (e != DPVO_OK) return e;
-  loop_select_kernel<<<1, LOOP_THREADS, smem, st>>>(scores, n_dev, last_ba, removal, max_age, freq, J, p2, thresh, max_pairs,
-                                                    pairs, n_pairs);
-  DPVO_LAUNCH_CHECK("loop_select_kernel");
   const int64_t work = (int64_t)max_pairs * M * 96;
   const unsigned grid = (unsigned)std::min<int64_t>((work + 255) / 256, (int64_t)sm_count() * 8);
-  loop_emit_kernel<<<grid, 256, 0, st>>>(pairs, n_pairs, M, ii, jj, kk, active, region, state,
-                                         n_active, overflow);
-  DPVO_LAUNCH_CHECK("loop_emit_kernel");
-  return DPVO_OK;
+  return launch("loop_emit_kernel", loop_emit_kernel, grid, 256, 0, st, pairs, n_pairs, M, ii, jj, kk, active, region, state, n_active, overflow);
 }
 
 extern "C" int dpvo_pgraph_remove_store(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* active, const float* target,
@@ -379,12 +370,9 @@ extern "C" int dpvo_pgraph_remove_store(int64_t* ii, int64_t* jj, int64_t* kk, u
   if (cap == 0) return DPVO_OK;
   DPVO_REQUIRE(ii && jj && kk && active && target && weight && n_dev && n_active && s_count, "pgraph_remove_store: null pointer");
   DPVO_REQUIRE(s_cap == 0 || (s_ii && s_jj && s_kk && s_target && s_weight), "pgraph_remove_store: null store pointer");
-  pgraph_remove_store_kernel<<<1, LOOP_THREADS, 0, (cudaStream_t)stream>>>(ii, jj, kk, active, target, weight, cap, n_dev, removal,
-                                                                           opt_window, enable, dummy_frame, dummy_patch, M, n_active,
-                                                                           s_ii, s_jj, s_kk, s_target, s_weight, s_cap, s_count,
-                                                                           s_overflow);
-  DPVO_LAUNCH_CHECK("pgraph_remove_store_kernel");
-  return DPVO_OK;
+  return launch("pgraph_remove_store_kernel", pgraph_remove_store_kernel, 1, LOOP_THREADS, 0, (cudaStream_t)stream, ii, jj, kk, active, target,
+                weight, cap, n_dev, removal, opt_window, enable, dummy_frame, dummy_patch, M, n_active, s_ii, s_jj, s_kk, s_target, s_weight,
+                s_cap, s_count, s_overflow);
 }
 
 extern "C" int dpvo_loop_flags(const int64_t* ii, const uint8_t* active, int64_t cap, int64_t normal, int64_t n, int removal,
@@ -392,9 +380,8 @@ extern "C" int dpvo_loop_flags(const int64_t* ii, const uint8_t* active, int64_t
   DPVO_REQUIRE(cap >= 0 && normal >= 0 && normal <= cap, "loop_flags: bad sizes (cap=%lld, normal=%lld)", (long long)cap,
                (long long)normal);
   DPVO_REQUIRE(flags && (cap == 0 || (ii && active)), "loop_flags: null pointer");
-  loop_flags_kernel<<<1, LOOP_THREADS, 0, (cudaStream_t)stream>>>(ii, active, cap, normal, n, removal, s_count, flags);
-  DPVO_LAUNCH_CHECK("loop_flags_kernel");
-  return DPVO_OK;
+  return launch("loop_flags_kernel", loop_flags_kernel, 1, LOOP_THREADS, 0, (cudaStream_t)stream, ii, active, cap, normal, n, removal, s_count,
+                flags);
 }
 
 extern "C" int dpvo_loop_normalize_deltas(float* poses, float* patches, int64_t n, int M, int P, float* delta, int64_t n_delta,
@@ -403,9 +390,7 @@ extern "C" int dpvo_loop_normalize_deltas(float* poses, float* patches, int64_t 
                P, (long long)n_delta);
   if (n == 0) return DPVO_OK;
   DPVO_REQUIRE(poses && patches && (delta || n_delta == 0), "loop_normalize: null pointer");
-  loop_normalize_kernel<<<1, LOOP_THREADS, 0, (cudaStream_t)stream>>>(poses, patches, n, M, P, delta, n_delta);
-  DPVO_LAUNCH_CHECK("loop_normalize_kernel");
-  return DPVO_OK;
+  return launch("loop_normalize_kernel", loop_normalize_kernel, 1, LOOP_THREADS, 0, (cudaStream_t)stream, poses, patches, n, M, P, delta, n_delta);
 }
 
 extern "C" int dpvo_loop_normalize(float* poses, float* patches, int64_t n, int M, int P, void* stream) {

@@ -72,7 +72,6 @@ extern "C" int dpvo_point_cloud(const float* poses, const float* patches, const 
     most = std::max(most, n[b] * M);
   }
   if (most == 0) return DPVO_OK;
-  point_cloud_kernel<<<dim3((unsigned)((most + MAP_THREADS - 1) / MAP_THREADS), (unsigned)B), MAP_THREADS, 0, (cudaStream_t)stream>>>(p);
-  DPVO_LAUNCH_CHECK("point_cloud_kernel");
-  return DPVO_OK;
+  return launch("point_cloud_kernel", point_cloud_kernel, dim3((unsigned)((most + MAP_THREADS - 1) / MAP_THREADS), (unsigned)B), MAP_THREADS, 0,
+                (cudaStream_t)stream, p);
 }

@@ -61,10 +61,8 @@ static int patchify_fwd_launch(const void* net, const int64_t* s, const float* c
   if (total == 0) return DPVO_OK;
   const int threads = 256;
   const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, (int64_t)sm_count() * 16);
-  patchify_fwd_kernel<T><<<(unsigned)blocks, threads, 0, st>>>(
-      reinterpret_cast<const T*>(net), s[0], s[1], s[2], s[3], coords, reinterpret_cast<T*>(patches), M, C, H, W, R, total);
-  DPVO_LAUNCH_CHECK("patchify_fwd_kernel");
-  return DPVO_OK;
+  return launch("patchify_fwd_kernel", patchify_fwd_kernel<T>, (unsigned)blocks, threads, 0, st,
+                reinterpret_cast<const T*>(net), s[0], s[1], s[2], s[3], coords, reinterpret_cast<T*>(patches), M, C, H, W, R, total);
 }
 
 template <typename T>
@@ -75,10 +73,8 @@ static int patchify_bwd_launch(const void* grad, const float* coords, void* net_
   if (total == 0) return DPVO_OK;
   const int threads = 256;
   const int64_t blocks = std::min<int64_t>((total + threads - 1) / threads, (int64_t)sm_count() * 16);
-  patchify_bwd_kernel<T><<<(unsigned)blocks, threads, 0, st>>>(
-      reinterpret_cast<const T*>(grad), coords, reinterpret_cast<T*>(net_grad), M, C, H, W, R, total);
-  DPVO_LAUNCH_CHECK("patchify_bwd_kernel");
-  return DPVO_OK;
+  return launch("patchify_bwd_kernel", patchify_bwd_kernel<T>, (unsigned)blocks, threads, 0, st,
+                reinterpret_cast<const T*>(grad), coords, reinterpret_cast<T*>(net_grad), M, C, H, W, R, total);
 }
 
 }  // namespace dpvo

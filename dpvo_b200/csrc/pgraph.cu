@@ -129,9 +129,8 @@ extern "C" int dpvo_pgraph_remove(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t
   if (cap == 0) return DPVO_OK;
   DPVO_REQUIRE(ii && jj && kk && active && frame && n_active, "pgraph_remove: null pointer");
   const unsigned grid = (unsigned)std::min<int64_t>((cap + 255) / 256, (int64_t)sm_count() * 4);
-  pgraph_remove_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(ii, jj, kk, active, cap, rule, frame, param, enable, dummy_frame, dummy_patch, M, n_active);
-  DPVO_LAUNCH_CHECK("pgraph_remove_kernel");
-  return DPVO_OK;
+  return launch("pgraph_remove_kernel", pgraph_remove_kernel, grid, 256, 0, (cudaStream_t)stream, ii, jj, kk, active, cap, rule, frame, param,
+                enable, dummy_frame, dummy_patch, M, n_active);
 }
 
 extern "C" int dpvo_pgraph_append(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t* active, int64_t cap, const int64_t* new_ii,
@@ -142,21 +141,16 @@ extern "C" int dpvo_pgraph_append(int64_t* ii, int64_t* jj, int64_t* kk, uint8_t
   DPVO_REQUIRE(ii && jj && kk && active && new_ii && new_jj && new_kk && n_active, "pgraph_append: null pointer");
   DPVO_REQUIRE(!state || slot_of_new, "pgraph_append: zeroing the state rows needs the slot_of_new scratch");
   cudaStream_t st = (cudaStream_t)stream;
-  pgraph_append_kernel<<<1, PG_THREADS, 0, st>>>(ii, jj, kk, active, cap, new_ii, new_jj, new_kk, n_new, enable, slot_of_new, n_active, overflow);
-  DPVO_LAUNCH_CHECK("pgraph_append_kernel");
-  if (state) {
-    const unsigned grid = (unsigned)std::min<int64_t>((n_new * 96 + 255) / 256, (int64_t)sm_count() * 8);
-    pgraph_zero_rows_kernel<<<grid, 256, 0, st>>>(state, slot_of_new, n_new);
-    DPVO_LAUNCH_CHECK("pgraph_zero_rows_kernel");
-  }
-  return DPVO_OK;
+  int rc = launch("pgraph_append_kernel", pgraph_append_kernel, 1, PG_THREADS, 0, st, ii, jj, kk, active, cap, new_ii, new_jj, new_kk, n_new,
+                  enable, slot_of_new, n_active, overflow);
+  if (rc || !state) return rc;
+  const unsigned grid = (unsigned)std::min<int64_t>((n_new * 96 + 255) / 256, (int64_t)sm_count() * 8);
+  return launch("pgraph_zero_rows_kernel", pgraph_zero_rows_kernel, grid, 256, 0, st, state, slot_of_new, n_new);
 }
 
 extern "C" int dpvo_pgraph_new_edges(const int64_t* n_dev, int M, int r, int64_t* ii, int64_t* jj, int64_t* kk, void* stream) {
   DPVO_REQUIRE(M > 0 && r > 1 && n_dev && ii && jj && kk, "pgraph_new_edges: bad arguments");
   const int64_t total = (int64_t)M * (2 * r - 1);
   const unsigned grid = (unsigned)((total + 255) / 256);
-  pgraph_new_edges_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(n_dev, M, r, ii, jj, kk);
-  DPVO_LAUNCH_CHECK("pgraph_new_edges_kernel");
-  return DPVO_OK;
+  return launch("pgraph_new_edges_kernel", pgraph_new_edges_kernel, grid, 256, 0, (cudaStream_t)stream, n_dev, M, r, ii, jj, kk);
 }

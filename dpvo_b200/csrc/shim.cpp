@@ -1300,7 +1300,7 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("update_gru_heads", &update_gru_heads, "fused group add + GRU + heads (net.py:88-92)", py::arg("net32"), py::arg("hij16"), py::arg("group_of"),
         py::arg("W6"), py::arg("params"), py::arg("coords") = py::none(), py::arg("workspace") = py::none(), py::arg("hkk16") = py::none(), py::arg("group_kk") = py::none(),
         py::arg("delta_out") = py::none(), py::arg("weight_out") = py::none());
-  m.def("update_gru_workspace_bytes", &update_gru_workspace_bytes, "scratch bytes of update_gru_heads");
+  m.def("update_gru_workspace_bytes", &update_gru_workspace_bytes, "scratch bytes of update_gru_heads (current device)");
   m.def("pgraph_remove", &pgraph_remove, "park edges by rule on the fixed-capacity edge store", py::arg("ii"), py::arg("jj"), py::arg("kk"), py::arg("active"),
         py::arg("rule"), py::arg("frame"), py::arg("param"), py::arg("enable"), py::arg("dummy_frame"), py::arg("dummy_patch"), py::arg("M"), py::arg("n_active"));
   m.def("pgraph_append", &pgraph_append, "fill parked slots with new edges", py::arg("ii"), py::arg("jj"), py::arg("kk"), py::arg("active"), py::arg("new_ii"),

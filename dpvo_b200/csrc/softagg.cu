@@ -292,14 +292,11 @@ extern "C" int dpvo_softagg_fused(const void* x16, int64_t ldx, const int32_t* o
     // a CTA keeps its channel slice: the grid is a multiple of the slice count
     const int64_t tiles = (E + SF_M - 1) / SF_M;
     const int64_t grid = std::max<int64_t>(SF_SLICES, std::min<int64_t>(tiles, sm_count() / SF_SLICES) * SF_SLICES);
-    cudaError_t e = cudaFuncSetAttribute(softagg_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SF_SMEM);
-    if (e != cudaSuccess) return check_cuda(e, "softagg_fused: cudaFuncSetAttribute");
-    softagg_fused_kernel<<<(unsigned)grid, SF_THREADS, SF_SMEM, st>>>((const __half*)x16, ldx, order, group_of, (const __half*)w16, bias, (__half*)y16, (float*)workspace,
-                                                                     (int)E, (int)max_groups);
-    DPVO_LAUNCH_CHECK("softagg_fused_kernel");
+    const int rc = launch("softagg_fused_kernel", softagg_fused_kernel, (unsigned)grid, SF_THREADS, SF_SMEM, st, (const __half*)x16, ldx, order,
+                          group_of, (const __half*)w16, bias, (__half*)y16, (float*)workspace, (int)E, (int)max_groups);
+    if (rc) return rc;
   }
   const unsigned grid = (unsigned)std::min<int64_t>(max_groups, (int64_t)sm_count() * 8);
-  softagg_combine_kernel<<<grid, SF_DIM / 2, 0, st>>>(group_start, n_groups, (const float*)workspace, (__half*)y16, (int)max_groups);
-  DPVO_LAUNCH_CHECK("softagg_combine_kernel");
-  return DPVO_OK;
+  return launch("softagg_combine_kernel", softagg_combine_kernel, grid, SF_DIM / 2, 0, st, group_start, n_groups, (const float*)workspace,
+                (__half*)y16, (int)max_groups);
 }

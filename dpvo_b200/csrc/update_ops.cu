@@ -299,18 +299,11 @@ static int launch_ln_bulk(const void* a, const void* b, const void* c, int db, c
   constexpr int ES = (DA == DPVO_F32) ? 4 : 2;
   const size_t smem = (size_t)LNB_STAGES * LNB_ROWS * LNB_DIM * (ES + (HAS_C ? 2 : 0) + (b ? 2 : 0) + (cs ? 2 : 0)) + LNB_STAGES * sizeof(uint64_t) + 128;
   if (smem > LNB_SMEM_CAP) return DPVO_ERR_UNSUPPORTED;          // all four operands at once: the register kernel takes it
-  {                                                      // the largest layout (all four operands) of this instantiation; per device, every call
-    const size_t smem_max = std::min<size_t>(LNB_SMEM_CAP, (size_t)LNB_STAGES * LNB_ROWS * LNB_DIM * (ES + (HAS_C ? 2 : 0) + 4) + LNB_STAGES * sizeof(uint64_t) + 128);
-    cudaError_t e = cudaFuncSetAttribute(add_layernorm_bulk_kernel<DA, HAS_C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
-    if (e != cudaSuccess) return check_cuda(e, "add_layernorm: cudaFuncSetAttribute");
-  }
   const int64_t n_tiles = (rows + LNB_ROWS - 1) / LNB_ROWS;
   const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(200 * 1024) / smem));
   const unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(n_tiles, (int64_t)sm_count() * per_sm));
-  add_layernorm_bulk_kernel<DA, HAS_C><<<grid, ROW_WARPS * 32 + 32, smem, st>>>(a, b, (const __half*)c, db, bi, (const __half*)cs, ld_cs, gamma, beta, eps,
-                                                                           (float*)y32, (__half*)y16, relu, rows);
-  DPVO_LAUNCH_CHECK("add_layernorm_bulk_kernel");
-  return DPVO_OK;
+  return launch("add_layernorm_bulk_kernel", add_layernorm_bulk_kernel<DA, HAS_C>, grid, ROW_WARPS * 32 + 32, smem, st, a, b, (const __half*)c, db,
+                bi, (const __half*)cs, ld_cs, gamma, beta, eps, (float*)y32, (__half*)y16, relu, rows);
 }
 
 // ---- gather / residual / scatter / gate -------------------------------------------------------
@@ -553,8 +546,8 @@ extern "C" int dpvo_add_layernorm(const void* a, const void* b, const void* c, c
   const int64_t* bi = b ? b_index : nullptr;
   cudaStream_t st = (cudaStream_t)stream;
 #define DPVO_LN_LAUNCH_T(NV, RPW, DA, DBC)                                                                                   \
-  add_layernorm_kernel<NV, RPW, DA, DBC><<<row_grid((rows + RPW - 1) / RPW), ROW_WARPS * 32, 0, st>>>(                     \
-      a, b, c, in_dtypes[0], db, dc, bi, (const __half*)c_scale, ld_c_scale, gamma, beta, eps, (float*)y32, (__half*)y16, relu, rows, dim)
+  return launch("add_layernorm_kernel", add_layernorm_kernel<NV, RPW, DA, DBC>, row_grid((rows + RPW - 1) / RPW), ROW_WARPS * 32, 0, st, a, b, c, \
+                in_dtypes[0], db, dc, bi, (const __half*)c_scale, ld_c_scale, gamma, beta, eps, (float*)y32, (__half*)y16, relu, rows, dim)
 #define DPVO_LN_LAUNCH(NV, RPW) DPVO_LN_LAUNCH_T(NV, RPW, -1, -1)
   // the update operator's shapes (dim 384): fp16 alone, fp32 alone, fp32 + fp16 (+ fp16)
   const bool bc16 = (!b || db == DPVO_F16) && (!c || dc == DPVO_F16);
@@ -573,24 +566,20 @@ extern "C" int dpvo_add_layernorm(const void* a, const void* b, const void* c, c
   }
   if (nv == 3 && bc16) {
     if (in_dtypes[0] == DPVO_F16) DPVO_LN_LAUNCH_T(3, 2, DPVO_F16, DPVO_F16);
-    else DPVO_LN_LAUNCH_T(3, 2, DPVO_F32, DPVO_F16);
-    DPVO_LAUNCH_CHECK("add_layernorm_kernel");
-    return DPVO_OK;
+    DPVO_LN_LAUNCH_T(3, 2, DPVO_F32, DPVO_F16);
   }
   switch (nv) {
-    case 1: DPVO_LN_LAUNCH(1, 4); break;
-    case 2: DPVO_LN_LAUNCH(2, 2); break;
-    case 3: DPVO_LN_LAUNCH(3, 2); break;
-    case 4: DPVO_LN_LAUNCH(4, 2); break;
-    case 5: DPVO_LN_LAUNCH(5, 1); break;
-    case 6: DPVO_LN_LAUNCH(6, 1); break;
-    case 7: DPVO_LN_LAUNCH(7, 1); break;
-    default: DPVO_LN_LAUNCH(8, 1); break;
+    case 1: DPVO_LN_LAUNCH(1, 4);
+    case 2: DPVO_LN_LAUNCH(2, 2);
+    case 3: DPVO_LN_LAUNCH(3, 2);
+    case 4: DPVO_LN_LAUNCH(4, 2);
+    case 5: DPVO_LN_LAUNCH(5, 1);
+    case 6: DPVO_LN_LAUNCH(6, 1);
+    case 7: DPVO_LN_LAUNCH(7, 1);
+    default: DPVO_LN_LAUNCH(8, 1);
   }
 #undef DPVO_LN_LAUNCH
 #undef DPVO_LN_LAUNCH_T
-  DPVO_LAUNCH_CHECK("add_layernorm_kernel");
-  return DPVO_OK;
 }
 
 extern "C" int dpvo_gather_rows_masked(const void* x, int x_dtype, const int64_t* idx,
@@ -598,9 +587,8 @@ extern "C" int dpvo_gather_rows_masked(const void* x, int x_dtype, const int64_t
   DPVO_REQUIRE(rows >= 0 && dim > 0 && dim % 4 == 0, "gather_rows_masked: bad sizes");
   if (rows == 0) return DPVO_OK;
   DPVO_REQUIRE(x && idx && y && ok_dt(x_dtype) && ok_dt(y_dtype), "gather_rows_masked: bad argument");
-  gather_rows_masked_kernel<<<row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream>>>(x, x_dtype, idx, y, y_dtype, rows, dim);
-  DPVO_LAUNCH_CHECK("gather_rows_masked_kernel");
-  return DPVO_OK;
+  return launch("gather_rows_masked_kernel", gather_rows_masked_kernel, row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream, x, x_dtype, idx, y,
+                y_dtype, rows, dim);
 }
 
 extern "C" int dpvo_residual_add(void* net32, const void* u, int u_dtype, const int32_t* group_of, void* net16,
@@ -608,9 +596,8 @@ extern "C" int dpvo_residual_add(void* net32, const void* u, int u_dtype, const 
   DPVO_REQUIRE(rows >= 0 && dim > 0 && dim % 4 == 0, "residual_add: bad sizes");
   if (rows == 0) return DPVO_OK;
   DPVO_REQUIRE(net32 && u && ok_dt(u_dtype), "residual_add: bad argument");
-  residual_add_kernel<<<row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream>>>((float*)net32, u, u_dtype, group_of, (__half*)net16, rows, dim, true);
-  DPVO_LAUNCH_CHECK("residual_add_kernel");
-  return DPVO_OK;
+  return launch("residual_add_kernel", residual_add_kernel, row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream, (float*)net32, u, u_dtype,
+                group_of, (__half*)net16, rows, dim, true);
 }
 
 extern "C" int dpvo_residual_sum16(const void* net32, const void* u, int u_dtype, const int32_t* group_of, void* net16,
@@ -618,9 +605,8 @@ extern "C" int dpvo_residual_sum16(const void* net32, const void* u, int u_dtype
   DPVO_REQUIRE(rows >= 0 && dim > 0 && dim % 4 == 0, "residual_sum16: bad sizes");
   if (rows == 0) return DPVO_OK;
   DPVO_REQUIRE(net32 && u && net16 && ok_dt(u_dtype), "residual_sum16: bad argument");
-  residual_add_kernel<<<row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream>>>((float*)const_cast<void*>(net32), u, u_dtype, group_of, (__half*)net16, rows, dim, false);
-  DPVO_LAUNCH_CHECK("residual_add_kernel");
-  return DPVO_OK;
+  return launch("residual_add_kernel", residual_add_kernel, row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream, (float*)const_cast<void*>(net32),
+                u, u_dtype, group_of, (__half*)net16, rows, dim, false);
 }
 
 extern "C" int dpvo_gated_residual(const void* x32, const void* gate16, const void* res16, void* y32, void* y16_relu,
@@ -628,10 +614,8 @@ extern "C" int dpvo_gated_residual(const void* x32, const void* gate16, const vo
   DPVO_REQUIRE(rows >= 0 && dim > 0 && dim % 4 == 0, "gated_residual: bad sizes");
   if (rows == 0) return DPVO_OK;
   DPVO_REQUIRE(x32 && gate16 && res16 && y32, "gated_residual: null pointer");
-  gated_residual_kernel<<<row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      (const float*)x32, (const __half*)gate16, (const __half*)res16, (float*)y32, (__half*)y16_relu, rows, dim);
-  DPVO_LAUNCH_CHECK("gated_residual_kernel");
-  return DPVO_OK;
+  return launch("gated_residual_kernel", gated_residual_kernel, row_grid(rows), ROW_WARPS * 32, 0, (cudaStream_t)stream,
+                (const float*)x32, (const __half*)gate16, (const __half*)res16, (float*)y32, (__half*)y16_relu, rows, dim);
 }
 
 extern "C" int dpvo_softagg_reduce(const void* f16, const void* g16, int64_t ld, const int32_t* order, const int32_t* group_start,
@@ -643,10 +627,8 @@ extern "C" int dpvo_softagg_reduce(const void* f16, const void* g16, int64_t ld,
   const unsigned grid = (unsigned)std::min<int64_t>(max_groups, (int64_t)sm_count() * 8);
   const int pairs = std::min(SA_MAXPAIRS, std::max(32, ((dim / 2 + 31) / 32) * 32));
   const int threads = pairs * SA_SPLIT;
-  softagg_reduce_kernel<<<grid, threads, 0, (cudaStream_t)stream>>>((const __half*)f16, (const __half*)g16, ld, order, group_start,
-                                                                   n_groups, (__half*)y16, dim, (int)max_groups);
-  DPVO_LAUNCH_CHECK("softagg_reduce_kernel");
-  return DPVO_OK;
+  return launch("softagg_reduce_kernel", softagg_reduce_kernel, grid, threads, 0, (cudaStream_t)stream, (const __half*)f16, (const __half*)g16, ld,
+                order, group_start, n_groups, (__half*)y16, dim, (int)max_groups);
 }
 
 extern "C" int dpvo_update_heads(void* net32, const void* gate16, int64_t ld_gate, const void* res16, int64_t ld_res,
@@ -660,13 +642,7 @@ extern "C" int dpvo_update_heads(void* net32, const void* gate16, int64_t ld_gat
                "update_heads: gate / res rows must be aligned to 4 elements");
   const unsigned grid = row_grid((rows + 1) / 2);
   const int PP = P * P, centre = (P / 2) * P + P / 2;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dim / 128) {
-    case 1: heads_kernel<1><<<grid, ROW_WARPS * 32, 0, st>>>((float*)net32, (const __half*)gate16, ld_gate, (const __half*)res16, ld_res, W4, b4, coords, PP, centre, delta, weight, rows, dim); break;
-    case 2: heads_kernel<2><<<grid, ROW_WARPS * 32, 0, st>>>((float*)net32, (const __half*)gate16, ld_gate, (const __half*)res16, ld_res, W4, b4, coords, PP, centre, delta, weight, rows, dim); break;
-    case 3: heads_kernel<3><<<grid, ROW_WARPS * 32, 0, st>>>((float*)net32, (const __half*)gate16, ld_gate, (const __half*)res16, ld_res, W4, b4, coords, PP, centre, delta, weight, rows, dim); break;
-    default: heads_kernel<4><<<grid, ROW_WARPS * 32, 0, st>>>((float*)net32, (const __half*)gate16, ld_gate, (const __half*)res16, ld_res, W4, b4, coords, PP, centre, delta, weight, rows, dim); break;
-  }
-  DPVO_LAUNCH_CHECK("heads_kernel");
-  return DPVO_OK;
+  decltype(&heads_kernel<1>) const kern[] = {heads_kernel<1>, heads_kernel<2>, heads_kernel<3>, heads_kernel<4>};
+  return launch("heads_kernel", kern[dim / 128 - 1], grid, ROW_WARPS * 32, 0, (cudaStream_t)stream, (float*)net32, (const __half*)gate16, ld_gate,
+                (const __half*)res16, ld_res, W4, b4, coords, PP, centre, delta, weight, rows, dim);
 }
