@@ -54,3 +54,17 @@ def extensions():
         if not os.path.abspath(m.__file__).startswith(EXT_DIR):
             raise ImportError("dpvo_b200: module %s resolved to %s, not the in-tree build" % (m.__name__, m.__file__))
     return cuda_corr, cuda_ba, lietorch_backends, dpvo_b200_ext
+
+
+def camera_extension():
+    """Import and return dpvo_b200_camera, the torch shim of the camera-image preparation (csrc/undistort.cu).  It is a
+    fifth module of the same shim object, under the same tensor contract; the four modules of extensions() keep the
+    entry points that the per-argument contract table of tests/test_shim_args_gpu.py lists."""
+    extensions()
+    try:
+        import dpvo_b200_camera
+    except ImportError as e:  # pragma: no cover
+        raise ImportError("dpvo_b200: the camera shim is missing or stale (%s) -- run `python -m dpvo_b200.build`" % e)
+    if not os.path.abspath(dpvo_b200_camera.__file__).startswith(EXT_DIR):
+        raise ImportError("dpvo_b200: module dpvo_b200_camera resolved to %s, not the in-tree build" % dpvo_b200_camera.__file__)
+    return dpvo_b200_camera

@@ -5,8 +5,8 @@
 
 Products (git-ignored):
     dpvo_b200/lib/libdpvo_b200.so                  C-ABI library (nvcc, no torch dependency)
-    dpvo_b200/_ext/{cuda_corr,cuda_ba,lietorch_backends,dpvo_b200_ext}<EXT_SUFFIX>
-                                                   pybind shims, one object copied four times
+    dpvo_b200/_ext/{cuda_corr,cuda_ba,lietorch_backends,dpvo_b200_ext,dpvo_b200_camera}<EXT_SUFFIX>
+                                                   pybind shims, one object copied five times
 nvcc cross-compiles for sm_90a without a GPU, so this also is the CPU-side "does it build" check.
 """
 import os
@@ -23,8 +23,8 @@ EXTDIR = os.path.join(ROOT, "_ext")
 OBJDIR = os.path.join(os.path.dirname(ROOT), "build", "obj")
 INCLUDE = os.path.join(os.path.dirname(ROOT), "include")
 
-CU_SOURCES = ["common.cu", "chain.cu", "corr.cu", "corr_bin.cu", "corr_tc.cu", "patchify.cu", "lie.cu", "graph.cu", "pgraph.cu", "loop.cu", "keyframe.cu", "ba.cu", "ba_wide.cu", "update_ops.cu", "gemm.cu", "softagg.cu", "encoder.cu", "map.cu"]
-SHIM_MODULES = ["cuda_corr", "cuda_ba", "lietorch_backends", "dpvo_b200_ext"]
+CU_SOURCES = ["common.cu", "chain.cu", "corr.cu", "corr_bin.cu", "corr_tc.cu", "patchify.cu", "lie.cu", "graph.cu", "pgraph.cu", "loop.cu", "keyframe.cu", "ba.cu", "ba_wide.cu", "update_ops.cu", "gemm.cu", "softagg.cu", "encoder.cu", "map.cu", "undistort.cu"]
+SHIM_MODULES = ["cuda_corr", "cuda_ba", "lietorch_backends", "dpvo_b200_ext", "dpvo_b200_camera"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",

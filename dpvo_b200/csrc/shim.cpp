@@ -1,11 +1,12 @@
 // Torch-extension shims over the C-ABI of include/dpvo_b200.h.
 //
-// One translation unit defines four Python modules; the build copies the resulting shared object
-// to cuda_corr*.so, cuda_ba*.so, lietorch_backends*.so and dpvo_b200_ext*.so:
+// One translation unit defines five Python modules; the build copies the resulting shared object
+// to cuda_corr*.so, cuda_ba*.so, lietorch_backends*.so, dpvo_b200_ext*.so and dpvo_b200_camera*.so:
 //   cuda_corr          same pybind surface as dpvo/altcorr/correlation.cpp:57-62
 //   cuda_ba            same as dpvo/fastba/ba.cpp:183-188
 //   lietorch_backends  same as dpvo/lietorch/src/lietorch.cpp:286-316
 //   dpvo_b200_ext      the fused entry points that have no counterpart in the reference
+//   dpvo_b200_camera   the camera-image preparation in front of the encoders (undistort.cu)
 // The shims only adapt torch::Tensor -> (pointer, sizes, strides, current CUDA stream), allocate
 // outputs and raise RuntimeError on a non-zero status.  There is no CPU path: a CPU tensor is an
 // error, not a fallback.
@@ -1206,6 +1207,32 @@ int64_t encode_frames_workspace_bytes(int64_t B, int64_t H, int64_t W) {
   return dpvo_encode_frames_workspace_bytes((int)B, (int)H, (int)W);
 }
 
+// ------------------------------------------------------------------------------ camera-image preparation
+// images uint8 [B, 3, H, W] (any strides) -> the window rows [y0, y0 + Ho) x columns [x0, x0 + Wo) of each undistorted
+// (and, with half, halved) image, into out uint8 [B, Ho, Wo, 3] (any strides).  cameras: B rows of 9 float64 values
+// (fx fy cx cy k1 k2 p1 p2 k3), passed by value.  The library checks the values and the window.
+void undistort_frames(Tensor images, std::vector<double> cameras, bool half, int64_t y0, int64_t x0, Tensor out) {
+  const Args arg("dpvo_b200_ext.undistort_frames", images, "images");
+  const c10::cuda::CUDAGuard guard(arg.dev);
+  arg.on(images, "images", at::kByte); arg.on(out, "out", at::kByte);
+  TORCH_CHECK(images.dim() == 4 && images.size(1) == 3, "undistort_frames: images must be uint8 [B, 3, H, W]");
+  const int64_t B = images.size(0);
+  TORCH_CHECK(out.dim() == 4 && out.size(0) == B && out.size(3) == 3, "undistort_frames: out must be uint8 [B, Ho, Wo, 3] with B = ", B);
+  TORCH_CHECK((int64_t)cameras.size() == 9 * B, "undistort_frames: 9 camera values (fx fy cx cy k1 k2 p1 p2 k3) per image, ", B,
+              " images, ", cameras.size(), " values");
+  TORCH_CHECK(images.size(2) <= INT32_MAX && images.size(3) <= INT32_MAX && out.size(1) <= INT32_MAX && out.size(2) <= INT32_MAX &&
+              y0 >= INT32_MIN && y0 <= INT32_MAX && x0 >= INT32_MIN && x0 <= INT32_MAX, "undistort_frames: sizes beyond 32-bit");
+  std::vector<dpvo_camera> cams((size_t)B);
+  for (int64_t b = 0; b < B; ++b) {
+    const double* c = cameras.data() + 9 * b;
+    cams[b] = dpvo_camera{c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7], c[8]};
+  }
+  check(dpvo_undistort_frames(images.data_ptr<uint8_t>(), images.stride(0), images.stride(1), images.stride(2), images.stride(3), (int)B,
+                              (int)images.size(2), (int)images.size(3), cams.data(), half ? 1 : 0, (int)y0, (int)x0, (int)out.size(1),
+                              (int)out.size(2), out.data_ptr<uint8_t>(), out.stride(0), out.stride(1), out.stride(2), out.stride(3), stream()),
+        "dpvo_b200_ext.undistort_frames");
+}
+
 // ------------------------------------------------------------------------------ map
 // points [B F M, 3] rows [b F M, b F M + n[b] M) of every stream b = 0 .. len(n) - 1, from poses [B F, 7], patches
 // [B F M, 3, 3, 3] and intrinsics [B F, 4]
@@ -1337,4 +1364,9 @@ PYBIND11_MODULE(dpvo_b200_ext, m) {
   m.def("encode_frames_workspace_bytes", &encode_frames_workspace_bytes, "scratch bytes of encode_frames for B H x W images");
   m.def("launch_count", &launch_count, "kernel launches issued by libdpvo_b200 so far");
   m.def("version", &version, "library version string");
+}
+
+PYBIND11_MODULE(dpvo_b200_camera, m) {
+  m.def("undistort_frames", &undistort_frames, "cv2.undistort (+ half-size INTER_AREA resize) and a crop window of B uint8 images",
+        py::arg("images"), py::arg("cameras"), py::arg("half"), py::arg("y0"), py::arg("x0"), py::arg("out"));
 }

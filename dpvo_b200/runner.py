@@ -13,6 +13,7 @@ from . import extensions
 from . import altcorr, fastba
 from . import projective_ops as pops
 from .net import Update, EdgeGroups, DIM
+from .camera import undistort_frames
 from .frontend import encoder_output_size
 from .streams import StreamBatch
 from .synthetic import check_map
@@ -271,18 +272,38 @@ class UpdateRunner:
         s.poses[s.n - 1].copy_(hf["pose"], non_blocking=True)
         return sum(v.numel() * v.element_size() for v in hf.values())
 
+    def _prepare(self, images, cameras):
+        """the raw images [B', 3, H, W] prepared by their cameras (camera.undistort_frames) into a buffer the runner
+        keeps, as [B', 3, h, w] views of HWC storage.  The buffer grows and is kept, like the encoder workspace, so a call
+        with coords and depth given can be captured (a graph captured before a call that grows it must be captured
+        again)."""
+        h, w = cameras[0].size
+        nb = len(cameras) * h * w * 3
+        buf = getattr(self, "_prepared", None)
+        if buf is None or buf.numel() < nb or buf.device != images.device:
+            self._prepared = buf = torch.empty(nb, dtype=torch.uint8, device=images.device)
+        out = buf[:nb].view(len(cameras), h, w, 3)
+        return undistort_frames(images, cameras, out).permute(0, 3, 1, 2)
+
     @torch.no_grad()
-    def ingest_image(self, image, depth=None, coords=None, stream=None):
+    def ingest_image(self, image, depth=None, coords=None, stream=None, camera=None):
         """Encode a uint8 camera image [3, H, W] (CHW or HWC strides) straight into the slots `ingest_frame` writes:
         fmap1 / fmap2 slot (n-1) % mem, gmap / imap slot (n-1) % pmem, patches[(n-1) M : n M] (dpvo.py:389-438), and
         colors[n-1] (dpvo.py:404) when the state has map buffers.
         Centroids are drawn as Patchifier.forward draws them, unless `coords` [M, 2] is given (CUDA-graph capture);
         the patch depths are then one torch.rand draw (dpvo.py:427), or `depth` (the median the caller computes once
         initialised, dpvo.py:429-431).  Poses, intrinsics and the motion model stay with the caller.  In a batch,
-        `stream` names the stream whose slots (at its own n) receive the frame.  Returns the centroids."""
+        `stream` names the stream whose slots (at its own n) receive the frame.  Returns the centroids.
+        With a `camera` (camera.Camera), `image` is the raw camera image: it is first prepared on the device
+        (undistorted, halved if the camera says so, cropped) and the prepared image is encoded, centroids and colours
+        included; intrinsics[n-1] is then set to camera.intrinsics / 4 (dpvo.py:401)."""
         if self.encoder is None:
             raise RuntimeError("ingest_image: this UpdateRunner was built without an encoder")
         s, M = self._stream_state(stream, "ingest_image"), self.M
+        if camera is not None:
+            if not isinstance(image, torch.Tensor) or image.dim() != 3:
+                raise RuntimeError("ingest_image: the raw image must be a uint8 tensor [3, H, W]")
+            image = self._prepare(image[None], [camera])[0]
         h, w = s.fmap1.shape[3], s.fmap1.shape[4]
         if image.dim() != 3 or encoder_output_size(image.shape[1], image.shape[2]) != (h, w):
             raise RuntimeError("ingest_image: a %s image encodes to %s features, the rings hold %dx%d"
@@ -298,17 +319,22 @@ class UpdateRunner:
         if depth is None:
             depth = torch.rand(M, 1, 1, device=patches.device, dtype=patches.dtype)
         patches[:, 2] = depth
+        if camera is not None:
+            s.intrinsics.view(-1, 4)[s.n - 1].copy_(camera.ring_intrinsics(patches.device))
         return coords
 
     @torch.no_grad()
-    def ingest_images(self, images, depth=None, coords=None, streams=None):
+    def ingest_images(self, images, depth=None, coords=None, streams=None, cameras=None):
         """Encode the images of several streams of a batch in one pass of the encoders: uint8 [B', 3, H, W] (or the
         permuted [B', H, W, 3] view), image i into stream streams[i]'s slots at that stream's own n -- the slots
         `ingest_image(images[i], stream=streams[i])` writes, with the same bytes.  `streams` lists B' distinct streams
         (default: all B, in order), so a rig where a camera dropped a frame passes the others.
         Without `coords` [B', M, 2] and `depth` (fp32, broadcastable to [B', M]) the CUDA generator is drawn as those
         ingest_image calls draw it, image by image: centroid x, centroid y, then the depths.  With both given nothing
-        is drawn and the call can be captured in a CUDA graph.  Returns the centroids [B', M, 2]."""
+        is drawn and the call can be captured in a CUDA graph.  Returns the centroids [B', M, 2].
+        With `cameras` (B' camera.Camera sharing raw size, half and crop), the images are raw camera images: one launch
+        prepares all of them, the prepared images are encoded, and each stream's intrinsics[n-1] is set to its camera's
+        intrinsics / 4 -- what `ingest_image(images[i], stream=streams[i], camera=cameras[i])` does."""
         if self.batch is None:
             raise RuntimeError("ingest_images: this UpdateRunner holds one stream; use ingest_image")
         if self.encoder is None:
@@ -327,6 +353,11 @@ class UpdateRunner:
         bad = [b for b in streams if not 0 <= b < batch.B]
         if bad:
             raise RuntimeError("ingest_images: streams %s outside the batch of %d" % (bad, batch.B))
+        if cameras is not None:
+            cameras = list(cameras)
+            if len(cameras) != n:
+                raise RuntimeError("ingest_images: %d cameras for %d images" % (len(cameras), n))
+            images = self._prepare(images, cameras)
         h, w = batch.fmap1.shape[3], batch.fmap1.shape[4]
         if encoder_output_size(images.shape[2], images.shape[3]) != (h, w):
             raise RuntimeError("ingest_images: a %s image encodes to %s features, the rings hold %dx%d"
@@ -346,10 +377,16 @@ class UpdateRunner:
             depth = torch.stack(drawn_d).view(n, M) if depth is None else depth
         depth = torch.broadcast_to(torch.as_tensor(depth, device=dev, dtype=torch.float32), (n, M)).contiguous()
         rows = [batch.frame_rows(b) for b in streams]
-        return self.encoder.encode_frames_into(images, M, self.encoder.strategy, batch.fmap1[0].permute(0, 2, 3, 1),
-                                               batch.fmap2[0].permute(0, 2, 3, 1), batch.gmap[0].permute(0, 2, 3, 1),
-                                               batch.imap[0], batch.patches, [r[0] for r in rows], [r[1] for r in rows],
-                                               [r[2] for r in rows], coords=coords, depth=depth, colors_ring=getattr(batch, "colors", None))
+        coords = self.encoder.encode_frames_into(images, M, self.encoder.strategy, batch.fmap1[0].permute(0, 2, 3, 1),
+                                                 batch.fmap2[0].permute(0, 2, 3, 1), batch.gmap[0].permute(0, 2, 3, 1),
+                                                 batch.imap[0], batch.patches, [r[0] for r in rows], [r[1] for r in rows],
+                                                 [r[2] for r in rows], coords=coords, depth=depth,
+                                                 colors_ring=getattr(batch, "colors", None))
+        if cameras is not None:
+            for b, cam in zip(streams, cameras):
+                s = batch.stream(b)
+                s.intrinsics[s.n - 1].copy_(cam.ring_intrinsics(dev))
+        return coords
 
     # A streaming front end has frame t+1 in pinned memory while update t runs: its H2D copy goes to a staging
     # buffer on a copy stream (overlapping the update), and only the short device-to-device move into the ring

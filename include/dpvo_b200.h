@@ -720,6 +720,30 @@ int dpvo_encode_frames_colors(const uint8_t* images, int64_t s_b, int64_t s_c, i
                               const int64_t* frame_row, const int64_t* feat_row, const int64_t* patch_row,
                               const float* depth, uint8_t* colors, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- Camera-image preparation (dpvo_b200/csrc/undistort.cu) ---------------------------------------------------------
+ * dpvo_undistort_frames: the image preparation of the reference's readers (dpvo/stream.py:image_stream / video_stream,
+ * evaluate_tum.py:tum_image_stream) for B (1..64) uint8 images of one raw size H x W in one launch:
+ *   cv2.undistort(image, K, (k1, k2, p1, p2, k3)), then, with half, cv2.resize(fx = fy = 0.5, INTER_AREA), then the
+ *   crop window rows [y0, y0 + Ho) x columns [x0, x0 + Wo) of the (halved) image.
+ * Image b is [3, H, W] at images + b s_b with element strides s_c, s_y, s_x (a stacked [B, 3, H, W] tensor or its
+ * permuted [B, H, W, 3] view); its window goes to out + b o_sb, element strides o_sy, o_sx, o_sc (e.g. [B, Ho, Wo, 3]).
+ * Channels are processed alike (BGR stays BGR).  Image b is undistorted with cameras[b] (host array, passed by value:
+ * a captured graph keeps it).  The arithmetic is OpenCV's exact integer specification (DESIGN §3.8): the float64
+ * map rounded to 1/32 pixel, the fixed-point bilinear with 2^15 weight sums and zeros outside the image, the 2 x 2
+ * average (sum + 2) >> 2.  A camera without coefficients maps every pixel onto itself (crop, and halve if asked).
+ * Rejected (DPVO_ERR_INVALID): B outside 1..64, a non-finite or non-positive focal length, a non-finite principal point
+ * or coefficient, halving an odd-sized image, a window outside the (halved) image, an empty window.
+ * No workspace, no atomics, no host synchronisation (graph-capturable).
+ */
+typedef struct dpvo_camera {
+  double fx, fy, cx, cy;           /* pinhole intrinsics of the raw image, pixels */
+  double k1, k2, p1, p2, k3;       /* OpenCV's radial (k1, k2, k3) and tangential (p1, p2) coefficients */
+} dpvo_camera;
+
+int dpvo_undistort_frames(const uint8_t* images, int64_t s_b, int64_t s_c, int64_t s_y, int64_t s_x, int B, int H, int W,
+                          const dpvo_camera* cameras, int half, int y0, int x0, int Ho, int Wo, uint8_t* out,
+                          int64_t o_sb, int64_t o_sy, int64_t o_sx, int64_t o_sc, void* stream);
+
 /* ---- Map (dpvo_b200/csrc/map.cu) --------------------------------------------------------------------------------------
  * dpvo_point_cloud: the points of DPVO.update (dpvo.py:358-360) for B (1..64) streams of F frame slots and M patches per
  * frame.  Stream b's frames are [b F, (b + 1) F) of poses fp32 [B F, 7] and intrinsics fp32 [B F, 4], its patches
